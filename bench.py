@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- disvae training hot path on B200 (contract: see the task statement / DESIGN.md section 6).
+"""bench.py -- disvae training hot path on H100 (DESIGN.md section 6).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|reference-cuda]
-                  [--workload c1..c5] [--scaling weak|strong]
+                  [--workload c1..c5] [--scaling weak|strong] [--dump-outputs DIR]
 
 One "step" = one full optimisation step (forward, loss, backward, gradient all-reduce for N>1, Adam) over one
 synthetic batch.  Default workload at every N: BASELINE.json configs[1] (btcvae, 1x64x64, batch 1024 PER GPU, z=10,
@@ -16,11 +16,12 @@ bernoulli, MSS, Adam lr 5e-4) -- weak scaling.  `--scaling strong` divides the c
   ddp_parity (N>1): rank r's loss == oracle on shard r, rank-averaged gradients == mean of the oracle's shard gradients
   roofline / roofline_logdensity / cpu_baseline / cuda_eager_baseline / clocks / gpu_launches : DESIGN.md section 6
 
---impl reference      : the UNMODIFIED reference (baseline/_ref, shipped by scripts/ship_reference.py) through its own
+--impl reference      : the UNMODIFIED reference (oracle/_ref, shipped by oracle/ship_reference.py) through its own
                         Trainer._train_iteration on the host cores (kind "reference"); the oracle port if the copy is
                         not there (kind "port").
 --impl reference-cuda : the same unmodified reference with device=cuda (stock PyTorch eager: cuDNN/cuBLAS, TF32 off) --
-                        the "existing Blackwell kernels" bar of SURVEY.md 8d.
+                        the stock-PyTorch bar of SURVEY.md 8d.
+--dump-outputs DIR    : write the last timed step's loss and updated parameters as DIR/<name>.npy (seeded inputs).
 """
 import argparse
 import json
@@ -50,7 +51,7 @@ WORKLOAD_NAMES = {"c1": "BASELINE.json configs[0]: VAE mnist-shape", "c2": "BASE
                   "c5": "BASELINE.json configs[4]: btcvae celeba-shape z=64"}
 # algorithmic work per image, forward + backward (SURVEY.md 8d): conv FLOPs
 CONV_FLOP_PER_IMG = {(1, 64, 64): 71.30e6, (3, 64, 64): 81.79e6, (1, 32, 32): 17.04e6}
-N_ROTATE = 8            # distinct batches cycled through (8 x 16.8 MB > 126 MB L2)
+N_ROTATE = 8            # distinct batches cycled through (8 x 16.8 MB > 50 MB L2)
 
 
 def loss_kwargs(workload, device):
@@ -87,7 +88,7 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, src="fallback")
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, src="H100 SXM data sheet (700 W)")
 
 
 class ClockSampler:
@@ -175,7 +176,7 @@ def run_ours(args):
     sys.path.insert(0, PKG)
     from disvae import _native
     L = _native.lib()
-    assert L.dv_device_check() == 0, "not an sm_100 device"
+    assert L.dv_device_check() == 0, "not an sm_90 (H100) device"
 
     loss_name, img, _, z, n_data, lkw, lr, _ = WORKLOADS[args.workload]
     B = per_gpu_batch(args, world)
@@ -203,7 +204,11 @@ def run_ours(args):
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return ms.item()
 
-    step_res = lambda i: trainer._step(resident[i % N_ROTATE], None)            # noqa: E731
+    last = {}
+
+    def step_res(i):
+        last["loss"] = trainer._step(resident[i % N_ROTATE], None)
+
     # end to end: the Trainer's epoch loop over a loader of PINNED HOST batches (H2D of every batch on the Trainer's
     # copy stream one step ahead, async D2H of every step's loss, one blocking read of the epoch mean at the end) with a
     # real storer, so the steps that log scalars (every 50th, losses.py:105-114) run their eager + host-sync path
@@ -219,6 +224,8 @@ def run_ours(args):
     ms = timed(step_res, K)
     launches = _native.launch_count() - l0
     clocks = clk.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, trainer, last["loss"])
     # untimed warm-up of the end-to-end path: three loader steps, and one EAGER step -- torch.cuda.graph empties the
     # caching allocator when it captures, so the first eager step afterwards (the every-50th logging step of a real
     # run) would otherwise pay ~2 GB of cudaMalloc inside the timed epoch, once
@@ -286,6 +293,19 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, trainer, loss):
+    """The timed step's loss and every parameter its optimiser step wrote (model, FactorVAE discriminator)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().double().cpu().numpy().reshape(1))
+    nets = [("model", trainer.model)]
+    if getattr(trainer.loss_f, "discriminator", None) is not None:
+        nets.append(("discriminator", trainer.loss_f.discriminator))
+    for prefix, net in nets:
+        for k, p in net.named_parameters():
+            np.save(os.path.join(out_dir, "%s.%s.npy" % (prefix, k)), p.detach().float().cpu().numpy())
+
+
 def sub_arm(impl, args, steps, warmup, key=None):
     """Run another arm of this script in a child process (the reference's `disvae` package cannot share a process with
     ours: same module name) and return its JSON line (or `key` of it)."""
@@ -342,9 +362,6 @@ def kernel_rooflines(trainer, resident, K, B, img, z, n_data, device, detail=Fal
            "profiled_call_ms_per_step": round(total / K, 4),
            "profiled_calls_per_step": sum(n for _, n in table.values()) // K}
     traffic_table = {}
-    tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tp):                                          # dram__bytes_read+write of one launch (ncu --set full)
-        traffic_table = json.load(open(tp))
     conv = [(k, v) for k, v in top if k.startswith("dv_conv_") and "[" in k]
     name, (tms, calls) = conv[0] if conv else top[0]
     if conv:
@@ -365,7 +382,7 @@ def kernel_rooflines(trainer, resident, K, B, img, z, n_data, device, detail=Fal
                            "hbm_frac": round(alg_bytes / (per_call_ms / 1e3) / 1e9 / pk["hbm"], 4),
                            "us_per_launch": round(per_call_ms * 1e3, 2), "launches_per_step": calls // K,
                            "peak_source": pk["src"] + " bf16 sustained (kernel timed inside a long step)",
-                           "note": "tcgen05 kind::tf32, error-compensated 3xTF32 (three tensor passes per algorithmic "
+                           "note": "mma.sync m16n8k8 tf32, error-compensated 3xTF32 (three tensor passes per algorithmic "
                                    "product; FLOPs counted once); time = CUDA events around the C-ABI call on its stream"}
         if CH != 32:
             # image-boundary layer (K = 16*CH): a streaming problem on the CUDA cores (dv_conv_img.cu), bounded by HBM
@@ -582,7 +599,7 @@ def oracle_job(workload, batch):
 
 def reference_job(workload, batch, device):
     """The unmodified reference's own training step: disvae.Trainer._train_iteration (training.py:137-164) of
-    baseline/_ref.  None if the copy is not there."""
+    oracle/_ref.  None if the copy is not there."""
     from oracle import reference_env
     ref = reference_env.find_reference()
     if ref is None:
@@ -664,7 +681,7 @@ def run_reference(args):
         step()
     dt = time.perf_counter() - t0
     v = round(Bs * args.steps / dt, 1)
-    what = ("unmodified reference (baseline/_ref) disvae.Trainer._train_iteration on CPU" if kind == "reference"
+    what = ("unmodified reference (oracle/_ref) disvae.Trainer._train_iteration on CPU" if kind == "reference"
             else "oracle port (oracle/disvae_oracle.py) on CPU")
     out = {"impl": "reference", "metric": "images/sec", "value": v, "unit": "img/s", "n_gpus": world, "steps": args.steps,
            "warmup": args.warmup, "ms_per_step": round(dt / args.steps * 1e3, 3), "higher_is_better": True,
@@ -678,8 +695,8 @@ def run_reference(args):
 
 
 def run_reference_cuda(args):
-    """The unmodified reference on the B200 through stock PyTorch eager (cuDNN / cuBLAS), TF32 disabled so that it
-    computes in the same fp32 as the CPU path -- SURVEY.md 8d's "existing Blackwell kernels" bar."""
+    """The unmodified reference on the GPU through stock PyTorch eager (cuDNN / cuBLAS), TF32 disabled so that it
+    computes in the same fp32 as the CPU path -- SURVEY.md 8d's stock-PyTorch bar."""
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if rank != 0:
@@ -695,7 +712,7 @@ def run_reference_cuda(args):
     B = per_gpu_batch(args, world)
     step = reference_job(args.workload, B, device)
     if step is None:
-        print(json.dumps({"impl": "reference-cuda", "unavailable": "baseline/_ref not shipped"}), flush=True)
+        print(json.dumps({"impl": "reference-cuda", "unavailable": "oracle/_ref not shipped"}), flush=True)
         return
     for _ in range(max(args.warmup, 3)):
         step()
@@ -712,7 +729,7 @@ def run_reference_cuda(args):
            "warmup": max(args.warmup, 3), "ms_per_step": round(ms / args.steps, 4), "higher_is_better": True,
            "scaling": args.scaling, "vs_baseline": None, "dtype": "f32", "data": "synthetic (torch.rand); random-init weights",
            "config": config_block(args, 1, B),
-           "what": "unmodified reference (baseline/_ref) disvae.Trainer._train_iteration, device=cuda, stock PyTorch %s eager "
+           "what": "unmodified reference (oracle/_ref) disvae.Trainer._train_iteration, device=cuda, stock PyTorch %s eager "
                    "(cuDNN %s), allow_tf32=False, cudnn.benchmark=True, batches resident" % (
                        torch.__version__, torch.backends.cudnn.version())}
     print(json.dumps(out), flush=True)
@@ -731,6 +748,8 @@ def main():
     ap.add_argument("--no-eager-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--detail", action="store_true", help="per-entry-point table on stderr")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss and updated parameters as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

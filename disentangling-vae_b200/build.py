@@ -1,4 +1,4 @@
-"""Builds libdisvae_b200.so in-tree with nvcc for sm_100a (no JIT cache, no torch extension:
+"""Builds libdisvae_b200.so in-tree with nvcc for sm_90a (H100) (no JIT cache, no torch extension:
 the library is a plain C-ABI shared object, see include/disvae_b200.h).
 
     python disentangling-vae_b200/build.py [--force] [--verbose]
@@ -15,9 +15,10 @@ INCLUDE = os.path.join(ROOT, "include")
 LIB = os.path.join(HERE, "libdisvae_b200.so")
 STAMP = os.path.join(HERE, ".libdisvae_b200.stamp")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
-              "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v",
-              "-I", INCLUDE, "-I", CSRC]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
+                     "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v",
+                     "-I", INCLUDE, "-I", CSRC]
 
 
 def sources():
@@ -61,7 +62,7 @@ def build(force=False, verbose=False):
         if p.returncode != 0:
             sys.stderr.write("\n".join(log))
             raise RuntimeError("nvcc failed on %s" % src)
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs + ["-lcudart"]
+    link = [nvcc, "-shared"] + ARCH + ["-o", LIB] + objs + ["-lcudart"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     log.append("==== link\n" + r.stdout)
     if r.returncode != 0:

@@ -9,7 +9,7 @@ long long g_launches = 0;
 extern "C" {
 
 int dv_version(void) { return 100; }            // 0.1.0
-int dv_built_arch(void) { return 100; }
+int dv_built_arch(void) { return 90; }
 
 const char* dv_status_string(int status) {
   switch (status) {
@@ -18,7 +18,7 @@ const char* dv_status_string(int status) {
     case DV_ERR_BAD_ARG: return "bad argument";
     case DV_ERR_WORKSPACE: return "workspace too small";
     case DV_ERR_CUDA: return "CUDA runtime error";
-    case DV_ERR_ARCH: return "device is not sm_100";
+    case DV_ERR_ARCH: return "device is not sm_90";
     default: return "unknown status";
   }
 }
@@ -32,7 +32,7 @@ int dv_device_check(void) {
     dv::g_last_cuda_error = (int)cudaGetLastError();
     return DV_ERR_CUDA;
   }
-  return (prop.major == 10) ? DV_OK : DV_ERR_ARCH;
+  return (prop.major == 9 && prop.minor == 0) ? DV_OK : DV_ERR_ARCH;
 }
 
 long long dv_launch_count(void) { return dv::g_launches; }

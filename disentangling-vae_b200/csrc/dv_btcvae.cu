@@ -84,7 +84,7 @@ __device__ __forceinline__ void lse_merge2(float& m, float& s, float m2, float s
 // the ranges in a fixed order, forms the row statistics and the three means.  Grid: (B/32) x (B/kJT).
 // ------------------------------------------------------------------------------------------
 // JT = columns per block: 64 (8 per lane), or 16 (2 per lane) when (rows/32) x (B/64) blocks would leave most SMs idle
-// (B = 256: 32 blocks -> 128; the z = 64 shard of BASELINE configs[4] went from 55 us to the low tens).
+// (B = 256: 32 blocks -> 128).
 constexpr int kJTBig = 64, kJTSmall = 16;
 constexpr int kRG = 32;            // rows per block
 
@@ -256,7 +256,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
 
 // ------------------------------------------------------------------------------------------
 // Forward, version 4 (D <= 16): ONE launch, thread-block CLUSTERS of 4.
-// What held version 3 at 24 us: every CTA staged the parameters of ALL B columns (148 x 176 KB = 26 MB of L2->smem
+// What limits version 3: every CTA stages the parameters of ALL B columns (176 KB per CTA of L2->smem
 // traffic, 176 KB smem CTAs) and every lane of a warp read a different column (LDS.128 with 32 distinct addresses =
 // 4 shared-memory wavefronts per 32 evaluations: the sweep was shared-memory-bandwidth bound).  Here
 //   * a cluster of 4 CTAs owns R rows; CTA c of the cluster stages only ITS QUARTER of the columns (40 KB at
@@ -266,7 +266,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
 //   * register blocking over ROWS: a lane owns columns (conflict-free LDS.128, odd float4 pitch) and applies each loaded
 //     column to RPT = 4 rows whose z_d and running sums it keeps in registers -- 4x less shared-memory traffic per
 //     evaluation (an LDS.128 is four shared-memory cycles whatever the addresses: broadcasting ACROSS lanes, the first
-//     attempt, bought nothing and its even pitch cost 2-way conflicts: 11.7 us for the sweep);
+//     attempt, bought nothing and its even pitch cost 2-way conflicts);
 //   * the reference exponent is per CTA and per dimension (r_cd = max over the CTA's columns of c_jd + w_j, an
 //     upper bound of every term it sums), folded with the column weight into the staged constant as before
 //     (t = z - mu; arg = x'' - hiv*t*t; a += arg; s_d += ex2(arg)); partial sums of different CTAs are brought to
@@ -275,7 +275,8 @@ __device__ __forceinline__ float ex2_approx(float x) {
 //     the column bound) are redone exactly (two passes straight from global memory) by the finalising warp.
 // Rows of a cluster are finalised by its 4 CTAs round-robin (one warp per row: lanes = latent dims); the block's
 // contribution to the three means goes to `blockpart`, the last block adds them in block order (deterministic).
-// Cluster size 4 leaves 132 of the 148 SMs usable (GPC sizes 16/18/20): 32 clusters x 4 at B = 1024.
+// Clusters of 4 CTAs, rows spread over at most 32 of them (B = 1024: 32 rows per cluster).  32 is an estimate of how
+// many 4-CTA clusters a 132-SM H100 holds at once (not measured); more clusters only run as a second wave.
 // ------------------------------------------------------------------------------------------
 constexpr int kF4Threads = 512;
 constexpr int kF4Warps = kF4Threads / 32;
@@ -756,7 +757,7 @@ int dv_btcvae_fwd_rows(const float* z, const float* mu, const float* logvar, int
     // single-launch cluster path (D <= 16): columns split over the 4 CTAs of a cluster, rows over the clusters
     static const int v4 = env_switch("DV_BTCVAE_V4", 1);
     const int dc = D == 10 ? 10 : 16;
-    const int max_clusters = 33;                               // cluster size 4 packs 132 of the 148 SMs
+    const int max_clusters = 32;                               // estimated 4-CTA cluster capacity of a 132-SM H100 (see above)
     int R = ((B + max_clusters - 1) / max_clusters + kRows - 1) / kRows * kRows;
     const int NC = ((B + kF4Clus - 1) / kF4Clus + kJL - 1) / kJL * kJL;
     const size_t smem = (size_t)NC * (dc + 1) * sizeof(float4);

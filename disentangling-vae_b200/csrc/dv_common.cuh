@@ -1,12 +1,12 @@
-// Shared helpers for the disvae_b200 kernels (sm_100a only).
+// Shared helpers for the disvae_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
 #include "disvae_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "disvae_b200 kernels are written for sm_100a (Blackwell B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "disvae_b200 kernels are written for sm_90a (Hopper H100) only"
 #endif
 
 namespace dv {
@@ -14,7 +14,7 @@ namespace dv {
 constexpr int kWarp = 32;
 constexpr int kLoCh = 32;          // channels of every "lo" tensor (encoders.py:43, decoders.py:43)
 constexpr int kTaps = 16;          // 4x4 kernel
-constexpr int kNumSMs = 148;       // B200
+constexpr int kNumSMs = 132;       // H100 SXM
 
 extern thread_local int g_last_cuda_error;
 extern long long g_launches;
@@ -26,6 +26,23 @@ inline int check_launch() {
   return DV_OK;
 }
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
+
+// Opt a kernel in to `bytes` of dynamic shared memory, once per process (*done caches the success).
+template <typename Kernel>
+inline int set_max_dynamic_smem(Kernel kernel, int bytes, bool* done) {
+  if (*done) return DV_OK;
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess) {
+    g_last_cuda_error = (int)cudaGetLastError();
+    return DV_ERR_CUDA;
+  }
+  *done = true;
+  return DV_OK;
+}
+
+// First 1024-byte aligned address at or after p (TMA destinations with the 128-byte swizzle need it).
+__device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
+}
 
 // Environment toggles exist for A/B measurements only.  Each one is read ONCE per process through a C++11 local static
 // (`static const int v = env_switch(...)`: initialisation is thread-safe), so the entry points stay re-entrant.

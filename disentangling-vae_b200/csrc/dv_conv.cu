@@ -1,5 +1,5 @@
 // Convolution entry points (dv_conv_down / dv_conv_up / dv_conv_wgrad / packs) of the Burgess 4x4/stride-2/pad-1 layers:
-// the dispatch to the tcgen05 kernels (dv_conv_tc.cu, 32-channel layers) and to the exact-fp32 image-boundary kernels
+// the dispatch to the tensor-core kernels (dv_conv_tc.cu, 32-channel layers) and to the exact-fp32 image-boundary kernels
 // (dv_conv_img.cu, CH in {1,3}), the split-K / channel-sum reductions they share, and the generic FP32 CUDA-core kernels
 // below -- the fallback for every geometry the specialised kernels do not take (and the A/B reference: DV_CONV_IMPL=ffma).
 //
@@ -570,7 +570,7 @@ static int wgrad_nsplit(int B, int H, int W, long long* chunk) {
 }  // namespace dv
 
 namespace dv {
-namespace tc {        // dv_conv_tc.cu: tcgen05 kernels of the 32-channel layers
+namespace tc {        // dv_conv_tc.cu: tensor-core kernels of the 32-channel layers
 int pack_tc(const float* w, float* wd, float* wu, float* wf, cudaStream_t st);
 int pack_multi(int n, const float* const* w, float* const* wp, const int* CH, cudaStream_t st);
 int conv_down32_tc(const float* hi, const float* wd_packed, const float* bias, const float* mask, float* lo,
@@ -590,7 +590,7 @@ int conv_up(const float* lo, const float* wu, const float* bias, float* hi, int 
 }  // namespace img
 
 // packed-weight sections for CH == 32 (floats): [0,16K) ffma down, [16K,32K) ffma up,
-// [32K,64K) tcgen05 down (hi|lo), [64K,96K) tcgen05 up (hi|lo)
+// [32K,64K) tensor-core down (hi|lo), [64K,96K) tensor-core up (hi|lo)
 constexpr int kPackFfma = 2 * kLoCh * 32 * kTaps;
 constexpr int kPackTcSection = kTaps * 64 * 32;
 
@@ -623,7 +623,7 @@ int dv_conv_pack_weights(const float* w, float* w_packed, int CH, void* stream) 
   if (!w || !w_packed) return DV_ERR_BAD_ARG;
   if (CH != 1 && CH != 3 && CH != 32) return DV_ERR_BAD_SHAPE;
   const int n = kLoCh * CH * kTaps;
-  if (CH == 32)                                     // ONE launch: both tcgen05 operand layouts + the two CUDA-core layouts
+  if (CH == 32)                                     // ONE launch: both tensor-core operand layouts + the two CUDA-core layouts
     return tc::pack_tc(w, w_packed + kPackFfma, w_packed + kPackFfma + kPackTcSection, w_packed, as_stream(stream));
   conv_pack_kernel<<<(n + 255) / 256, 256, 0, as_stream(stream)>>>(w, w_packed, CH);
   return check_launch();
@@ -751,7 +751,7 @@ int dv_conv_up(const float* lo, const float* w_packed, const float* bias, const 
 size_t dv_conv_wgrad_workspace_bytes(int B, int H, int W, int CH) {
   long long chunk;
   int ns = wgrad_nsplit(B, H, W, &chunk);
-  if (ns < kNumSMs) ns = kNumSMs;                    // the tcgen05 path uses at most one CTA per SM
+  if (ns < kNumSMs) ns = kNumSMs;                    // the tensor-core path uses at most one CTA per SM
   return (size_t)ns * (kTaps * CH + 1) * kLoCh * sizeof(float);
 }
 

@@ -4,9 +4,8 @@
 //
 // With K = 16*CH these layers have ~1/30 of the arithmetic intensity of the 32->32 layers: 2*512*CH FLOP per lo
 // pixel against 128 B (lo) + 16*CH B (hi) of compulsory traffic, i.e. they are pure HBM streaming problems (151 MB per
-// launch at B = 1024, 1x64x64) whose whole arithmetic (1.07 GFLOP) fits in ~15 us of FP32 FMA issue.  The tcgen05
-// variants of round 1 (conv_*_small_tc_kernel, conv_up_c2i_kernel; deleted) paid for operand staging they could not
-// amortise (im2col gather by 4 builder warps, hi/lo splitting, three tensor passes) and ran at 15-22 % of HBM bandwidth;
+// launch at B = 1024, 1x64x64) whose whole arithmetic (1.07 GFLOP) is small next to that traffic.  Tensor-core
+// variants would pay for operand staging they cannot amortise (im2col gather, hi/lo splitting, three tensor passes);
 // these kernels do exact fp32 FMAs from shared-memory tiles with register blocking instead:
 //
 //   down  (Conv2d fwd, ConvTranspose2d dgrad): thread = 8 (4) consecutive output pixels x 8 output channels; the image
@@ -68,8 +67,7 @@ __device__ __forceinline__ void load_hi_tile(float* __restrict__ s_hi, const flo
 // (4 threads cover the 32 channels of a pixel group; 256 threads = one 16-row tile).  Per input row kh the thread
 // fetches the 2*PXG+2 input values its pixels share (broadcast among the 4 channel threads) and per tap two LDS.128
 // of weights feed 8*PXG FMAs -- ~1 shared-memory instruction per 14 FMAs.  (The first mapping, 2 pixels x 32
-// channels per thread, needed one LDS.128 per 8 FMAs and was bound by the LSU queue: ncu mio_throttle 1.2, FMA pipe
-// 24 %, 74 us at B = 1024.)  A lane quartet writes 64 contiguous bytes per store instruction (whole sectors).
+// channels per thread, needed one LDS.128 per 8 FMAs and was bound by the LSU queue.)  A lane quartet writes 64 contiguous bytes per store instruction (whole sectors).
 // ------------------------------------------------------------------------------------------------------------
 template <int CH, int W>
 __global__ void __launch_bounds__(kThreads, 2)

@@ -1,20 +1,16 @@
-// tcgen05 implicit-GEMM convolutions for the 32-channel Burgess layers (sm_100a): down, up (halo-resident) and wgrad.
+// Tensor-core implicit-GEMM convolutions for the 32-channel Burgess layers (sm_90a): down, up (halo-resident) and wgrad.
 //
 // Common scheme (details above each kernel):
 //   * The operand that comes from the ACTIVATIONS is fetched by TMA tiled loads straight from the NHWC tensor -- for the
 //     down kernel one load per tap with box {32 c, W cols, TR rows, TB images}, element strides {1,2,2,1} and start
 //     coordinate (0, kw-1, 2*i0-1+kh, b0): the stride-2 gather and the zero padding (out-of-bounds fill) are done by the
-//     TMA unit, nothing is im2col'ed in memory.
-//   * fp32 parity on tf32 tensor cores: error-compensated 3xTF32.  a = a_hi + a_lo with a_hi = a with the low 13 mantissa
-//     bits cleared (exact in tf32), a_lo = a - a_hi (exact in fp32); D += a_hi*b_hi + a_hi*b_lo + a_lo*b_hi.  The
-//     activation-side operand is split by dedicated warps IN REGISTERS and written to TENSOR MEMORY (tcgen05.st), which
-//     holds the A operand of every MMA ("TS" form: an MMA with both operands in shared memory cannot go faster than its A
-//     tile can be fetched, scripts/micro/mma_rate.cu); the other operand (packed weights, or the lo tile for wgrad) sits in
-//     shared memory as [hi rows | lo rows], so the first two products are ONE N=64 MMA and the third an N=32 MMA.
-//   * warp roles (512 threads, 1 CTA/SM, persistent over tiles): warp 0 TMA producer, warp 1 MMA issuer (one elected
-//     lane), warp 2 TMEM allocator, warps 4-7 epilogue (TMEM -> registers -> bias/ReLU/mask -> 128-byte NHWC pixel lines),
-//     warps 8-11 and 12-15 two split groups working on alternate operand stages.  mbarrier rings: raw-full / raw-empty,
-//     A-ready / A-empty (4 TMEM stages), accumulator full / empty (2 TMEM stages).
+//     TMA unit, nothing is im2col'ed in memory.  Every tile lands with the 128-byte swizzle, so the fragment loads of the
+//     MMAs below are free of bank conflicts.
+//   * fp32 parity on tf32 tensor cores: error-compensated 3xTF32 (dv_ptx.cuh).  The operands are split into hi/lo planes
+//     in registers right after their fragment loads; the packed weights already hold both planes.
+//   * warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 load fragments, issue mma.sync m16n8k8 and run
+//     the epilogue; warp 8 is the TMA producer.  mbarrier rings between them: raw-full (TMA transaction count) and
+//     raw-empty (one arrival per consumer warp).
 #include <stdlib.h>
 #include "dv_common.cuh"
 #include "dv_ptx.cuh"
@@ -27,373 +23,66 @@ using namespace ptx;
 constexpr int kATile = 128 * 128;            // bytes: 128 pixel rows x 32 fp32
 constexpr int kBTap = 64 * 128;              // bytes: (32 hi + 32 lo) rows x 32 fp32
 constexpr int kBBytes = kTaps * kBTap;       // 131072
-constexpr uint32_t kHiMask = 0xFFFFE000u;    // keep sign, exponent and the 10 tf32 mantissa bits
+constexpr int kConsumers = 8;                // MMA / epilogue warps
+constexpr int kThreads = (kConsumers + 1) * 32;
+constexpr int kSmemMax = 232448;             // 227 KB per block on sm_90
 
-// raw fp32 tile -> residual plane lo = x - tf32_trunc(x).  The hi plane is the RAW tile itself: kind::tf32 reads only the
-// upper 19 bits of a 32-bit shared-memory operand, i.e. it truncates exactly like kHiMask (checked by the fp64-accuracy tests)
-__device__ __forceinline__ void split_lo_only(const uint4* raw, uint4* lo4, int t) {
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const int idx = t + 128 * k;
-    const uint4 v = raw[idx];
-    uint4 l;
-    l.x = __float_as_uint(__uint_as_float(v.x) - __uint_as_float(v.x & kHiMask));
-    l.y = __float_as_uint(__uint_as_float(v.y) - __uint_as_float(v.y & kHiMask));
-    l.z = __float_as_uint(__uint_as_float(v.z) - __uint_as_float(v.z & kHiMask));
-    l.w = __float_as_uint(__uint_as_float(v.w) - __uint_as_float(v.w & kHiMask));
-    lo4[idx] = l;
-  }
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers * 32) : "memory"); }
+
+// Four B fragments (hi and lo planes) of k slice ks for output columns nt*8 + g, from a packed-weight tap:
+// 64 rows x 128 B, rows [0,32) hi and [32,64) lo of the N-by-K (K contiguous) weight.
+__device__ __forceinline__ void load_b_tap(uint32_t tap_base, int nt, int ks, int g, int t, uint32_t (&bh)[2], uint32_t (&bl)[2]) {
+  const int n = nt * 8 + g;
+  bh[0] = lds32(tap_base + swz128(n, 8 * ks + t));
+  bh[1] = lds32(tap_base + swz128(n, 8 * ks + t + 4));
+  bl[0] = lds32(tap_base + swz128(32 + n, 8 * ks + t));
+  bl[1] = lds32(tap_base + swz128(32 + n, 8 * ks + t + 4));
 }
 
-// v[c] of lane l = value of (row l, channel c).  Returns, in lane l, the sum over the 32 rows of channel l
-// (butterfly transpose-reduce: 31 shuffles).  All 32 lanes must call it; v is destroyed.
-__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
-#define DV_CS_STEP(BIT, HALF)                                                        \
-  {                                                                                  \
-    const bool up = (lane & BIT) != 0;                                               \
-    _Pragma("unroll") for (int i = 0; i < HALF; ++i) {                               \
-      const float send = up ? v[i] : v[i + HALF];                                    \
-      const float keep = up ? v[i + HALF] : v[i];                                    \
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, BIT);                         \
-    }                                                                                \
-  }
-  DV_CS_STEP(16, 16) DV_CS_STEP(8, 8) DV_CS_STEP(4, 4) DV_CS_STEP(2, 2) DV_CS_STEP(1, 1)
-#undef DV_CS_STEP
-  return v[0];
-}
-
+// ------------------------------------------------------------------------------------------
+// down: lo[p][cl] = act(sum_{tap,c} hi(2i-1+kh, 2j-1+kw)[c] * w[cl][c][tap] + bias) * mask
+//   M = 128 lo pixels per tile (warp w: rows [16w, 16w+16)), N = 32, K = 16 taps x 32 channels.
+//   smem: weights (hi|lo, 128 KB) resident + a 5-stage ring of 16 KB tap tiles.
+// ------------------------------------------------------------------------------------------
 struct DownGeom {
   int B, H, W;          // lo geometry
   int rows_per_tile;    // 128 / W image-rows of lo per tile
   int num_tiles;
   long long total_px;
   int prefetch;         // L2-prefetch the next tile's hi rows (DV_TC_PREFETCH=0 switches it off)
-  int pipe;             // split warps overlap the TMEM stores of one tile with the loads/split of their next tile
-  int debug;            // DV_TC_DEBUG (timing experiments only, results are WRONG): 2 = load 4 of the 16 tap tiles
 };
-
-// MN-major tf32 operand.  32-bit MN-major data must use the "128B swizzle, 32-byte atom" layout
-// (cute::UMMA::LayoutType::SWIZZLE_128B_BASE32B = 1; TMA: CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B): rows of
-// 128 B (32 channels), 32-byte chunks XOR-ed with (row & 3), i.e. a K atom is 4 rows (512 B).
-// LBO = distance between 32-channel groups, SBO = distance between 4-row K atoms.
-__device__ __forceinline__ uint64_t umma_desc_sw128_mnmajor(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(512 >> 4) << 32) |
-         (1ull << 46) | (1ull << 61);
-}
-
-// ------------------------------------------------------------------------------------------
-// wgrad: dw[cl][c][tap] = sum_p lo[p][cl] * hi(2i-1+kh, 2j-1+kw)[c]   (reduction over PIXELS), hi-patch operand in
-// TENSOR MEMORY.  The round-1 kernel fed both operands from shared memory (MN-major tiles, M = 128 = two taps x hi/lo
-// planes, N = 64) and was bound by operand traffic: per 128-pixel tile the tensor core fetched 768 KB of A/B tiles on top
-// of 816 KB of TMA writes and split reads/writes (1.6 MB at 128 B/clk = 12.4 K clk against 4 K clk of tensor time):
-// 130.7 us at (1024,16,32).  Here the A operand never exists in shared memory (73.0 us, same launch):
-//      A (TMEM, M = 128 lanes) = four taps x 32 hi channels of one kernel row,   K = 32 pixels per stage
-//      B (smem, MN-major)      = [L_raw | L_lo] of the lo tile (N = 64) and L_raw alone (N = 32)
-//      D_g[:, 0:32] = T_hi x L_hi,   D_g[:, 32:64] = T_hi x L_lo + T_lo x L_hi        (3xTF32, no lo x lo product;
-//      the two correction products accumulate apart from the main one, so they are not rounded at its magnitude)
-// The split warps own one tap each (lane = hi channel): they read 32 pixels of their channel from the raw TMA
-// tile (one conflict-free 128-byte row per warp load), split hi/lo in registers and tcgen05.st the two planes to
-// the A stage -- the transposition pixel-major -> channel-on-lanes costs nothing.  Only the 32 KB of lo-tile
-// planes are fetched by the MMAs (192 KB per tile), and no lo plane of the hi patch is written anywhere.
-//   smem : 8 raw tap tiles x 16 KB (unswizzled) + 2 x (L_raw | L_lo) x 16 KB
-//   TMEM : [0,256) accumulators (GPC kernel rows x 64 columns), [256,512) A stages (4 x {hi 32 | lo 32})
-// Split-K over CTAs; the partials are reduced in a fixed order by conv_wgrad_reduce_kernel.
-// ------------------------------------------------------------------------------------------
-constexpr int kWtThreads = 512;
-constexpr int kWtRawSlots = 8;
-constexpr int kWtAStages = 4;
-constexpr int kWtACol0 = 256;
-struct WtBarriers {
-  uint64_t raw_full[kWtRawSlots], raw_empty[kWtRawSlots];
-  uint64_t a_ready[kWtAStages], a_empty[kWtAStages];
-  uint64_t l_raw_full[2], l_ready[2], l_empty[2];
-  uint64_t acc_full;
-  uint32_t tmem_base;
-  float lscr[128][4];
-};
-constexpr int kWgLBytes = 2 * kATile;                  // L_raw, L_lo
-constexpr int kWtSmemBytes = kWtRawSlots * kATile + 2 * kWgLBytes + 1024 + 3072;
-static_assert(sizeof(WtBarriers) <= 3072, "barrier block too large");
-static_assert(kWtSmemBytes <= 232448, "smem");
-
-struct WtGeom {
-  int B, H, W, rows_per_tile, num_tiles, tiles_per_cta;
-  int prefetch;
-};
-
-// GPC = kernel rows (groups of four taps) per CTA: blockIdx.y owns rows [y*GPC, (y+1)*GPC).  (A second accumulator
-// per row for the odd K steps was measured: 74.0 vs 73.0 us, no gain.)
-template <int GPC>
-__global__ void __launch_bounds__(kWtThreads, 1)
-conv_wgrad32_ts_kernel(const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo,
-                       float* __restrict__ ws, WtGeom g) {
-  static_assert(GPC * 64 <= kWtACol0, "accumulators overlap the A stages");
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* Raw = smem;                                       // [slot][128 px][32 ch], no swizzle
-  uint8_t* Ls = smem + kWtRawSlots * kATile;                 // [buf][L_raw | L_lo], 128B swizzle with 32-byte atoms
-  WtBarriers* bars = reinterpret_cast<WtBarriers*>(Ls + 2 * kWgLBytes);
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-  const int t_begin = blockIdx.x * g.tiles_per_cta;
-  const int t_end = min(g.num_tiles, t_begin + g.tiles_per_cta);
-  const int g_begin = blockIdx.y * GPC;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kWtRawSlots; ++s) { mbar_init(&bars->raw_full[s], 1); mbar_init(&bars->raw_empty[s], 128); }
-    for (int s = 0; s < kWtAStages; ++s) { mbar_init(&bars->a_ready[s], 128); mbar_init(&bars->a_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&bars->l_raw_full[s], 1); mbar_init(&bars->l_ready[s], 128); mbar_init(&bars->l_empty[s], 1); }
-    mbar_init(&bars->acc_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == 2) tmem_alloc(&bars->tmem_base, 512);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  if (bars->tmem_base != 0u) __trap();                       // whole TMEM is ours: base column 0
-  constexpr uint32_t tmem_base = 0u;
-
-  if (warp == 0 && elect_one()) {
-    prefetch_tmap(&tmap_hi); prefetch_tmap(&tmap_lo);
-    int lb = 0; uint32_t lphase = 0; uint32_t m = 0;
-    for (int tile = t_begin; tile < t_end; ++tile) {
-      const int r0 = tile * g.rows_per_tile;
-      const int b0 = r0 / g.H, i0 = r0 % g.H;
-      if (g.prefetch && tile + 1 < t_end) {                  // pull the next tile's hi rows (and lo tile) into L2
-        const int rn = (tile + 1) * g.rows_per_tile;
-        const int bn = rn / g.H, in_ = rn % g.H;
-        for (int t4 = 0; t4 < 4; ++t4) tma_prefetch_4d(&tmap_hi, 0, (t4 & 1), 2 * in_ + (t4 >> 1), bn);
-        tma_prefetch_4d(&tmap_lo, 0, 0, in_, bn);
-      }
-      mbar_wait(&bars->l_empty[lb], lphase ^ 1);
-      mbar_arrive_expect_tx(&bars->l_raw_full[lb], kATile);
-      tma_load_4d(Ls + lb * kWgLBytes, &tmap_lo, &bars->l_raw_full[lb], 0, 0, i0, b0);
-      if (++lb == 2) { lb = 0; lphase ^= 1; }
-      for (int gi = 0; gi < GPC; ++gi) {
-        const int kh = g_begin + gi;
-        for (int kw = 0; kw < 4; ++kw, ++m) {
-          const int slot = m % kWtRawSlots;
-          mbar_wait(&bars->raw_empty[slot], ((m / kWtRawSlots) & 1u) ^ 1u);
-          mbar_arrive_expect_tx(&bars->raw_full[slot], kATile);
-          tma_load_4d(Raw + slot * kATile, &tmap_hi, &bars->raw_full[slot], 0, kw - 1, 2 * i0 - 1 + kh, b0);
-        }
-      }
-    }
-  } else if (warp == 1 && elect_one()) {      // ONE elected lane runs the whole issue loop (waits included)
-    // A from TMEM (K along the columns), B MN-major (bit 16)
-    constexpr uint32_t idesc64 = umma_idesc_tf32(128, 64) | (1u << 16), idesc32 = umma_idesc_tf32(128, 32) | (1u << 16);
-    int lb = 0; uint32_t lphase = 0; uint32_t n = 0;
-    for (int tile = t_begin; tile < t_end; ++tile) {
-      mbar_wait(&bars->l_ready[lb], lphase);
-      tc_fence_after_sync();
-      const uint32_t l_addr = smem_u32(Ls + lb * kWgLBytes);
-      for (int gi = 0; gi < GPC; ++gi) {
-        for (int s = 0; s < 4; ++s, ++n) {
-          const int as = n % kWtAStages;
-          mbar_wait(&bars->a_ready[as], (n / kWtAStages) & 1u);
-          tc_fence_after_sync();
-          const uint32_t a_hi = tmem_base + kWtACol0 + as * 64, a_lo = a_hi + 32;
-#pragma unroll
-          for (int k4 = 0; k4 < 4; ++k4) {                   // 8 pixels per MMA
-            const uint64_t b_d = umma_desc_sw128_mnmajor(l_addr + (s * 4 + k4) * 1024, kATile);
-            const uint32_t d = tmem_base + gi * 64;
-            const bool first = (tile == t_begin) && (s == 0) && (k4 == 0);
-            umma_tf32_ts_1t(d, a_hi + 8 * k4, b_d, idesc64, first ? 0u : 1u);     // [T_hi x L_hi | T_hi x L_lo]
-            umma_tf32_ts_1t(d + 32, a_lo + 8 * k4, b_d, idesc32, 1u);             // T_lo x L_hi joins the corrections
-          }
-          umma_commit_1t(&bars->a_empty[as]);
-        }
-      }
-      umma_commit_1t(&bars->l_empty[lb]);
-      if (++lb == 2) { lb = 0; lphase ^= 1; }
-    }
-    umma_commit_1t(&bars->acc_full);
-  } else if (warp >= 8) {
-    // split warps: warp quarter q owns tap (kh, kw = q) of the current kernel row, lane = hi channel; the two groups
-    // alternate over the 32-pixel stages.  The tcgen05.st of one stage stay in flight while the next one is loaded.
-    const int q = warp & 3, grp = (warp - 8) >> 2;
-    const uint32_t raw0 = smem_u32(Raw) + lane * 4;
-    uint32_t n = 0, tseq = 0;
-    int prev_as = -1, prev_slot = 0;
-    for (int tile = t_begin; tile < t_end; ++tile, ++tseq) {
-      for (int gi = 0; gi < GPC; ++gi) {
-        const uint32_t m = (tseq * GPC + gi) * 4 + q;
-        const int slot = m % kWtRawSlots;
-        for (int s = 0; s < 4; ++s, ++n) {
-          if ((int)(n & 1u) != grp) continue;
-          const int as = n % kWtAStages;
-          mbar_wait(&bars->raw_full[slot], (m / kWtRawSlots) & 1u);
-          const uint32_t src = raw0 + slot * kATile + s * 32 * 128;
-          uint32_t h[32], l[32];
-#pragma unroll
-          for (int k = 0; k < 32; ++k) {
-            const uint32_t v = lds32(src + k * 128);
-            const uint32_t hb = v & kHiMask;
-            h[k] = hb;
-            l[k] = __float_as_uint(__uint_as_float(v) - __uint_as_float(hb));
-          }
-          if (prev_as >= 0) {
-            tmem_st_wait();
-            mbar_arrive(&bars->raw_empty[prev_slot]);
-            tc_fence_before_sync();
-            mbar_arrive(&bars->a_ready[prev_as]);
-          }
-          mbar_wait(&bars->a_empty[as], ((n / kWtAStages) & 1u) ^ 1u);
-          tc_fence_after_sync();
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + kWtACol0 + as * 64;
-          tmem_st_32x32b_x32(taddr, h);
-          tmem_st_32x32b_x32(taddr + 32, l);
-          prev_as = as; prev_slot = slot;
-        }
-      }
-    }
-    if (prev_as >= 0) {
-      tmem_st_wait();
-      mbar_arrive(&bars->raw_empty[prev_slot]);
-      tc_fence_before_sync();
-      mbar_arrive(&bars->a_ready[prev_as]);
-    }
-  } else if (warp >= 4) {
-    // warps 4-7: lo tile -> (raw | residual) planes and its channel sums (bias gradient) while the tiles stream,
-    // then the epilogue (once per CTA): TMEM -> main + correction columns -> workspace partial
-    const int t = threadIdx.x - 128;
-    float ls[4] = {0.f, 0.f, 0.f, 0.f};
-    int lb = 0; uint32_t lphase = 0;
-    for (int tile = t_begin; tile < t_end; ++tile) {
-      mbar_wait(&bars->l_raw_full[lb], lphase);
-      const uint4* raw = reinterpret_cast<const uint4*>(Ls + lb * kWgLBytes);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const uint4 v = raw[t + 128 * k];
-        ls[0] += __uint_as_float(v.x); ls[1] += __uint_as_float(v.y); ls[2] += __uint_as_float(v.z); ls[3] += __uint_as_float(v.w);
-      }
-      split_lo_only(raw, reinterpret_cast<uint4*>(Ls + lb * kWgLBytes + kATile), t);
-      fence_proxy_async_smem();
-      mbar_arrive(&bars->l_ready[lb]);
-      if (++lb == 2) { lb = 0; lphase ^= 1; }
-    }
-#pragma unroll
-    for (int e = 0; e < 4; ++e) bars->lscr[t][e] = ls[e];
-    asm volatile("bar.sync 2, 128;" ::: "memory");
-    if (t < 32 && blockIdx.y == 0) {                        // (every kernel-row group sees the same lo tiles)
-      const int want = t >> 2, e = t & 3;
-      float acc = 0.f;
-      for (int u = 0; u < 128; ++u)
-        if ((((((u & 7) >> 1) ^ ((u >> 3) & 3)) << 1) | (u & 1)) == want) acc += bars->lscr[u][e];
-      ws[(long long)blockIdx.x * (kTaps * 32 + 1) * kLoCh + (kTaps * 32) * kLoCh + t] = acc;
-    }
-    const int q = warp & 3;
-    mbar_wait(&bars->acc_full, 0);
-    tc_fence_after_sync();
-    float* out = ws + (long long)blockIdx.x * (kTaps * 32 + 1) * kLoCh;
-#pragma unroll 1
-    for (int gi = 0; gi < GPC; ++gi) {
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + gi * 64;
-      uint32_t r0[32], r1[32];
-      float v[32];
-      tmem_ld_32x32b_x32(taddr, r0);
-      tmem_ld_32x32b_x32(taddr + 32, r1);
-      tmem_ld_wait();
-#pragma unroll
-      for (int cl = 0; cl < 32; ++cl) v[cl] = __uint_as_float(r0[cl]) + __uint_as_float(r1[cl]);
-      const int tap = (g_begin + gi) * 4 + q;
-      float* dst = out + (tap * 32 + lane) * kLoCh;
-#pragma unroll
-      for (int c4 = 0; c4 < 8; ++c4)
-        *reinterpret_cast<float4*>(dst + c4 * 4) = make_float4(v[c4 * 4], v[c4 * 4 + 1], v[c4 * 4 + 2], v[c4 * 4 + 3]);
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after_sync(); tmem_dealloc(tmem_base, 512); }
-}
-
-
-// ==========================================================================================
-// "TS" variants of down/up for CH == 32: the A operand of the MMA lives in TENSOR MEMORY.
-// The split warps read their pixel row from the TMA-swizzled raw tile (thread = row, conflict-free),
-// compute the hi/lo planes in registers and tcgen05.st them into TMEM (lane = pixel row, column = k),
-// so the shared-memory copy of the lo plane, its 32 KB/tap of write traffic and the 48 KB/tap of
-// operand reads disappear, and the freed shared memory deepens the TMA pipeline from 3 to 6 stages
-// (these kernels are latency-bound on TMA -> split -> MMA -> commit round trips otherwise).
-//   smem : weights 128 KB resident + 6 raw stages x 16 KB
-//   TMEM : columns [0,256) accumulators (2 stages), [256,512) A operand (4 stages x {hi 32 | lo 32})
-// ==========================================================================================
-// Round-2 experiments on these kernels, all measured on hardware and all slower, none kept (DESIGN.md section 4):
-//   * hi operand straight from the raw TMA tile (SS MMA, only the lo plane through TMEM): 87.5 vs 75.6 us at
-//     (1024,16,32) -- the 16 KB/tap operand fetch competes with the weight tile for shared-memory read bandwidth;
-//   * a third group of split warps (640 threads): 83.1 vs 73.1 us (down), 93.0 vs 90.9 us (up) without register
-//     re-balancing, 78.1 / 93.4 us with setmaxnreg (control 40 / epilogue 112) -- the split warps are NOT what the
-//     MMA issuer waits for once two groups alternate (a setmaxnreg budget that also grew the split warps deadlocked).
-constexpr int kTsThreads = 512;          // warps 8-11 and 12-15: two split groups working on alternate tiles
-constexpr int kTsRawStages = 6;
-constexpr int kTsAStages = 4;
-constexpr int kTsACol0 = 256;
-struct TsBarriers {
-  uint64_t raw_full[kTsRawStages], raw_empty[kTsRawStages];
-  uint64_t a_ready[kTsAStages], a_empty[kTsAStages];
+constexpr int kDownStages = 5;
+struct DownBarriers {
+  uint64_t raw_full[kDownStages], raw_empty[kDownStages];
   uint64_t b_full;
-  uint64_t acc_full[2], acc_empty[2];
-  uint32_t tmem_base;
   float bias[32];
+  float csum[kConsumers][32];
 };
-constexpr int kTsSmemBytes = kBBytes + kTsRawStages * kATile + 1024 + 512;
-static_assert(sizeof(TsBarriers) <= 512, "barrier block too large");
-static_assert(kTsSmemBytes <= 232448, "smem");
+constexpr int kDownSmem = kBBytes + kDownStages * kATile + 1024 + 2048;
+static_assert(sizeof(DownBarriers) <= 2048, "barrier block too large");
+static_assert(kDownSmem <= kSmemMax, "smem");
 
-__device__ __forceinline__ void ts_init(TsBarriers* bars, const float* bias, int warp) {
+__global__ void __launch_bounds__(kThreads, 1)
+conv_down32_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const float* __restrict__ bias, const float* __restrict__ mask, float* __restrict__ lo,
+                       DownGeom g, int act, float* __restrict__ colsum_part,
+                       const uint32_t* __restrict__ mask_bits, uint32_t* __restrict__ bits_out) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  uint8_t* Bs = smem;
+  uint8_t* Raw = smem + kBBytes;
+  DownBarriers* bars = reinterpret_cast<DownBarriers*>(Raw + kDownStages * kATile);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kTsRawStages; ++s) { mbar_init(&bars->raw_full[s], 1); mbar_init(&bars->raw_empty[s], 128); }
-    for (int s = 0; s < kTsAStages; ++s) { mbar_init(&bars->a_ready[s], 128); mbar_init(&bars->a_empty[s], 1); }
+    for (int s = 0; s < kDownStages; ++s) { mbar_init(&bars->raw_full[s], 1); mbar_init(&bars->raw_empty[s], kConsumers); }
     mbar_init(&bars->b_full, 1);
-    for (int a = 0; a < 2; ++a) { mbar_init(&bars->acc_full[a], 1); mbar_init(&bars->acc_empty[a], 128); }
     fence_mbar_init();
   }
   if (threadIdx.x < 32) bars->bias[threadIdx.x] = bias ? bias[threadIdx.x] : 0.f;
-  if (warp == 2) tmem_alloc(&bars->tmem_base, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-}
 
-// split warps (warps 8-11): one raw tile -> hi/lo planes in TMEM stage `as`
-__device__ __forceinline__ void ts_split_tile(const uint8_t* raw, uint32_t tmem_base, int as, int q, int lane) {
-  const int row = q * 32 + lane;
-  uint32_t h[32], l[32];
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    const uint4 v = lds128(raw + row * 128 + ((c ^ (row & 7)) << 4));
-    const uint32_t vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const uint32_t hb = vv[e] & kHiMask;
-      h[c * 4 + e] = hb;
-      l[c * 4 + e] = __float_as_uint(__uint_as_float(vv[e]) - __uint_as_float(hb));
-    }
-  }
-  const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + kTsACol0 + as * 64;
-  tmem_st_32x32b_x32(taddr, h);
-  tmem_st_32x32b_x32(taddr + 32, l);
-  tmem_st_wait();
-}
-
-__global__ void __launch_bounds__(kTsThreads, 1)
-conv_down32_ts_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                      const float* __restrict__ bias, const float* __restrict__ mask, float* __restrict__ lo,
-                      DownGeom g, int act, float* __restrict__ colsum_part,
-                      const uint32_t* __restrict__ mask_bits, uint32_t* __restrict__ bits_out) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* Bs = smem;
-  uint8_t* Raw = smem + kBBytes;
-  TsBarriers* bars = reinterpret_cast<TsBarriers*>(Raw + kTsRawStages * kATile);
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // provably warp-uniform role index
-  ts_init(bars, bias, warp);
-  // All 512 columns are ours (1 CTA/SM), so the allocation starts at column 0.  Using the literal keeps every
-  // tensor-memory address a compile-time/warp-uniform value (no per-MMA register -> uniform-register moves).
-  if (bars->tmem_base != 0u) __trap();
-  constexpr uint32_t tmem_base = 0u;
-
-  if (warp == 0 && elect_one()) {
+  if (warp == kConsumers) {
+    if (lane != 0) return;
     prefetch_tmap(&tmap_a); prefetch_tmap(&tmap_b);
     mbar_arrive_expect_tx(&bars->b_full, kBBytes);
     for (int tap = 0; tap < kTaps; ++tap) tma_load_2d(Bs + tap * kBTap, &tmap_b, &bars->b_full, 0, tap * 64);
@@ -410,172 +99,252 @@ conv_down32_ts_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
       for (int tap = 0; tap < kTaps; ++tap) {
         const int kh = tap >> 2, kw = tap & 3;
         mbar_wait(&bars->raw_empty[stage], phase ^ 1);
-        if ((g.debug & 2) && (tap & 3)) {
-          mbar_arrive(&bars->raw_full[stage]);                 // timing experiment: no data for this tap
-        } else {
-          mbar_arrive_expect_tx(&bars->raw_full[stage], kATile);
-          tma_load_4d(Raw + stage * kATile, &tmap_a, &bars->raw_full[stage], 0, kw - 1, 2 * i0 - 1 + kh, b0);
-        }
-        if (++stage == kTsRawStages) { stage = 0; phase ^= 1; }
+        mbar_arrive_expect_tx(&bars->raw_full[stage], kATile);
+        tma_load_4d(Raw + stage * kATile, &tmap_a, &bars->raw_full[stage], 0, kw - 1, 2 * i0 - 1 + kh, b0);
+        if (++stage == kDownStages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1 && elect_one()) {      // ONE elected lane runs the whole issue loop (barrier waits included):
-                                              // ptxas then keeps every MMA operand in uniform registers (back-to-back UTCHMMA)
-    constexpr uint32_t idesc64 = umma_idesc_tf32(128, 64), idesc32 = umma_idesc_tf32(128, 32);
-    mbar_wait(&bars->b_full, 0);
-    int as = 0; uint32_t aphase = 0; int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      mbar_wait(&bars->acc_empty[acc], acc_phase ^ 1);
-      tc_fence_after_sync();
-      const uint32_t d_tmem = tmem_base + acc * 128;
-      for (int tap = 0; tap < kTaps; ++tap) {
-        mbar_wait(&bars->a_ready[as], aphase);
-        tc_fence_after_sync();
-        const uint32_t a_hi = tmem_base + kTsACol0 + as * 64, a_lo = a_hi + 32;
-        const uint64_t b_d = umma_desc_sw128_kmajor(smem_u32(Bs + tap * kBTap));
+    return;
+  }
+
+  const int gq = lane >> 2, t = lane & 3;
+  const int r0 = warp * 16 + gq;                             // this thread's tile rows: r0 and r0 + 8
+  const uint32_t bs = smem_u32(Bs), raw0 = smem_u32(Raw);
+  float csum[4][2] = {};                                     // channel sums of the stored output (colsum_part)
+  mbar_wait(&bars->b_full, 0);
+  int stage = 0; uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
+    float tot[4][4] = {}, corr[4][4] = {};
+    for (int tap = 0; tap < kTaps; ++tap) {
+      mbar_wait(&bars->raw_full[stage], phase);
+      const uint32_t a_base = raw0 + stage * kATile, b_base = bs + tap * kBTap;
+      float mn[4][4] = {};                                   // hi*hi of this tap, added to tot in fp32 below
 #pragma unroll
-        for (int k4 = 0; k4 < 4; ++k4) {
-          const uint32_t d = d_tmem + (k4 & 1) * 64;          // two accumulation chains, see the SS kernel
-          umma_tf32_ts_1t(d, a_hi + 8 * k4, b_d + 2 * k4, idesc64, (tap | (k4 >> 1)) != 0);
-          umma_tf32_ts_1t(d, a_lo + 8 * k4, b_d + 2 * k4, idesc32, 1);
+      for (int ks = 0; ks < 4; ++ks) {
+        uint32_t a[4], ah[4], al[4];
+        a[0] = lds32(a_base + swz128(r0, 8 * ks + t));
+        a[1] = lds32(a_base + swz128(r0 + 8, 8 * ks + t));
+        a[2] = lds32(a_base + swz128(r0, 8 * ks + t + 4));
+        a[3] = lds32(a_base + swz128(r0 + 8, 8 * ks + t + 4));
+#pragma unroll
+        for (int e = 0; e < 4; ++e) split_tf32(a[e], ah[e], al[e]);
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+          uint32_t bh[2], bl[2];
+          load_b_tap(b_base, nt, ks, gq, t, bh, bl);
+          mma_3xtf32(mn[nt], corr[nt], ah, al, bh, bl);
         }
-        umma_commit_1t(&bars->a_empty[as]);
-        if (++as == kTsAStages) { as = 0; aphase ^= 1; }
       }
-      umma_commit_1t(&bars->acc_full[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->raw_empty[stage]);
+      if (++stage == kDownStages) { stage = 0; phase ^= 1; }
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) tot[nt][e] += mn[nt][e];
     }
-  } else if (warp >= 4 && warp < 8) {
-    const int q = warp & 3;
-    int acc = 0; uint32_t acc_phase = 0;
-    float csum = 0.f;                                         // lane l: running sum of output channel l over this warp's rows
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      const long long p = (long long)tile * 128 + q * 32 + lane;
-      // ReLU-backward mask as one word per pixel (bit c = channel c), requested before the accumulator wait
-      uint32_t mbits = 0xffffffffu;
-      if (mask_bits && p < g.total_px) mbits = __ldg(mask_bits + p);
-      mbar_wait(&bars->acc_full[acc], acc_phase);
-      tc_fence_after_sync();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * 128;
-      uint32_t r0[32], r1[32];
-      float sum[32];
-      tmem_ld_32x32b_x32(taddr, r0);
-      tmem_ld_32x32b_x32(taddr + 64, r1);
-      tmem_ld_wait();
 #pragma unroll
-      for (int c = 0; c < 32; ++c) sum[c] = __uint_as_float(r0[c]) + __uint_as_float(r1[c]);
-      tmem_ld_32x32b_x32(taddr + 32, r0);
-      tmem_ld_32x32b_x32(taddr + 96, r1);
-      tmem_ld_wait();
-      tc_fence_before_sync();
-      mbar_arrive(&bars->acc_empty[acc]);
-      if (p < g.total_px) {
-        float* dst = lo + p * 32;
-        const float* mk = (mask && !mask_bits) ? mask + p * 32 : nullptr;
-        uint32_t obits = 0u;
+    for (int h = 0; h < 2; ++h) {
+      const long long p = (long long)tile * 128 + r0 + 8 * h;
+      const bool valid = p < g.total_px;
+      uint32_t mb = 0xffffffffu;                             // ReLU-backward mask as one word per pixel (bit c = channel c)
+      if (mask_bits && valid) mb = __ldg(mask_bits + p);
+      const float* mk = (mask && !mask_bits && valid) ? mask + p * 32 : nullptr;
+      uint32_t ob = 0u;
 #pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4) {
-          float v[4];
+      for (int nt = 0; nt < 4; ++nt) {
+        const int c = nt * 8 + 2 * t;
+        float v[2];
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int c = c4 * 4 + e;
-            float x = (sum[c] + (__uint_as_float(r0[c]) + __uint_as_float(r1[c]))) + bars->bias[c];
-            if (act == DV_ACT_RELU) x = fmaxf(x, 0.f);
-            v[e] = ((mbits >> c) & 1u) ? x : 0.f;
-          }
-          if (mk) {
-            const float4 m4 = ldg4(mk + c4 * 4);
-            v[0] = m4.x > 0.f ? v[0] : 0.f; v[1] = m4.y > 0.f ? v[1] : 0.f;
-            v[2] = m4.z > 0.f ? v[2] : 0.f; v[3] = m4.w > 0.f ? v[3] : 0.f;
-          }
-          *reinterpret_cast<float4*>(dst + c4 * 4) = make_float4(v[0], v[1], v[2], v[3]);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            sum[c4 * 4 + e] = v[e];
-            obits |= (v[e] > 0.f ? 1u : 0u) << (c4 * 4 + e);
-          }
+        for (int e = 0; e < 2; ++e) {
+          float x = (tot[nt][2 * h + e] + corr[nt][2 * h + e]) + bars->bias[c + e];
+          if (act == DV_ACT_RELU) x = fmaxf(x, 0.f);
+          v[e] = ((mb >> (c + e)) & 1u) ? x : 0.f;
         }
-        if (bits_out) bits_out[p] = obits;                     // [x > 0] of the stored pixel: the next backward pass's mask
-      } else {
-#pragma unroll
-        for (int c = 0; c < 32; ++c) sum[c] = 0.f;
-      }
-      if (colsum_part) csum += warp_colsum32(sum, lane);      // channel sums of the stored output (next layer's bias gradient)
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-    if (colsum_part) {
-      // the last accumulator was complete -> every MMA and TMA load of this CTA is done: the raw stages are free
-      float* scr = reinterpret_cast<float*>(Raw);
-      scr[q * 32 + lane] = csum;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (q == 0) colsum_part[blockIdx.x * 32 + lane] = (scr[lane] + scr[32 + lane]) + (scr[64 + lane] + scr[96 + lane]);
-    }
-  } else if (warp >= 8) {
-    const int q = warp & 3, grp = (warp - 8) >> 2;
-    uint32_t n = 0;                                           // sequence number of the raw tile within this CTA
-    if (!g.pipe) {
-      for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-        for (int tap = 0; tap < kTaps; ++tap, ++n) {
-          if ((int)(n & 1u) != grp) continue;
-          const int stage = n % kTsRawStages, as = n % kTsAStages;
-          mbar_wait(&bars->raw_full[stage], (n / kTsRawStages) & 1u);
-          mbar_wait(&bars->a_empty[as], ((n / kTsAStages) & 1u) ^ 1u);
-          tc_fence_after_sync();
-          ts_split_tile(Raw + stage * kATile, tmem_base, as, q, lane);
-          mbar_arrive(&bars->raw_empty[stage]);
-          tc_fence_before_sync();
-          mbar_arrive(&bars->a_ready[as]);
+        if (mk) {
+          const float2 m2 = __ldg(reinterpret_cast<const float2*>(mk + c));
+          v[0] = m2.x > 0.f ? v[0] : 0.f; v[1] = m2.y > 0.f ? v[1] : 0.f;
         }
+        if (valid) *reinterpret_cast<float2*>(lo + p * 32 + c) = make_float2(v[0], v[1]);
+        else v[0] = v[1] = 0.f;
+        ob |= (v[0] > 0.f ? 1u : 0u) << c | (v[1] > 0.f ? 1u : 0u) << (c + 1);
+        csum[nt][0] += v[0]; csum[nt][1] += v[1];
       }
-    } else {
-      // Software pipeline: the tcgen05.st of tile n stay in flight while tile n+2 (this group's next one) is loaded
-      // from shared memory and split in registers; tile n is published (and its raw stage released -- only after
-      // tcgen05.wait::st, when its shared-memory reads have certainly been consumed) just before the next stores.
-      const int row = q * 32 + lane;
-      int prev_stage = -1, prev_as = 0;
-      for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-        for (int tap = 0; tap < kTaps; ++tap, ++n) {
-          if ((int)(n & 1u) != grp) continue;
-          const int stage = n % kTsRawStages, as = n % kTsAStages;
-          mbar_wait(&bars->raw_full[stage], (n / kTsRawStages) & 1u);
-          const uint8_t* raw = Raw + stage * kATile;
-          uint32_t h[32], l[32];
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const uint4 v = lds128(raw + row * 128 + ((c ^ (row & 7)) << 4));
-            const uint32_t vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const uint32_t hb = vv[e] & kHiMask;
-              h[c * 4 + e] = hb;
-              l[c * 4 + e] = __float_as_uint(__uint_as_float(vv[e]) - __uint_as_float(hb));
-            }
-          }
-          if (prev_stage >= 0) {
-            tmem_st_wait();
-            mbar_arrive(&bars->raw_empty[prev_stage]);
-            tc_fence_before_sync();
-            mbar_arrive(&bars->a_ready[prev_as]);
-          }
-          mbar_wait(&bars->a_empty[as], ((n / kTsAStages) & 1u) ^ 1u);
-          tc_fence_after_sync();
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + kTsACol0 + as * 64;
-          tmem_st_32x32b_x32(taddr, h);
-          tmem_st_32x32b_x32(taddr + 32, l);
-          prev_stage = stage; prev_as = as;
-        }
-      }
-      if (prev_stage >= 0) {
-        tmem_st_wait();
-        mbar_arrive(&bars->raw_empty[prev_stage]);
-        tc_fence_before_sync();
-        mbar_arrive(&bars->a_ready[prev_as]);
-      }
+      ob |= __shfl_xor_sync(0xffffffffu, ob, 1);
+      ob |= __shfl_xor_sync(0xffffffffu, ob, 2);
+      if (bits_out && valid && t == 0) bits_out[p] = ob;     // [x > 0] of the stored pixel: the next backward pass's mask
     }
   }
-  tc_fence_before_sync();
+  if (colsum_part) {                                         // fixed-order reduction: lanes of a quad column, then warps
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float s = csum[nt][e];
+        s += __shfl_xor_sync(0xffffffffu, s, 4);
+        s += __shfl_xor_sync(0xffffffffu, s, 8);
+        s += __shfl_xor_sync(0xffffffffu, s, 16);
+        if (gq == 0) bars->csum[warp][nt * 8 + 2 * t + e] = s;
+      }
+    consumers_sync();
+    if (warp == 0) {
+      float s = 0.f;
+      for (int w = 0; w < kConsumers; ++w) s += bars->csum[w][lane];
+      colsum_part[blockIdx.x * 32 + lane] = s;
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// wgrad: dw[cl][c][tap] = sum_p lo[p][cl] * hi(2i-1+kh, 2j-1+kw)[c]   (reduction over PIXELS)
+//   Per 128-pixel tile: the lo tile (B operand, N = 32 lo channels) and the 16 tap tiles of the hi patch (A operand,
+//   M = 32 hi channels, read transposed out of the [pixel][channel] tile).  Warp w owns taps w and w + 8 and always
+//   consumes ring slot w.  K slot t of an MMA holds pixel 8ks + 2t and slot t + 4 pixel 8ks + 2t + 1: with the 128-byte
+//   swizzle the transposed fragment loads then hit 32 distinct banks.  The fp32 running totals (2 taps x 32 x 32 per
+//   warp) live in shared memory, lane-interleaved (conflict-free), which keeps the MMA loop free of register spills.
+//   Split-K over CTAs; the partials are reduced in a fixed order by conv_wgrad_reduce_kernel.
+// ------------------------------------------------------------------------------------------
+constexpr int kWtSlots = kConsumers;
+struct WtBarriers {
+  uint64_t raw_full[kWtSlots], raw_empty[kWtSlots];
+  uint64_t l_full[2], l_empty[2];
+  float lsum[kConsumers][32];
+};
+constexpr int kWtTotFloats = 2 * 32 * 32;              // per consumer warp: [tap w / w+8][32 fragment values][lane]
+constexpr int kWtSmem = kWtSlots * kATile + 2 * kATile + 2048 + kConsumers * kWtTotFloats * 4 + 1024;
+static_assert(sizeof(WtBarriers) <= 2048, "barrier block too large");
+static_assert(kWtSmem <= kSmemMax, "smem");
+
+struct WtGeom {
+  int B, H, W, rows_per_tile, num_tiles, tiles_per_cta;
+  int prefetch;
+};
+
+__global__ void __launch_bounds__(kThreads, 1)
+conv_wgrad32_mma_kernel(const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo,
+                        float* __restrict__ ws, WtGeom g) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  uint8_t* Raw = smem;                                       // [slot][128 px][32 ch]
+  uint8_t* Ls = smem + kWtSlots * kATile;                    // [buf][128 px][32 ch]
+  WtBarriers* bars = reinterpret_cast<WtBarriers*>(Ls + 2 * kATile);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* tot = reinterpret_cast<float*>(Ls + 2 * kATile + 2048) + warp * kWtTotFloats + lane;   // tot[k * 32]
+  const int t_begin = blockIdx.x * g.tiles_per_cta;
+  const int t_end = min(g.num_tiles, t_begin + g.tiles_per_cta);
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kWtSlots; ++s) { mbar_init(&bars->raw_full[s], 1); mbar_init(&bars->raw_empty[s], 1); }
+    for (int s = 0; s < 2; ++s) { mbar_init(&bars->l_full[s], 1); mbar_init(&bars->l_empty[s], kConsumers); }
+    fence_mbar_init();
+  }
   __syncthreads();
-  if (warp == 2) { tc_fence_after_sync(); tmem_dealloc(tmem_base, 512); }
+
+  if (warp == kConsumers) {
+    if (lane != 0) return;
+    prefetch_tmap(&tmap_hi); prefetch_tmap(&tmap_lo);
+    uint32_t tseq = 0;
+    for (int tile = t_begin; tile < t_end; ++tile, ++tseq) {
+      const int r0 = tile * g.rows_per_tile;
+      const int b0 = r0 / g.H, i0 = r0 % g.H;
+      if (g.prefetch && tile + 1 < t_end) {                  // pull the next tile's hi rows (and lo tile) into L2
+        const int rn = (tile + 1) * g.rows_per_tile;
+        const int bn = rn / g.H, in_ = rn % g.H;
+        for (int t4 = 0; t4 < 4; ++t4) tma_prefetch_4d(&tmap_hi, 0, (t4 & 1), 2 * in_ + (t4 >> 1), bn);
+        tma_prefetch_4d(&tmap_lo, 0, 0, in_, bn);
+      }
+      const int lb = tseq & 1;
+      mbar_wait(&bars->l_empty[lb], ((tseq >> 1) & 1u) ^ 1u);
+      mbar_arrive_expect_tx(&bars->l_full[lb], kATile);
+      tma_load_4d(Ls + lb * kATile, &tmap_lo, &bars->l_full[lb], 0, 0, i0, b0);
+      for (int tap = 0; tap < kTaps; ++tap) {
+        const int kh = tap >> 2, kw = tap & 3, slot = tap & 7;
+        const uint32_t use = tseq * 2 + (tap >> 3);          // uses of this slot so far
+        mbar_wait(&bars->raw_empty[slot], (use & 1u) ^ 1u);
+        mbar_arrive_expect_tx(&bars->raw_full[slot], kATile);
+        tma_load_4d(Raw + slot * kATile, &tmap_hi, &bars->raw_full[slot], 0, kw - 1, 2 * i0 - 1 + kh, b0);
+      }
+    }
+    return;
+  }
+
+  const int gq = lane >> 2, t = lane & 3;
+  const uint32_t slot_base = smem_u32(Raw) + warp * kATile, l0 = smem_u32(Ls);
+  for (int k = 0; k < 64; ++k) tot[k * 32] = 0.f;          // k = (tap w / w+8) * 32 + (c block * 4 + cl block) * 4 + fragment
+  float lsum = 0.f;                                          // lo channel `lane` over this warp's 16 rows of every tile
+  uint32_t tseq = 0;
+  for (int tile = t_begin; tile < t_end; ++tile, ++tseq) {
+    const int lb = tseq & 1;
+    mbar_wait(&bars->l_full[lb], (tseq >> 1) & 1u);
+    const uint32_t l_base = l0 + lb * kATile;
+#pragma unroll 4
+    for (int r = 0; r < 16; ++r) lsum += __uint_as_float(lds32(l_base + swz128(warp * 16 + r, lane)));
+#pragma unroll 1
+    for (int j = 0; j < 2; ++j) {
+      const uint32_t use = tseq * 2 + j;
+      mbar_wait(&bars->raw_full[warp], use & 1u);
+      float mn[2][4][4] = {}, cr[2][4][4] = {};
+#pragma unroll 1
+      for (int ks = 0; ks < 16; ++ks) {
+        const int px0 = 8 * ks + 2 * t, px1 = px0 + 1;
+        uint32_t ah[2][4], al[2][4], bh[4][2], bl[4][2];
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+          const int c = mt * 16 + gq;
+          uint32_t a[4];
+          a[0] = lds32(slot_base + swz128(px0, c));
+          a[1] = lds32(slot_base + swz128(px0, c + 8));
+          a[2] = lds32(slot_base + swz128(px1, c));
+          a[3] = lds32(slot_base + swz128(px1, c + 8));
+#pragma unroll
+          for (int e = 0; e < 4; ++e) split_tf32(a[e], ah[mt][e], al[mt][e]);
+        }
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+          const int cl = nt * 8 + gq;
+          split_tf32(lds32(l_base + swz128(px0, cl)), bh[nt][0], bl[nt][0]);
+          split_tf32(lds32(l_base + swz128(px1, cl)), bh[nt][1], bl[nt][1]);
+        }
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt) mma_3xtf32(mn[mt][nt], cr[mt][nt], ah[mt], al[mt], bh[nt], bl[nt]);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->raw_empty[warp]);
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) tot[(j * 32 + (mt * 4 + nt) * 4 + e) * 32] += mn[mt][nt][e] + cr[mt][nt][e];
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars->l_empty[lb]);
+  }
+
+  float* out = ws + (long long)blockIdx.x * (kTaps * 32 + 1) * kLoCh;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int tap = warp + 8 * j;
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int c = mt * 16 + gq + 8 * h, cl = nt * 8 + 2 * t;
+          *reinterpret_cast<float2*>(out + (tap * 32 + c) * kLoCh + cl) =
+              make_float2(tot[(j * 32 + (mt * 4 + nt) * 4 + 2 * h) * 32], tot[(j * 32 + (mt * 4 + nt) * 4 + 2 * h + 1) * 32]);
+        }
+  }
+  bars->lsum[warp][lane] = lsum;                             // bias gradient: channel sums of lo, fixed order
+  consumers_sync();
+  if (warp == 0) {
+    float s = 0.f;
+    for (int w = 0; w < kConsumers; ++w) s += bars->lsum[w][lane];
+    out[(kTaps * 32) * kLoCh + lane] = s;
+  }
 }
 
 // ==========================================================================================
@@ -583,69 +352,49 @@ conv_down32_ts_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
 // The nine shifted operand tiles of the up convolution overlap almost completely, so instead of
 // nine TMA loads per 128 positions ONE tile with a row halo [TB images][(TR+2) rows][W cols][32 ch] is
 // loaded per tile (box start row i0-1: the rows above / below the image are TMA out-of-bounds fill).
-// The 128 MMA rows enumerate the TB*TR*W valid pixels (all 128 for the layers of the networks), so
-// the operand of shift (di,dj) is the resident pixel (row + di, col + dj): the split warps read it
-// (un-swizzling by the absolute row index; a column shift that leaves the image row yields zero),
-// split hi/lo and tcgen05.st the planes to TMEM.  (Round 1 enumerated a column-padded grid instead:
-// 112 / 64 / 48 useful rows of 128 at W = 16 / 8 / 4 and a ragged third tile per 16-row image.)
-// L2->smem traffic drops 9x, and the kernel becomes MMA-bound: per output phase N = 32, three MMAs per
-// K slice (hi*hi, hi*lo, lo*hi), weights 128 KB resident.  (The image-boundary layer, CH in {1,3}, is
-// not a tensor-core problem: dv_conv_img.cu.)
+// The 128 MMA rows enumerate the TB*TR*W valid lo pixels, so the operand of shift (di,dj) is the resident
+// pixel (row + di, col + dj) (a column shift that leaves the image row yields zero).  Shift (di,dj) feeds the
+// output phase (ph,pw) through tap (ph+1-2di, pw+1-2dj) when that tap exists: four accumulators of N = 32 per
+// row, one per phase, weights 128 KB resident.  (The image-boundary layer, CH in {1,3}, is not a tensor-core
+// problem: dv_conv_img.cu.)
 // ==========================================================================================
 constexpr int kHaloStageBytes = 26 * 1024;      // 208 pixel rows: the largest box of the supported geometries is 192 px
 constexpr int kHaloStages = 3;
 struct HaloGeom {
   int B, H, W, TR, TB, tiles_per_img, num_tiles, valid_rows, box_px, box_bytes;
-  int pipe;             // see DownGeom::pipe
-  int debug;            // DV_TC_DEBUG (timing experiments only, results are WRONG): 1 = issue 1 of the 3 MMAs per product
 };
 struct HaloBarriers {
   uint64_t raw_full[kHaloStages], raw_empty[kHaloStages];
-  uint64_t a_ready[kTsAStages], a_empty[kTsAStages];
   uint64_t b_full;
-  uint64_t acc_full[2], acc_empty[2];
-  uint32_t tmem_base;
   float bias[32];
 };
-struct HaloCfg {
-  // one 64-row (hi|lo) weight tile per tap, one 32-column accumulator per output phase
-  static constexpr int kBAll = kTaps * kBTap;
-  static constexpr int kEpiBytes = 4 * 4096;                 // per epilogue warp: 32 pixel rows of 128 B (store transposition)
-  static constexpr int kSmem = kBAll + kHaloStages * kHaloStageBytes + kEpiBytes + 1024 + 512;
-  static constexpr int kAccPerPhase = 32;
-};
+constexpr int kHaloSmem = kBBytes + kHaloStages * kHaloStageBytes + 1024 + 1024;
+static_assert(sizeof(HaloBarriers) <= 1024, "barrier block too large");
+static_assert(kHaloSmem <= kSmemMax, "smem");
 
-__global__ void __launch_bounds__(kTsThreads, 1)
-conv_up_halo_ts_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                       const float* __restrict__ bias, const float* __restrict__ mask, float* __restrict__ hi_out,
-                       HaloGeom g, int act, const uint32_t* __restrict__ mask_bits, uint32_t* __restrict__ bits_out) {
-  using C = HaloCfg;
+__global__ void __launch_bounds__(kThreads, 1)
+conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                        const float* __restrict__ bias, const float* __restrict__ mask, float* __restrict__ hi_out,
+                        HaloGeom g, int act, const uint32_t* __restrict__ mask_bits, uint32_t* __restrict__ bits_out) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = align1024(smem_raw);
   uint8_t* Bs = smem;
-  uint8_t* Raw = smem + C::kBAll;
-  uint8_t* Epi = Raw + kHaloStages * kHaloStageBytes;
-  HaloBarriers* bars = reinterpret_cast<HaloBarriers*>(Epi + C::kEpiBytes);
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // provably warp-uniform role index
+  uint8_t* Raw = smem + kBBytes;
+  HaloBarriers* bars = reinterpret_cast<HaloBarriers*>(Raw + kHaloStages * kHaloStageBytes);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kHaloStages; ++s) { mbar_init(&bars->raw_full[s], 1); mbar_init(&bars->raw_empty[s], 9 * 128); }
-    for (int s = 0; s < kTsAStages; ++s) { mbar_init(&bars->a_ready[s], 128); mbar_init(&bars->a_empty[s], 1); }
+    for (int s = 0; s < kHaloStages; ++s) { mbar_init(&bars->raw_full[s], 1); mbar_init(&bars->raw_empty[s], kConsumers); }
     mbar_init(&bars->b_full, 1);
-    for (int a = 0; a < 2; ++a) { mbar_init(&bars->acc_full[a], 1); mbar_init(&bars->acc_empty[a], 128); }
     fence_mbar_init();
   }
   if (threadIdx.x < 32) bars->bias[threadIdx.x] = bias ? bias[threadIdx.x] : 0.f;
-  if (warp == 2) tmem_alloc(&bars->tmem_base, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  if (bars->tmem_base != 0u) __trap();                       // whole TMEM is ours: base column 0 (see the TS kernels)
-  constexpr uint32_t tmem_base = 0u;
 
-  if (warp == 0 && elect_one()) {
+  if (warp == kConsumers) {
+    if (lane != 0) return;
     prefetch_tmap(&tmap_a); prefetch_tmap(&tmap_b);
-    mbar_arrive_expect_tx(&bars->b_full, C::kBAll);
+    mbar_arrive_expect_tx(&bars->b_full, kBBytes);
     for (int tap = 0; tap < kTaps; ++tap) tma_load_2d(Bs + tap * kBTap, &tmap_b, &bars->b_full, 0, tap * 64);
     uint32_t t_seq = 0;
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x, ++t_seq) {
@@ -656,190 +405,111 @@ conv_up_halo_ts_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       mbar_arrive_expect_tx(&bars->raw_full[stage], g.box_bytes);
       tma_load_4d(Raw + stage * kHaloStageBytes, &tmap_a, &bars->raw_full[stage], 0, 0, i0 - 1, b0);
     }
-  } else if (warp == 1 && elect_one()) {      // ONE elected lane runs the whole issue loop (waits included)
-    constexpr uint32_t idescN = umma_idesc_tf32(128, 32);
-    mbar_wait(&bars->b_full, 0);
-    uint32_t n = 0; int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      mbar_wait(&bars->acc_empty[acc], acc_phase ^ 1);
-      tc_fence_after_sync();
-      uint32_t inited = 0;
-      for (int s = 0; s < 9; ++s, ++n) {
-        const int di = s / 3 - 1, dj = s % 3 - 1;
-        const int as = n % kTsAStages;
-        mbar_wait(&bars->a_ready[as], (n / kTsAStages) & 1u);
-        tc_fence_after_sync();
-        const uint32_t a_hi = tmem_base + kTsACol0 + as * 64, a_lo = a_hi + 32;
-        for (int ph = 0; ph < 2; ++ph) {
-          const int kh = ph + 1 - 2 * di;
-          if (kh < 0 || kh > 3) continue;
-          for (int pw = 0; pw < 2; ++pw) {
-            const int kw = pw + 1 - 2 * dj;
-            if (kw < 0 || kw > 3) continue;
-            const int pidx = ph * 2 + pw;
-            const uint32_t d = tmem_base + acc * 128 + pidx * C::kAccPerPhase;
-            const uint64_t b_hi = umma_desc_sw128_kmajor(smem_u32(Bs + (kh * 4 + kw) * kBTap));
-            const uint32_t first = (inited >> pidx) & 1u;
-            inited |= 1u << pidx;
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {
-              umma_tf32_ts_1t(d, a_hi + 8 * k4, b_hi + 2 * k4, idescN, (first | (uint32_t)k4) != 0);
-              umma_tf32_ts_1t(d, a_hi + 8 * k4, b_hi + (4096 >> 4) + 2 * k4, idescN, 1);      // a_hi * b_lo
-              umma_tf32_ts_1t(d, a_lo + 8 * k4, b_hi + 2 * k4, idescN, 1);                    // a_lo * b_hi
-            }
-          }
-        }
-        umma_commit_1t(&bars->a_empty[as]);
-      }
-      umma_commit_1t(&bars->acc_full[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    const int q = warp & 3;
-    const int HH = 2 * g.H, WW = 2 * g.W;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      int b0, i0;
-      if (g.TB > 1) { b0 = tile * g.TB; i0 = 0; } else { b0 = tile / g.tiles_per_img; i0 = (tile % g.tiles_per_img) * g.TR; }
-      const int r = q * 32 + lane, t = r / g.W;
-      const int tb = t / g.TR, rr = t - tb * g.TR;
-      const int b = b0 + tb, i = i0 + rr, j = r - t * g.W;
-      const bool valid = r < g.valid_rows && b < g.B && i < g.H;
-      // ReLU-backward mask of the four output pixels as one bit per channel, fetched BEFORE waiting for the accumulator:
-      // the loads' latency hides behind this tile's MMAs instead of sitting between the TMEM loads and the stores
-      // (masked dgrad launches used to be 1.7x slower than the unmasked forward ones).
-      uint32_t mbits[4] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu};
-      if (mask_bits && valid) {                               // the mask already as one word per pixel: 4 x 4 bytes
-#pragma unroll
-        for (int pidx = 0; pidx < 4; ++pidx)
-          mbits[pidx] = __ldg(mask_bits + (long long)(b * HH + 2 * i + (pidx >> 1)) * WW + 2 * j + (pidx & 1));
-      } else if (mask && valid) {
-#pragma unroll
-        for (int pidx = 0; pidx < 4; ++pidx) {
-          const float* mk = mask + ((long long)(b * HH + 2 * i + (pidx >> 1)) * WW + 2 * j + (pidx & 1)) * 32;
-          uint32_t bits = 0;
-#pragma unroll
-          for (int c4 = 0; c4 < 8; ++c4) {
-            const float4 m4 = ldg4(mk + c4 * 4);
-            bits |= (m4.x > 0.f ? 1u : 0u) << (c4 * 4) | (m4.y > 0.f ? 2u : 0u) << (c4 * 4) |
-                    (m4.z > 0.f ? 4u : 0u) << (c4 * 4) | (m4.w > 0.f ? 8u : 0u) << (c4 * 4);
-          }
-          mbits[pidx] = bits;
-        }
-      }
-      const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
-      const uint32_t epi = smem_u32(Epi) + q * 4096;
-      mbar_wait(&bars->acc_full[acc], acc_phase);
-      tc_fence_after_sync();
-      const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16) + acc * 128;
-#pragma unroll
-      for (int pidx = 0; pidx < 4; ++pidx) {
-        uint32_t r0[32];
-        tmem_ld_32x32b_x32(tbase + pidx * 32, r0);
-        tmem_ld_wait();
-        if (pidx == 3) { tc_fence_before_sync(); mbar_arrive(&bars->acc_empty[acc]); }
-        // bias / activation / mask in registers (lane = lo pixel), then the pixel's 128-byte line goes through this warp's
-        // shared-memory scratch so that EIGHT lanes store one whole line (four full lines per STG.128 instead of 32 partial
-        // ones: the uncoalesced stores kept L1/TEX 83 % busy, r02 ncu)
-        const int ph = pidx >> 1, pw = pidx & 1;
-        const int opix = valid ? (b * HH + 2 * i + ph) * WW + 2 * j + pw : 0;
-        const uint32_t bits = mbits[pidx];
-        uint32_t obits = 0u;
-#pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4) {
-          float v[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            float x = __uint_as_float(r0[c4 * 4 + e]) + bars->bias[c4 * 4 + e];
-            if (act == DV_ACT_RELU) x = fmaxf(x, 0.f);
-            v[e] = ((bits >> (c4 * 4 + e)) & 1u) ? x : 0.f;
-            obits |= (v[e] > 0.f ? 1u : 0u) << (c4 * 4 + e);
-          }
-          sts128(epi + lane * 128 + ((c4 ^ (lane & 7)) << 4), make_float4(v[0], v[1], v[2], v[3]));
-        }
-        if (bits_out && valid) bits_out[opix] = obits;         // [x > 0] of the stored pixel
-        __syncwarp();
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const int pl = 4 * k + (lane >> 3), ch = lane & 7;   // lane -> (pixel of lane pl, 16-byte chunk ch)
-          const float4 t = lds128f(epi + pl * 128 + ((ch ^ (pl & 7)) << 4));
-          const int op = __shfl_sync(0xffffffffu, opix, pl);
-          if ((vmask >> pl) & 1u) *reinterpret_cast<float4*>(hi_out + (long long)op * 32 + ch * 4) = t;
-        }
-        __syncwarp();
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp >= 8) {
-    const int q = warp & 3, grp = (warp - 8) >> 2;
-    const int row = q * 32 + lane;
-    // centre pixel of this MMA row inside the resident box [TB][TR+2][W] (one halo row above and below every image slab)
-    const int rt = row / g.W, rj = row - rt * g.W, rtb = rt / g.TR;
-    const int src0 = min((rtb * (g.TR + 2) + (rt - rtb * g.TR) + 1) * g.W + rj, g.box_px - 1);
-    const bool row_ok = row < g.valid_rows;
-    uint32_t n = 0, t_seq = 0;
-    int prev_stage = -1, prev_as = 0;                         // g.pipe: shifted tile whose TMEM stores are still in flight
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x, ++t_seq) {
-      const int stage = t_seq % kHaloStages;
-      const uint8_t* raw = Raw + stage * kHaloStageBytes;
-      bool waited = false;
-      for (int s = 0; s < 9; ++s, ++n) {
-        if ((int)(n & 1u) != grp) continue;
-        const int di = s / 3 - 1, dj = s % 3 - 1;
-        const int as = n % kTsAStages;
-        if (!waited) { mbar_wait(&bars->raw_full[stage], (t_seq / kHaloStages) & 1u); waited = true; }
-        // source pixel of the resident tile; a column shift that leaves the image row reads the zero padding instead
-        // (the neighbouring row's pixel sits at that address: the rows are stored without column padding)
-        const bool ok = row_ok && (unsigned)(rj + dj) < (unsigned)g.W;
-        const int p = ok ? src0 + di * g.W + dj : src0;
-        const uint32_t keep = ok ? 0xffffffffu : 0u;
-        uint32_t h[32], l[32];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const uint4 v = lds128(raw + p * 128 + ((c ^ (p & 7)) << 4));
-          const uint32_t vv[4] = {v.x & keep, v.y & keep, v.z & keep, v.w & keep};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const uint32_t hb = vv[e] & kHiMask;
-            h[c * 4 + e] = hb;
-            l[c * 4 + e] = __float_as_uint(__uint_as_float(vv[e]) - __uint_as_float(hb));
-          }
-        }
-        if (g.pipe && prev_stage >= 0) {                      // publish the previous shifted tile (its stores overlapped this split)
-          tmem_st_wait();
-          mbar_arrive(&bars->raw_empty[prev_stage]);
-          tc_fence_before_sync();
-          mbar_arrive(&bars->a_ready[prev_as]);
-        }
-        mbar_wait(&bars->a_empty[as], ((n / kTsAStages) & 1u) ^ 1u);
-        tc_fence_after_sync();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + kTsACol0 + as * 64;
-        tmem_st_32x32b_x32(taddr, h);
-        tmem_st_32x32b_x32(taddr + 32, l);
-        if (g.pipe) { prev_stage = stage; prev_as = as; continue; }
-        tmem_st_wait();
-        // Release the halo tile only now: the tcgen05.st above consumed every loaded value, so the shared-memory
-        // reads have certainly completed (an arrive issued right after the loads can overtake them and let the
-        // next TMA overwrite the tile under the reader).  9 x 128 arrivals free the stage.
-        mbar_arrive(&bars->raw_empty[stage]);
-        tc_fence_before_sync();
-        mbar_arrive(&bars->a_ready[as]);
-      }
-    }
-    if (prev_stage >= 0) {
-      tmem_st_wait();
-      mbar_arrive(&bars->raw_empty[prev_stage]);
-      tc_fence_before_sync();
-      mbar_arrive(&bars->a_ready[prev_as]);
-    }
+    return;
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after_sync(); tmem_dealloc(tmem_base, 512); }
+
+  const int gq = lane >> 2, t = lane & 3;
+  const int HH = 2 * g.H, WW = 2 * g.W;
+  const uint32_t bs = smem_u32(Bs), raw0 = smem_u32(Raw);
+  // the two MMA rows of this thread (r = 16*warp + gq + 8h): centre pixel inside the resident box [TB][TR+2][W]
+  int rj[2], src0[2];
+  bool row_ok[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = warp * 16 + gq + 8 * h;
+    const int rt = row / g.W, rtb = rt / g.TR;
+    rj[h] = row - rt * g.W;
+    src0[h] = min((rtb * (g.TR + 2) + (rt - rtb * g.TR) + 1) * g.W + rj[h], g.box_px - 1);
+    row_ok[h] = row < g.valid_rows;
+  }
+  mbar_wait(&bars->b_full, 0);
+  uint32_t t_seq = 0;
+  for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x, ++t_seq) {
+    const int stage = t_seq % kHaloStages;
+    const uint32_t a_base = raw0 + stage * kHaloStageBytes;
+    mbar_wait(&bars->raw_full[stage], (t_seq / kHaloStages) & 1u);
+    int b0, i0;
+    if (g.TB > 1) { b0 = tile * g.TB; i0 = 0; } else { b0 = tile / g.tiles_per_img; i0 = (tile % g.tiles_per_img) * g.TR; }
+    // one output phase (ph, pw) at a time: its four (shift, tap) products, hi*hi added to the fp32 total after every
+    // shift, the correction products in their own accumulator
+#pragma unroll 1
+    for (int pidx = 0; pidx < 4; ++pidx) {
+      const int ph = pidx >> 1, pw = pidx & 1;
+      float tot[4][4] = {}, corr[4][4] = {};
+#pragma unroll
+      for (int s = 0; s < 9; ++s) {
+        const int di = s / 3 - 1, dj = s % 3 - 1;
+        const int kh = ph + 1 - 2 * di, kw = pw + 1 - 2 * dj;
+        if (kh < 0 || kh > 3 || kw < 0 || kw > 3) continue;
+        const uint32_t b_base = bs + (kh * 4 + kw) * kBTap;
+        int p[2];
+        uint32_t keep[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const bool ok = row_ok[h] && (unsigned)(rj[h] + dj) < (unsigned)g.W;
+          p[h] = ok ? src0[h] + di * g.W + dj : src0[h];
+          keep[h] = ok ? 0xffffffffu : 0u;
+        }
+        float mn[4][4] = {};
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+          uint32_t ah[4], al[4];
+          split_tf32(lds32(a_base + swz128(p[0], 8 * ks + t)) & keep[0], ah[0], al[0]);
+          split_tf32(lds32(a_base + swz128(p[1], 8 * ks + t)) & keep[1], ah[1], al[1]);
+          split_tf32(lds32(a_base + swz128(p[0], 8 * ks + t + 4)) & keep[0], ah[2], al[2]);
+          split_tf32(lds32(a_base + swz128(p[1], 8 * ks + t + 4)) & keep[1], ah[3], al[3]);
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt) {
+            uint32_t bh[2], bl[2];
+            load_b_tap(b_base, nt, ks, gq, t, bh, bl);
+            mma_3xtf32(mn[nt], corr[nt], ah, al, bh, bl);
+          }
+        }
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) tot[nt][e] += mn[nt][e];
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = warp * 16 + gq + 8 * h, tr = r / g.W;
+        const int tb = tr / g.TR, rr = tr - tb * g.TR;
+        const int b = b0 + tb, i = i0 + rr, j = r - tr * g.W;
+        const bool valid = r < g.valid_rows && b < g.B && i < g.H;
+        const long long opix = valid ? ((long long)(b * HH + 2 * i + ph) * WW + 2 * j + pw) : 0;
+        uint32_t mb = 0xffffffffu;
+        if (mask_bits && valid) mb = __ldg(mask_bits + opix);
+        const float* mk = (mask && !mask_bits && valid) ? mask + opix * 32 : nullptr;
+        uint32_t ob = 0u;
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+          const int c = nt * 8 + 2 * t;
+          float v[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float x = (tot[nt][2 * h + e] + corr[nt][2 * h + e]) + bars->bias[c + e];
+            if (act == DV_ACT_RELU) x = fmaxf(x, 0.f);
+            v[e] = ((mb >> (c + e)) & 1u) ? x : 0.f;
+          }
+          if (mk) {
+            const float2 m2 = __ldg(reinterpret_cast<const float2*>(mk + c));
+            v[0] = m2.x > 0.f ? v[0] : 0.f; v[1] = m2.y > 0.f ? v[1] : 0.f;
+          }
+          if (valid) *reinterpret_cast<float2*>(hi_out + opix * 32 + c) = make_float2(v[0], v[1]);
+          ob |= (v[0] > 0.f ? 1u : 0u) << c | (v[1] > 0.f ? 1u : 0u) << (c + 1);
+        }
+        ob |= __shfl_xor_sync(0xffffffffu, ob, 1);
+        ob |= __shfl_xor_sync(0xffffffffu, ob, 2);
+        if (bits_out && valid && t == 0) bits_out[opix] = ob;  // [x > 0] of the stored pixel
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars->raw_empty[stage]);
+  }
 }
 
 // ---- weight packing for the tensor-core kernels ------------------------------------------
-// w[cl][c][tap] ->  down: Wd[tap][row][c],  row <  32: tf32-exact hi of w[row][c][tap], row >= 32: lo
+// w[cl][c][tap] ->  down: Wd[tap][row][c],  row <  32: hi (nearest tf32) of w[row][c][tap], row >= 32: lo
 //                   up  : Wu[tap][row][cl], row <  32: hi of w[cl][row][tap],          row >= 32: lo
 // wf != NULL: the same launch also writes the two CUDA-core layouts of conv_pack_kernel (dv_conv.cu): Wd[tap*32+c][cl]
 // and Wu[tap][cl][c] -- the fallbacks for geometries the tensor-core kernels do not take.
@@ -853,8 +523,8 @@ __global__ void conv_pack_tc_kernel(const float* __restrict__ w, float* __restri
       wf[(tap * 32 + c) * kLoCh + cl] = v;
       wf[n + (tap * kLoCh + cl) * 32 + c] = v;
     }
-    const float hi = __uint_as_float(__float_as_uint(v) & kHiMask);
-    const float lo = v - hi;
+    const float hi = tf32_round(v);
+    const float lo = tf32_round(v - hi);
     wd[(tap * 64 + cl) * 32 + c] = hi;
     wd[(tap * 64 + 32 + cl) * 32 + c] = lo;
     wu[(tap * 64 + c) * 32 + cl] = hi;
@@ -863,8 +533,8 @@ __global__ void conv_pack_tc_kernel(const float* __restrict__ w, float* __restri
 }
 
 // every conv layer of a network node in ONE launch (blockIdx.y = layer): the CH == 32 layers get the four layouts of
-// conv_pack_tc_kernel at wp + {0 (CUDA-core), 32768 (tcgen05 down), 65536 (tcgen05 up)}, the image-boundary layers
-// (CH in {1,3}) the two layouts of conv_pack_kernel (dv_conv.cu): Wd[tap*CH + c][cl] and Wu[tap][c][cl]
+// conv_pack_tc_kernel at wp + {0 (CUDA-core), 32768 (tensor-core down), 65536 (tensor-core up)}, the image-boundary
+// layers (CH in {1,3}) the two layouts of conv_pack_kernel (dv_conv.cu): Wd[tap*CH + c][cl] and Wu[tap][c][cl]
 constexpr int kPackMultiMax = 8;
 struct ConvPackTable {
   const float* w[kPackMultiMax];
@@ -884,8 +554,8 @@ __global__ void conv_pack_multi_kernel(ConvPackTable tab) {
     wp[n + (tap * kLoCh + cl) * 32 + c] = v;
     float* wd = wp + 2 * n;
     float* wu = wd + kTaps * 64 * 32;
-    const float hi = __uint_as_float(__float_as_uint(v) & kHiMask);
-    const float lo = v - hi;
+    const float hi = tf32_round(v);
+    const float lo = tf32_round(v - hi);
     wd[(tap * 64 + cl) * 32 + c] = hi;
     wd[(tap * 64 + 32 + cl) * 32 + c] = lo;
     wu[(tap * 64 + c) * 32 + cl] = hi;
@@ -894,14 +564,6 @@ __global__ void conv_pack_multi_kernel(ConvPackTable tab) {
 }
 
 // ---- host side ---------------------------------------------------------------------------
-static int use_debug() {
-  static const int v = env_int("DV_TC_DEBUG", 0);
-  return v;
-}
-static int use_pipe() {
-  static const int v = env_switch("DV_TC_PIPE", 1);
-  return v;
-}
 static int use_prefetch() {
   static const int v = env_switch("DV_TC_PREFETCH", 1);
   return v;
@@ -924,9 +586,8 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-// NHWC activation [B][HH][WW][32] fp32; box = {32, bw, bh, bb} traversed with element strides {1, sw, sh, 1}
-static bool make_act_tmap(CUtensorMap* m, const float* base, int B, int HH, int WW, int bw, int bh, int bb, int stride,
-                          CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+// NHWC activation [B][HH][WW][32] fp32; box = {32, bw, bh, bb} traversed with element strides {1, sw, sh, 1}, 128-byte swizzle
+static bool make_act_tmap(CUtensorMap* m, const float* base, int B, int HH, int WW, int bw, int bh, int bb, int stride) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return false;
   cuuint64_t gdim[4] = {32, (cuuint64_t)WW, (cuuint64_t)HH, (cuuint64_t)B};
@@ -934,7 +595,7 @@ static bool make_act_tmap(CUtensorMap* m, const float* base, int B, int HH, int 
   cuuint32_t box[4] = {32, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bb};
   cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
   return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), gdim, gstr, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 // packed weights [16*64 rows][32] fp32, box = one tap (64 rows)
@@ -968,14 +629,14 @@ int pack_tc(const float* w, float* wd, float* wu, float* wf, cudaStream_t st) {
 
 // lo[B,H,W,32] = act(down(hi[B,2H,2W,32]) + bias) * [mask > 0]
 // colsum_part != NULL: the kernel also leaves per-CTA channel sums of `lo` in colsum_part[grid][32] and sets
-// *nparts = grid (0 when the selected variant cannot do it: the caller then sums `lo` separately).
+// *nparts = grid.
 int conv_down32_tc(const float* hi, const float* wd_packed, const float* bias, const float* mask, float* lo,
                    int B, int H, int W, int act, cudaStream_t st, float* colsum_part, int* nparts,
                    const uint32_t* mask_bits, uint32_t* bits_out) {
   if (nparts) *nparts = 0;
   if (W > 128 || 128 % W != 0) return DV_ERR_BAD_SHAPE;
   DownGeom g = {};
-  g.B = B; g.H = H; g.W = W; g.prefetch = use_prefetch(); g.pipe = use_pipe(); g.debug = use_debug();
+  g.B = B; g.H = H; g.W = W; g.prefetch = use_prefetch();
   g.rows_per_tile = 128 / W;
   const int TR = g.rows_per_tile < H ? g.rows_per_tile : H;
   if (H % TR != 0 || g.rows_per_tile % TR != 0) return DV_ERR_BAD_SHAPE;
@@ -986,32 +647,11 @@ int conv_down32_tc(const float* hi, const float* wd_packed, const float* bias, c
   if (!make_act_tmap(&ta, hi, B, 2 * H, 2 * W, 2 * W, 2 * TR, TB, 2)) return DV_ERR_CUDA;
   if (!make_w_tmap(&tb, wd_packed)) return DV_ERR_CUDA;
   static bool attr = false;
-  if (!attr) {
-    if (cudaFuncSetAttribute(conv_down32_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTsSmemBytes) != cudaSuccess) {
-      g_last_cuda_error = (int)cudaGetLastError();
-      return DV_ERR_CUDA;
-    }
-    attr = true;
-  }
+  const int rc = set_max_dynamic_smem(conv_down32_mma_kernel, kDownSmem, &attr);
+  if (rc != DV_OK) return rc;
   const int grid = g.num_tiles < kNumSMs ? g.num_tiles : kNumSMs;
-  conv_down32_ts_kernel<<<grid, kTsThreads, kTsSmemBytes, st>>>(ta, tb, bias, mask, lo, g, act, colsum_part, mask_bits, bits_out);
+  conv_down32_mma_kernel<<<grid, kThreads, kDownSmem, st>>>(ta, tb, bias, mask, lo, g, act, colsum_part, mask_bits, bits_out);
   if (nparts && colsum_part) *nparts = grid;
-  return check_launch();
-}
-
-int wgrad32_tc_max_splits() { return kNumSMs; }
-
-template <int GPC>
-static int launch_wgrad_ts(const CUtensorMap& thi, const CUtensorMap& tlo, float* ws, WtGeom g, int grid, cudaStream_t st) {
-  static bool attr = false;
-  if (!attr) {
-    if (cudaFuncSetAttribute(conv_wgrad32_ts_kernel<GPC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWtSmemBytes) != cudaSuccess) {
-      g_last_cuda_error = (int)cudaGetLastError();
-      return DV_ERR_CUDA;
-    }
-    attr = true;
-  }
-  conv_wgrad32_ts_kernel<GPC><<<dim3(grid, 4 / GPC), kWtThreads, kWtSmemBytes, st>>>(thi, tlo, ws, g);
   return check_launch();
 }
 
@@ -1025,42 +665,17 @@ int conv_wgrad32_tc(const float* lo, const float* hi, float* ws, int B, int H, i
   if (H % TR != 0 || g.rows_per_tile % TR != 0) return DV_ERR_BAD_SHAPE;
   const int TB = g.rows_per_tile / TR;
   g.num_tiles = (int)(((long long)B * H * W + 127) / 128);
-  // (tile group, kernel-row group) decomposition: big layers keep all four kernel rows in one CTA (one pass over the
-  // tiles); small layers spread the rows over blockIdx.y so that every CTA still streams >= 8 tiles
-  static const int split_rows = env_switch("DV_WG_PAIRSPLIT", 1);
-  int gpc = 4, grid = 1;
-  for (;; gpc >>= 1) {
-    const int gmax = kNumSMs / (4 / gpc);
-    grid = g.num_tiles < gmax ? g.num_tiles : gmax;
-    g.tiles_per_cta = (g.num_tiles + grid - 1) / grid;
-    if (g.tiles_per_cta >= 8 || gpc == 1 || !split_rows) break;
-  }
-  grid = (g.num_tiles + g.tiles_per_cta - 1) / g.tiles_per_cta;
+  int grid = g.num_tiles < kNumSMs ? g.num_tiles : kNumSMs;
+  g.tiles_per_cta = (g.num_tiles + grid - 1) / grid;
+  grid = (g.num_tiles + g.tiles_per_cta - 1) / g.tiles_per_cta;   // no empty CTA
   *nsplit = grid;
   CUtensorMap thi, tlo;
-  if (!make_act_tmap(&thi, hi, B, 2 * H, 2 * W, 2 * W, 2 * TR, TB, 2, CU_TENSOR_MAP_SWIZZLE_NONE)) return DV_ERR_CUDA;
-  if (!make_act_tmap(&tlo, lo, B, H, W, W, TR, TB, 1, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return DV_ERR_CUDA;
-  if (gpc == 4) return launch_wgrad_ts<4>(thi, tlo, ws, g, grid, st);
-  if (gpc == 2) return launch_wgrad_ts<2>(thi, tlo, ws, g, grid, st);
-  return launch_wgrad_ts<1>(thi, tlo, ws, g, grid, st);
-}
-
-
-static int launch_up_halo(const float* lo, const float* wu, const float* bias, const float* mask, float* hi,
-                          HaloGeom g, int act, cudaStream_t st, const uint32_t* mask_bits, uint32_t* bits_out) {
-  CUtensorMap ta, tb;
-  if (!make_act_tmap(&ta, lo, g.B, g.H, g.W, g.W, g.TR + 2, g.TB, 1)) return DV_ERR_CUDA;
-  if (!make_w_tmap(&tb, wu)) return DV_ERR_CUDA;
+  if (!make_act_tmap(&thi, hi, B, 2 * H, 2 * W, 2 * W, 2 * TR, TB, 2)) return DV_ERR_CUDA;
+  if (!make_act_tmap(&tlo, lo, B, H, W, W, TR, TB, 1)) return DV_ERR_CUDA;
   static bool attr = false;
-  if (!attr) {
-    if (cudaFuncSetAttribute(conv_up_halo_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HaloCfg::kSmem) != cudaSuccess) {
-      g_last_cuda_error = (int)cudaGetLastError();
-      return DV_ERR_CUDA;
-    }
-    attr = true;
-  }
-  const int grid = g.num_tiles < kNumSMs ? g.num_tiles : kNumSMs;
-  conv_up_halo_ts_kernel<<<grid, kTsThreads, HaloCfg::kSmem, st>>>(ta, tb, bias, mask, hi, g, act, mask_bits, bits_out);
+  const int rc = set_max_dynamic_smem(conv_wgrad32_mma_kernel, kWtSmem, &attr);
+  if (rc != DV_OK) return rc;
+  conv_wgrad32_mma_kernel<<<grid, kThreads, kWtSmem, st>>>(thi, tlo, ws, g);
   return check_launch();
 }
 
@@ -1068,7 +683,7 @@ static int launch_up_halo(const float* lo, const float* wu, const float* bias, c
 int conv_up_halo(const float* lo, const float* wu, const float* bias, const float* mask, float* hi,
                  int B, int H, int W, int act, cudaStream_t st, const uint32_t* mask_bits, uint32_t* bits_out) {
   HaloGeom g = {};
-  g.B = B; g.H = H; g.W = W; g.pipe = use_pipe(); g.debug = use_debug();
+  g.B = B; g.H = H; g.W = W;
   if (W > 32 || 128 % W != 0) return DV_ERR_BAD_SHAPE;
   // 128 MMA rows = 128 / W image rows of W pixels: whole rows of one image (TB = 1) or whole small images (TB > 1)
   const int rpt = 128 / W;
@@ -1087,7 +702,15 @@ int conv_up_halo(const float* lo, const float* wu, const float* bias, const floa
   g.box_px = g.TB * (g.TR + 2) * W;
   g.box_bytes = g.box_px * 128;
   if (g.box_bytes > kHaloStageBytes) return DV_ERR_BAD_SHAPE;
-  return launch_up_halo(lo, wu, bias, mask, hi, g, act, st, mask_bits, bits_out);
+  CUtensorMap ta, tb;
+  if (!make_act_tmap(&ta, lo, g.B, g.H, g.W, g.W, g.TR + 2, g.TB, 1)) return DV_ERR_CUDA;
+  if (!make_w_tmap(&tb, wu)) return DV_ERR_CUDA;
+  static bool attr = false;
+  const int rc = set_max_dynamic_smem(conv_up_halo_mma_kernel, kHaloSmem, &attr);
+  if (rc != DV_OK) return rc;
+  const int grid = g.num_tiles < kNumSMs ? g.num_tiles : kNumSMs;
+  conv_up_halo_mma_kernel<<<grid, kThreads, kHaloSmem, st>>>(ta, tb, bias, mask, hi, g, act, mask_bits, bits_out);
+  return check_launch();
 }
 
 }  // namespace tc

@@ -1,16 +1,14 @@
-// tcgen05 GEMM for the fully connected layers (encoder/decoder MLPs and the FactorVAE discriminator):
+// Tensor-core GEMMs for the fully connected layers (encoder/decoder MLPs and the FactorVAE discriminator):
 //     C[M, Nout] = epilogue( A[M, R] . Bw[Nout, R]^T )          (both operands K-major = R contiguous)
 // used for the forward pass (A = activations, Bw = weight [N, K], bias + ReLU/LeakyReLU epilogue) and for the
-// input gradient (A = upstream gradient [M, N], Bw = weight transposed [K, N], activation-gradient mask epilogue).
-// Replaces nn.Linear + activation (disvae/models/encoders.py:81-86, decoders.py:71-73, discriminator.py:63-68)
-// and the dgrad half of their autograd backward.
+// input gradient (A = upstream gradient [M, N], Bw = weight transposed [K, N], activation-gradient mask epilogue),
+// and the weight gradient dW = G^T . X further down.  Replaces nn.Linear + activation
+// (disvae/models/encoders.py:81-86, decoders.py:71-73, discriminator.py:63-68) and their autograd backward.
 //
-// Error-compensated 3xTF32 like the convolutions: the weight is split once by a pack kernel into tf32-exact hi
-// and residual lo planes (plus the transposed copy for dgrad); the activation tile is split on the fly by the
-// split warps into TMEM.  Per 32-wide K block and K=8 slice: one MMA  a_hi x [b_hi | b_lo]  (N = 2*BN) and one
-// a_lo x b_hi (N = BN); the two accumulator halves are added in the epilogue.
-//   CTA tile 128 x 64, grid = ceil(M/128) x ceil(Nout/64); 6-stage TMA ring of {A raw 16 KB, B hi 8 KB, B lo 8 KB};
-//   warp 0 TMA, warp 1 MMA, warp 2 TMEM alloc, warps 4-7 epilogue, warps 8-15 two split groups.
+// Error-compensated 3xTF32 like the convolutions (dv_ptx.cuh): the weight is split once by a pack kernel into tf32
+// hi and residual lo planes (plus the transposed copy for dgrad); the activation fragments are split in registers.
+//   CTA tile 128 x 64, grid = ceil(M/128) x ceil(Nout/64); 4-stage TMA ring of {A raw 16 KB, B hi 8 KB, B lo 8 KB};
+//   warps 0-7 (4 x 2, 32 x 32 each) issue mma.sync m16n8k8 and run the epilogue, warp 8 is the TMA producer.
 //   Row / column / K tails are handled by TMA out-of-bounds zero fill and guarded stores.
 #include "dv_common.cuh"
 #include "dv_ptx.cuh"
@@ -23,23 +21,18 @@ namespace ltc {
 using namespace ptx;
 
 constexpr int kBM = 128, kBN = 64, kBK = 32;
-constexpr int kThreads = 512;
-constexpr int kStages = 6;
+constexpr int kConsumers = 8;
+constexpr int kThreads = (kConsumers + 1) * 32;
+constexpr int kStages = 4;
 constexpr int kATile = kBM * 128;                 // 16 KB raw activation tile
 constexpr int kBTile = kBN * 128;                 // 8 KB per weight plane tile
 constexpr int kStageBytes = kATile + 2 * kBTile;  // 32 KB
-constexpr int kAStages = 4;                       // TMEM A stages (hi 32 | lo 32 columns each)
-constexpr int kACol0 = 256;
-constexpr uint32_t kHiMask = 0xFFFFE000u;
 
 struct Barriers {
-  uint64_t full[kStages], a_consumed[kStages], b_consumed[kStages];
-  uint64_t a_ready[kAStages], a_empty[kAStages];
-  uint64_t acc_full;
-  uint32_t tmem_base;
+  uint64_t full[kStages], empty[kStages];
 };
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 512;
-static_assert(sizeof(Barriers) <= 512, "barriers");
+constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
+static_assert(sizeof(Barriers) <= 256, "barriers");
 
 struct Epilogue {
   const float* bias;       // [Nout] or null
@@ -48,184 +41,233 @@ struct Epilogue {
   float slope;
 };
 
+
 __global__ void __launch_bounds__(kThreads, 1)
-linear_nt_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_bhi,
-                    const __grid_constant__ CUtensorMap tmap_blo, float* __restrict__ C, int M, int Nout, int R,
-                    Epilogue ep) {
+linear_nt_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_bhi,
+                     const __grid_constant__ CUtensorMap tmap_blo, float* __restrict__ C, int M, int Nout, int R,
+                     Epilogue ep) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = align1024(smem_raw);
   Barriers* bars = reinterpret_cast<Barriers*>(smem + kStages * kStageBytes);
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // provably warp-uniform role index
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * kBM, n0 = blockIdx.y * kBN;
   const int nkb = (R + kBK - 1) / kBK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(&bars->full[s], 1); mbar_init(&bars->a_consumed[s], 128); mbar_init(&bars->b_consumed[s], 1); }
-    for (int s = 0; s < kAStages; ++s) { mbar_init(&bars->a_ready[s], 128); mbar_init(&bars->a_empty[s], 1); }
-    mbar_init(&bars->acc_full, 1);
+    for (int s = 0; s < kStages; ++s) { mbar_init(&bars->full[s], 1); mbar_init(&bars->empty[s], kConsumers); }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(&bars->tmem_base, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  if (bars->tmem_base != 0u) __trap();                       // 1 CTA/SM owns the whole tensor memory
-  constexpr uint32_t tmem_base = 0u;
 
-  if (warp == 0 && elect_one()) {
-    // ---- TMA producer: {A raw, B hi, B lo} of one K block per stage ----
+  if (warp == kConsumers) {
+    if (lane != 0) return;
     prefetch_tmap(&tmap_a); prefetch_tmap(&tmap_bhi); prefetch_tmap(&tmap_blo);
     for (int kb = 0; kb < nkb; ++kb) {
       const int stage = kb % kStages;
-      const uint32_t par = ((kb / kStages) & 1u) ^ 1u;
-      mbar_wait(&bars->a_consumed[stage], par);              // split warps are done with the raw A tile
-      mbar_wait(&bars->b_consumed[stage], par);              // MMAs that read the B tiles have completed
+      mbar_wait(&bars->empty[stage], ((kb / kStages) & 1u) ^ 1u);
       uint8_t* st = smem + stage * kStageBytes;
       mbar_arrive_expect_tx(&bars->full[stage], kStageBytes);
       tma_load_2d(st, &tmap_a, &bars->full[stage], kb * kBK, m0);
       tma_load_2d(st + kATile, &tmap_bhi, &bars->full[stage], kb * kBK, n0);
       tma_load_2d(st + kATile + kBTile, &tmap_blo, &bars->full[stage], kb * kBK, n0);
     }
-  } else if (warp == 1 && elect_one()) {      // ONE elected lane runs the whole issue loop (barrier waits included):
-                                              // ptxas then keeps every MMA operand in uniform registers (back-to-back UTCHMMA)
-    // ---- MMA issuer (whole warp, one elected lane issues) ----
-    constexpr uint32_t idesc2 = umma_idesc_tf32(128, 2 * kBN), idesc1 = umma_idesc_tf32(128, kBN);
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int stage = kb % kStages, as = kb % kAStages;
-      mbar_wait(&bars->full[stage], (kb / kStages) & 1u);    // B tiles landed (A raw too)
-      mbar_wait(&bars->a_ready[as], (kb / kAStages) & 1u);   // A hi/lo in TMEM
-      tc_fence_after_sync();
-      const uint32_t a_hi = tmem_base + kACol0 + as * 64, a_lo = a_hi + 32;
-      const uint64_t b_d = umma_desc_sw128_kmajor(smem_u32(smem + stage * kStageBytes + kATile));   // [b_hi (64 rows) | b_lo (64 rows)]
-#pragma unroll
-      for (int k4 = 0; k4 < 4; ++k4) {
-        // two accumulation chains (even / odd K slices): the tensor core truncates when it accumulates, shorter
-        // chains keep the result fp32-grade.  Chain c: cols [128c, 128c+64) hi*hi + lo*hi, [128c+64, 128c+128) hi*lo.
-        const uint32_t d = tmem_base + (k4 & 1) * 128;
-        umma_tf32_ts_1t(d, a_hi + 8 * k4, b_d + 2 * k4, idesc2, (kb | (k4 >> 1)) != 0);
-        umma_tf32_ts_1t(d, a_lo + 8 * k4, b_d + 2 * k4, idesc1, 1);
-      }
-      umma_commit_1t(&bars->a_empty[as]);
-      umma_commit_1t(&bars->b_consumed[stage]);
-    }
-    umma_commit_1t(&bars->acc_full);
-  } else if (warp >= 4 && warp < 8) {
-    // ---- epilogue: thread = output row ----
-    const int q = warp & 3;
-    const int m = m0 + q * 32 + lane;
-    mbar_wait(&bars->acc_full, 0);
-    tc_fence_after_sync();
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-    for (int half = 0; half < 2; ++half) {
-      uint32_t r0[32], r1[32];
-      float acc[32];
-      tmem_ld_32x32b_x32(taddr + half * 32, r0);             // chain 0: hi*hi + lo*hi
-      tmem_ld_32x32b_x32(taddr + kBN + half * 32, r1);       //          hi*lo
-      tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < 32; ++c) acc[c] = __uint_as_float(r0[c]) + __uint_as_float(r1[c]);
-      tmem_ld_32x32b_x32(taddr + 128 + half * 32, r0);       // chain 1
-      tmem_ld_32x32b_x32(taddr + 128 + kBN + half * 32, r1);
-      tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < 32; ++c) acc[c] += __uint_as_float(r0[c]) + __uint_as_float(r1[c]);
-      if (m < M) {
-        const int nb = n0 + half * 32;
-        float* crow = C + (long long)m * Nout;
-        const float* mrow = ep.mask_src ? ep.mask_src + (long long)m * Nout : nullptr;
-        if ((Nout & 3) == 0) {
-          // 16-byte path: each thread writes 128 contiguous bytes of its row
-#pragma unroll
-          for (int c4 = 0; c4 < 8; ++c4) {
-            const int n = nb + c4 * 4;
-            if (n < Nout) {
-              float v[4] = {acc[c4 * 4], acc[c4 * 4 + 1], acc[c4 * 4 + 2], acc[c4 * 4 + 3]};
-              if (mrow) {
-                const float4 y = *reinterpret_cast<const float4*>(mrow + n);
-                const float yy[4] = {y.x, y.y, y.z, y.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  if (ep.act == DV_ACT_RELU) v[e] = yy[e] > 0.f ? v[e] : 0.f;
-                  else if (ep.act == DV_ACT_LEAKY) v[e] = yy[e] > 0.f ? v[e] : v[e] * ep.slope;
-                }
-              } else {
-                if (ep.bias) {
-                  const float4 bb = *reinterpret_cast<const float4*>(ep.bias + n);
-                  v[0] += bb.x; v[1] += bb.y; v[2] += bb.z; v[3] += bb.w;
-                }
-#pragma unroll
-                for (int e = 0; e < 4; ++e) v[e] = apply_act(v[e], ep.act, ep.slope);
-              }
-              *reinterpret_cast<float4*>(crow + n) = make_float4(v[0], v[1], v[2], v[3]);
-            }
-          }
-        } else {
-#pragma unroll
-          for (int c = 0; c < 32; ++c) {
-            const int n = nb + c;
-            if (n < Nout) {
-              float v = acc[c];
-              if (mrow) {
-                const float y = mrow[n];
-                if (ep.act == DV_ACT_RELU) v = y > 0.f ? v : 0.f;
-                else if (ep.act == DV_ACT_LEAKY) v = y > 0.f ? v : v * ep.slope;
-              } else {
-                if (ep.bias) v += ep.bias[n];
-                v = apply_act(v, ep.act, ep.slope);
-              }
-              crow[n] = v;
-            }
-          }
-        }
-      }
-    }
-  } else if (warp >= 8) {
-    // ---- split warps: raw A tile -> hi/lo planes in TMEM (two groups on alternate K blocks) ----
-    const int q = warp & 3, grp = (warp - 8) >> 2;
-    const int row = q * 32 + lane;
-    int prev_stage = -1, prev_as = 0;                         // K block whose TMEM stores are still in flight
-    for (int kb = grp; kb < nkb; kb += 2) {
-      const int stage = kb % kStages, as = kb % kAStages;
-      mbar_wait(&bars->full[stage], (kb / kStages) & 1u);
-      const uint8_t* raw = smem + stage * kStageBytes;
-      uint32_t h[32], l[32];
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        const uint4 v = lds128(raw + row * 128 + ((c ^ (row & 7)) << 4));
-        const uint32_t vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const uint32_t hb = vv[e] & kHiMask;
-          h[c * 4 + e] = hb;
-          l[c * 4 + e] = __float_as_uint(__uint_as_float(vv[e]) - __uint_as_float(hb));
-        }
-      }
-      // software pipeline: the stores of the previous K block overlapped this block's loads and split; publish
-      // it (and release its raw tile -- only after tcgen05.wait::st, when its reads were certainly consumed) now
-      if (prev_stage >= 0) {
-        tmem_st_wait();
-        mbar_arrive(&bars->a_consumed[prev_stage]);
-        tc_fence_before_sync();
-        mbar_arrive(&bars->a_ready[prev_as]);
-      }
-      mbar_wait(&bars->a_empty[as], ((kb / kAStages) & 1u) ^ 1u);
-      tc_fence_after_sync();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + kACol0 + as * 64;
-      tmem_st_32x32b_x32(taddr, h);
-      tmem_st_32x32b_x32(taddr + 32, l);
-      prev_stage = stage; prev_as = as;
-    }
-    if (prev_stage >= 0) {
-      tmem_st_wait();
-      mbar_arrive(&bars->a_consumed[prev_stage]);
-      tc_fence_before_sync();
-      mbar_arrive(&bars->a_ready[prev_as]);
-    }
+    return;
   }
-  tc_fence_before_sync();
+
+  const int gq = lane >> 2, t = lane & 3;
+  const int wm = warp & 3, wn = warp >> 2;                   // rows [32 wm, 32 wm + 32), columns [32 wn, 32 wn + 32)
+  float tot[2][4][4] = {}, corr[2][4][4] = {};
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int stage = kb % kStages;
+    mbar_wait(&bars->full[stage], (kb / kStages) & 1u);
+    const uint32_t a_base = smem_u32(smem + stage * kStageBytes);
+    const uint32_t bh_base = a_base + kATile, bl_base = bh_base + kBTile;
+    float mn[2][4][4] = {};                                  // hi*hi of this K block, added to tot in fp32 below
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      uint32_t ah[2][4], al[2][4], bh[4][2], bl[4][2];
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) {
+        const int r = wm * 32 + mt * 16 + gq;
+        split_tf32(lds32(a_base + swz128(r, 8 * ks + t)), ah[mt][0], al[mt][0]);
+        split_tf32(lds32(a_base + swz128(r + 8, 8 * ks + t)), ah[mt][1], al[mt][1]);
+        split_tf32(lds32(a_base + swz128(r, 8 * ks + t + 4)), ah[mt][2], al[mt][2]);
+        split_tf32(lds32(a_base + swz128(r + 8, 8 * ks + t + 4)), ah[mt][3], al[mt][3]);
+      }
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt) {
+        const int n = wn * 32 + nt * 8 + gq;
+        bh[nt][0] = lds32(bh_base + swz128(n, 8 * ks + t));
+        bh[nt][1] = lds32(bh_base + swz128(n, 8 * ks + t + 4));
+        bl[nt][0] = lds32(bl_base + swz128(n, 8 * ks + t));
+        bl[nt][1] = lds32(bl_base + swz128(n, 8 * ks + t + 4));
+      }
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) mma_3xtf32(mn[mt][nt], corr[mt][nt], ah[mt], al[mt], bh[nt], bl[nt]);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars->empty[stage]);
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) tot[mt][nt][e] += mn[mt][nt][e];
+  }
+
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = m0 + wm * 32 + mt * 16 + gq + 8 * h;
+      if (m >= M) continue;
+      float* crow = C + (long long)m * Nout;
+      const float* mrow = ep.mask_src ? ep.mask_src + (long long)m * Nout : nullptr;
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int n = n0 + wn * 32 + nt * 8 + 2 * t + e;
+          if (n >= Nout) continue;
+          float v = tot[mt][nt][2 * h + e] + corr[mt][nt][2 * h + e];
+          if (mrow) {
+            const float y = mrow[n];
+            if (ep.act == DV_ACT_RELU) v = y > 0.f ? v : 0.f;
+            else if (ep.act == DV_ACT_LEAKY) v = y > 0.f ? v : v * ep.slope;
+          } else {
+            if (ep.bias) v += ep.bias[n];
+            v = apply_act(v, ep.act, ep.slope);
+          }
+          crow[n] = v;
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------
+// weight gradient:  dW[n][k] = sum_m G[m][n] * X[m][k]   (reduction over the batch rows)
+// Both operands come from TMA as [128 batch rows][32 features] tiles (128-byte swizzle), read transposed by the fragment
+// loads: A = G^T (M = 32 output rows n), B = X (N = 64 columns k, warp w owns columns [8w, 8w+8)).  K slot t of an MMA
+// holds batch row 8ks + 2t and slot t + 4 row 8ks + 2t + 1, which keeps the transposed loads free of bank conflicts.
+// A CTA owns one 32 x 64 block of dW and one slice of the batch (deterministic split-K: partials to the workspace,
+// reduced in a fixed order).  Warp 0 also sums the columns of G (bias gradient).
+// ------------------------------------------------------------------------------------------
+constexpr int kWgStages = 3;
+constexpr int kWgStageBytes = 3 * kATile;              // G, X columns [0,32), X columns [32,64)
+struct WgBarriers {
+  uint64_t full[kWgStages], empty[kWgStages];
+};
+constexpr int kWgSmemBytes = kWgStages * kWgStageBytes + 1024 + 256;
+static_assert(sizeof(WgBarriers) <= 256, "barriers");
+static_assert(kWgSmemBytes <= 232448, "smem");
+
+struct WgGeom {
+  int M, N, K;
+  int m_tiles, tiles_per_split;
+};
+
+__global__ void __launch_bounds__(kThreads, 1)
+linear_wgrad_mma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_g,
+                        float* __restrict__ out_base, long long split_stride, float* __restrict__ dbias_base,
+                        long long dbias_stride, WgGeom g) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  WgBarriers* bars = reinterpret_cast<WgBarriers*>(smem + kWgStages * kWgStageBytes);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int ng = blockIdx.x, kg = blockIdx.y, sp = blockIdx.z;
+  const int t_begin = sp * g.tiles_per_split;
+  const int t_end = min(g.m_tiles, t_begin + g.tiles_per_split);
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kWgStages; ++s) { mbar_init(&bars->full[s], 1); mbar_init(&bars->empty[s], kConsumers); }
+    fence_mbar_init();
+  }
   __syncthreads();
-  if (warp == 2) { tc_fence_after_sync(); tmem_dealloc(tmem_base, 512); }
+
+  if (warp == kConsumers) {
+    if (lane != 0) return;
+    prefetch_tmap(&tmap_x); prefetch_tmap(&tmap_g);
+    for (int tile = t_begin, i = 0; tile < t_end; ++tile, ++i) {
+      const int stage = i % kWgStages, m0 = tile * 128;
+      mbar_wait(&bars->empty[stage], ((i / kWgStages) & 1u) ^ 1u);
+      uint8_t* st = smem + stage * kWgStageBytes;
+      mbar_arrive_expect_tx(&bars->full[stage], kWgStageBytes);
+      tma_load_2d(st, &tmap_g, &bars->full[stage], ng * 32, m0);
+      tma_load_2d(st + kATile, &tmap_x, &bars->full[stage], kg * 64, m0);        // columns past K: zero fill
+      tma_load_2d(st + 2 * kATile, &tmap_x, &bars->full[stage], kg * 64 + 32, m0);
+    }
+    return;
+  }
+
+  const int gq = lane >> 2, t = lane & 3;
+  const bool want_bias = dbias_base != nullptr && kg == 0 && warp == 0;   // (every k block sees the same G tiles)
+  float tot[2][4] = {};                                      // [n block][fragment]
+  float bsum[2][2] = {};                                     // G column sums of n = 16 mt + gq + 8 h
+  for (int tile = t_begin, i = 0; tile < t_end; ++tile, ++i) {
+    const int stage = i % kWgStages;
+    mbar_wait(&bars->full[stage], (i / kWgStages) & 1u);
+    const uint32_t g_base = smem_u32(smem + stage * kWgStageBytes);
+    const uint32_t x_base = g_base + kATile + (warp >> 2) * kATile;
+    const int xc = (warp & 3) * 8 + gq;                      // this lane's X column inside its 32-column tile
+    float mn[2][4] = {}, cr[2][4] = {};
+#pragma unroll 4
+    for (int ks = 0; ks < 16; ++ks) {
+      const int r0 = 8 * ks + 2 * t, r1 = r0 + 1;
+      uint32_t ah[2][4], al[2][4], bh[2], bl[2];
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) {
+        const int n = mt * 16 + gq;
+        uint32_t a[4];
+        a[0] = lds32(g_base + swz128(r0, n));
+        a[1] = lds32(g_base + swz128(r0, n + 8));
+        a[2] = lds32(g_base + swz128(r1, n));
+        a[3] = lds32(g_base + swz128(r1, n + 8));
+        if (want_bias) {
+          bsum[mt][0] += __uint_as_float(a[0]) + __uint_as_float(a[2]);
+          bsum[mt][1] += __uint_as_float(a[1]) + __uint_as_float(a[3]);
+        }
+#pragma unroll
+        for (int e = 0; e < 4; ++e) split_tf32(a[e], ah[mt][e], al[mt][e]);
+      }
+      split_tf32(lds32(x_base + swz128(r0, xc)), bh[0], bl[0]);
+      split_tf32(lds32(x_base + swz128(r1, xc)), bh[1], bl[1]);
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) mma_3xtf32(mn[mt], cr[mt], ah[mt], al[mt], bh, bl);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars->empty[stage]);
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) tot[mt][e] += mn[mt][e] + cr[mt][e];
+  }
+
+  float* out = out_base + (long long)sp * split_stride;
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int n = ng * 32 + mt * 16 + gq + 8 * h;
+      if (n >= g.N) continue;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int k = kg * 64 + warp * 8 + 2 * t + e;
+        if (k < g.K) out[(long long)n * g.K + k] = tot[mt][2 * h + e];
+      }
+    }
+  if (want_bias) {                                           // fixed order: the four lanes of a row group, then store
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float s = bsum[mt][h];
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        const int n = ng * 32 + mt * 16 + gq + 8 * h;
+        if (t == 0 && n < g.N) dbias_base[(long long)sp * dbias_stride + n] = s;
+      }
+  }
 }
 
 // w[N][K] -> hi/lo planes.  transpose == 0: [N][Kp] (forward; Kp = K rounded up to 4 floats, TMA pitch is 16-byte);
@@ -241,9 +283,9 @@ __global__ void linear_pack_kernel(const float* __restrict__ w, float* __restric
     if (transpose) {
       tile[r][tx] = v;
     } else if (n < N && k < pitch) {
-      const float hi = __uint_as_float(__float_as_uint(v) & kHiMask);
+      const float hi = tf32_round(v);
       p_hi[(long long)n * pitch + k] = hi;
-      p_lo[(long long)n * pitch + k] = v - hi;
+      p_lo[(long long)n * pitch + k] = tf32_round(v - hi);
     }
   }
   if (!transpose) return;
@@ -252,9 +294,9 @@ __global__ void linear_pack_kernel(const float* __restrict__ w, float* __restric
     const int k = k0 + r, n = n0 + tx;
     if (k < K && n < pitch) {
       const float v = tile[tx][r];
-      const float hi = __uint_as_float(__float_as_uint(v) & kHiMask);
+      const float hi = tf32_round(v);
       p_hi[(long long)k * pitch + n] = hi;
-      p_lo[(long long)k * pitch + n] = v - hi;
+      p_lo[(long long)k * pitch + n] = tf32_round(v - hi);
     }
   }
 }
@@ -289,9 +331,9 @@ __global__ void linear_pack_multi_kernel(PackTable t) {
     const float v = (n < N && k < K) ? w[(long long)n * K + k] : 0.f;
     tile[r][tx] = v;
     if (n < N && k < Kp) {
-      const float hi = __uint_as_float(__float_as_uint(v) & kHiMask);
+      const float hi = tf32_round(v);
       f_hi[(long long)n * Kp + k] = hi;
-      f_lo[(long long)n * Kp + k] = v - hi;
+      f_lo[(long long)n * Kp + k] = tf32_round(v - hi);
     }
   }
   __syncthreads();
@@ -299,9 +341,9 @@ __global__ void linear_pack_multi_kernel(PackTable t) {
     const int k = k0 + r, n = n0 + tx;
     if (k < K && n < Np) {
       const float v = tile[tx][r];
-      const float hi = __uint_as_float(__float_as_uint(v) & kHiMask);
+      const float hi = tf32_round(v);
       t_hi[(long long)k * Np + n] = hi;
-      t_lo[(long long)k * Np + n] = v - hi;
+      t_lo[(long long)k * Np + n] = tf32_round(v - hi);
     }
   }
 }
@@ -322,9 +364,8 @@ static EncodeTiledFn get_encode() {
   }
   return fn;
 }
-// row-major [rows][cols] fp32 with a row pitch of `pitch` floats; box = {32 cols, box_rows}
-static bool make_2d(CUtensorMap* m, const float* base, long long rows, long long cols, long long pitch, int box_rows,
-                    CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+// row-major [rows][cols] fp32 with a row pitch of `pitch` floats; box = {32 cols, box_rows}, 128-byte swizzle
+static bool make_2d(CUtensorMap* m, const float* base, long long rows, long long cols, long long pitch, int box_rows) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return false;
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
@@ -332,7 +373,7 @@ static bool make_2d(CUtensorMap* m, const float* base, long long rows, long long
   cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstr, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
@@ -353,215 +394,11 @@ static int launch_nt(const float* A, long long a_pitch, const float* b_hi, const
   if (!make_2d(&tbh, b_hi, Nout, R, round4(R), kBN)) return DV_ERR_CUDA;
   if (!make_2d(&tbl, b_lo, Nout, R, round4(R), kBN)) return DV_ERR_CUDA;
   static bool attr = false;
-  if (!attr) {
-    if (cudaFuncSetAttribute(linear_nt_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess) {
-      g_last_cuda_error = (int)cudaGetLastError();
-      return DV_ERR_CUDA;
-    }
-    attr = true;
-  }
+  const int rc = set_max_dynamic_smem(linear_nt_mma_kernel, kSmemBytes, &attr);
+  if (rc != DV_OK) return rc;
   dim3 grid((M + kBM - 1) / kBM, (Nout + kBN - 1) / kBN);
-  linear_nt_tc_kernel<<<grid, kThreads, kSmemBytes, st>>>(ta, tbh, tbl, C, M, Nout, R, ep);
+  linear_nt_mma_kernel<<<grid, kThreads, kSmemBytes, st>>>(ta, tbh, tbl, C, M, Nout, R, ep);
   return check_launch();
-}
-
-// ------------------------------------------------------------------------------------------
-// weight gradient:  dW[n][k] = sum_m G[m][n] * X[m][k]   (reduction over the batch rows)
-// Both operands come from TMA as [128 batch rows][32 features] tiles, i.e. with the reduction index along the
-// smem rows -> MN-major tcgen05 operands (32-byte-atom 128B swizzle), no transposition anywhere.  One MMA
-// (M=128, N=64, K=8 rows):  A = [Xa_hi | Xb_hi | Xa_lo | Xb_lo] (two 32-wide k groups of X, hi/lo planes),
-// B = [G_hi | G_lo] (one 32-wide n group): D holds all four hi/lo cross products.  A CTA owns one n group,
-// up to 16 k groups (8 pair accumulators x 64 columns = all of TMEM) and one slice of the batch (deterministic
-// split-K: partials to the workspace, reduced in a fixed order).  Same scheme as the conv weight gradient.
-// ------------------------------------------------------------------------------------------
-constexpr int kWgStages = 2;
-constexpr int kWgStageBytes = 4 * kATile;              // Xa_hi, Xb_hi, Xa_lo, Xb_lo
-constexpr int kWgGBytes = 2 * kATile;                  // G_hi, G_lo
-struct WgBarriers {
-  uint64_t raw_full[kWgStages], ready[kWgStages], empty[kWgStages];
-  uint64_t g_raw_full[2], g_ready[2], g_empty[2];
-  uint64_t acc_full;
-  uint32_t tmem_base;
-  float lscr[128][4];                                    // column sums of G (bias gradient), per split thread
-};
-constexpr int kWgSmemBytes = kWgStages * kWgStageBytes + 2 * kWgGBytes + 1024 + 3072;
-static_assert(sizeof(WgBarriers) <= 3072, "barriers");
-static_assert(kWgSmemBytes <= 232448, "smem");
-
-__device__ __forceinline__ uint64_t umma_desc_sw128_mnmajor(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(512 >> 4) << 32) |
-         (1ull << 46) | (1ull << 61);
-}
-// residual plane lo = v - trunc_tf32(v).  The hi operand is the RAW fp32 tile itself: kind::tf32 reads only the upper
-// 19 bits of each 32-bit element, which is exactly the truncation the mask performs (the fp64-accuracy tests hold this).
-__device__ __forceinline__ void split_lo_only(const uint4* raw, uint4* lo4, int t) {
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const int idx = t + 128 * k;
-    const uint4 v = raw[idx];
-    uint4 l;
-    l.x = __float_as_uint(__uint_as_float(v.x) - __uint_as_float(v.x & kHiMask));
-    l.y = __float_as_uint(__uint_as_float(v.y) - __uint_as_float(v.y & kHiMask));
-    l.z = __float_as_uint(__uint_as_float(v.z) - __uint_as_float(v.z & kHiMask));
-    l.w = __float_as_uint(__uint_as_float(v.w) - __uint_as_float(v.w & kHiMask));
-    lo4[idx] = l;
-  }
-}
-
-struct WgGeom {
-  int M, N, K;
-  int m_tiles, tiles_per_split;
-};
-
-__global__ void __launch_bounds__(kThreads, 1)
-linear_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_g,
-                       float* __restrict__ out_base, long long split_stride, float* __restrict__ dbias_base,
-                       long long dbias_stride, WgGeom g) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* St = smem;                                        // [stage][Xa_hi|Xb_hi|Xa_lo|Xb_lo]
-  uint8_t* Gs = smem + kWgStages * kWgStageBytes;            // [buf][G_hi|G_lo]
-  WgBarriers* bars = reinterpret_cast<WgBarriers*>(Gs + 2 * kWgGBytes);
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // provably warp-uniform role index
-  const int ng = blockIdx.x, kc = blockIdx.y, sp = blockIdx.z;
-  const int kgroups = (g.K + 31) / 32;
-  const int my_groups = min(16, kgroups - kc * 16);
-  const int npairs = (my_groups + 1) / 2;
-  const int t_begin = sp * g.tiles_per_split;
-  const int t_end = min(g.m_tiles, t_begin + g.tiles_per_split);
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kWgStages; ++s) { mbar_init(&bars->raw_full[s], 1); mbar_init(&bars->ready[s], 128); mbar_init(&bars->empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&bars->g_raw_full[s], 1); mbar_init(&bars->g_ready[s], 128); mbar_init(&bars->g_empty[s], 1); }
-    mbar_init(&bars->acc_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == 2) tmem_alloc(&bars->tmem_base, 512);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  if (bars->tmem_base != 0u) __trap();
-  constexpr uint32_t tmem_base = 0u;
-
-  if (warp == 0 && elect_one()) {
-    prefetch_tmap(&tmap_x); prefetch_tmap(&tmap_g);
-    int stage = 0; uint32_t phase = 0; int gb = 0; uint32_t gphase = 0;
-    for (int tile = t_begin; tile < t_end; ++tile) {
-      const int m0 = tile * 128;
-      mbar_wait(&bars->g_empty[gb], gphase ^ 1);
-      mbar_arrive_expect_tx(&bars->g_raw_full[gb], kATile);
-      tma_load_2d(Gs + gb * kWgGBytes, &tmap_g, &bars->g_raw_full[gb], ng * 32, m0);
-      if (++gb == 2) { gb = 0; gphase ^= 1; }
-      for (int pr = 0; pr < npairs; ++pr) {
-        mbar_wait(&bars->empty[stage], phase ^ 1);
-        mbar_arrive_expect_tx(&bars->raw_full[stage], 2 * kATile);
-#pragma unroll
-        for (int h = 0; h < 2; ++h)                          // a k group past the end is all out-of-bounds: zero filled
-          tma_load_2d(St + stage * kWgStageBytes + h * kATile, &tmap_x, &bars->raw_full[stage], (kc * 16 + 2 * pr + h) * 32, m0);
-        if (++stage == kWgStages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1 && elect_one()) {      // ONE elected lane runs the whole issue loop (barrier waits included):
-                                              // ptxas then keeps every MMA operand in uniform registers (back-to-back UTCHMMA)
-    constexpr uint32_t idesc = umma_idesc_tf32(128, 64) | (1u << 15) | (1u << 16);   // both operands MN-major
-    int stage = 0; uint32_t phase = 0; int gb = 0; uint32_t gphase = 0;
-    for (int tile = t_begin; tile < t_end; ++tile) {
-      mbar_wait(&bars->g_ready[gb], gphase);
-      tc_fence_after_sync();
-      const uint32_t g_addr = smem_u32(Gs + gb * kWgGBytes);
-      for (int pr = 0; pr < npairs; ++pr) {
-        mbar_wait(&bars->ready[stage], phase);
-        tc_fence_after_sync();
-        const uint32_t a_addr = smem_u32(St + stage * kWgStageBytes);
-        const uint32_t d = tmem_base + pr * 64;
-#pragma unroll 4
-        for (int kk = 0; kk < 16; ++kk)                      // 8 batch rows per MMA
-          umma_tf32_ss_1t(d, umma_desc_sw128_mnmajor(a_addr + kk * 1024, kATile),
-                       umma_desc_sw128_mnmajor(g_addr + kk * 1024, kATile), idesc, (tile != t_begin) || (kk != 0));
-        umma_commit_1t(&bars->empty[stage]);
-        if (++stage == kWgStages) { stage = 0; phase ^= 1; }
-      }
-      umma_commit_1t(&bars->g_empty[gb]);
-      if (++gb == 2) { gb = 0; gphase ^= 1; }
-    }
-    umma_commit_1t(&bars->acc_full);
-  } else if (warp >= 8 && warp < 12) {
-    const int t = threadIdx.x - 256;
-    int stage = 0; uint32_t phase = 0; int gb = 0; uint32_t gphase = 0;
-    float ls[4] = {0.f, 0.f, 0.f, 0.f};                       // this thread's 16-byte chunk of every G row it touches
-    const bool want_bias = dbias_base != nullptr && kc == 0;   // (every k chunk sees the same G tiles)
-    for (int tile = t_begin; tile < t_end; ++tile) {
-      mbar_wait(&bars->g_raw_full[gb], gphase);
-      if (want_bias) {
-        const uint4* graw = reinterpret_cast<const uint4*>(Gs + gb * kWgGBytes);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint4 u = graw[t + 128 * k];
-          ls[0] += __uint_as_float(u.x); ls[1] += __uint_as_float(u.y); ls[2] += __uint_as_float(u.z); ls[3] += __uint_as_float(u.w);
-        }
-      }
-      split_lo_only(reinterpret_cast<const uint4*>(Gs + gb * kWgGBytes), reinterpret_cast<uint4*>(Gs + gb * kWgGBytes + kATile), t);
-      fence_proxy_async_smem();
-      mbar_arrive(&bars->g_ready[gb]);
-      if (++gb == 2) { gb = 0; gphase ^= 1; }
-      for (int pr = 0; pr < npairs; ++pr) {
-        mbar_wait(&bars->raw_full[stage], phase);
-        uint8_t* base = St + stage * kWgStageBytes;
-        split_lo_only(reinterpret_cast<const uint4*>(base), reinterpret_cast<uint4*>(base + 2 * kATile), t);
-        split_lo_only(reinterpret_cast<const uint4*>(base + kATile), reinterpret_cast<uint4*>(base + 3 * kATile), t);
-        fence_proxy_async_smem();
-        mbar_arrive(&bars->ready[stage]);
-        if (++stage == kWgStages) { stage = 0; phase ^= 1; }
-      }
-    }
-    // bias gradient = column sums of G: under the 32-byte-atom swizzle thread t always sees logical 16-byte chunk
-    // `quad` of a row (quad = ((t&7)>>1 ^ (t>>3)&3) << 1 | t&1); 16 threads share a chunk, summed in a fixed order
-#pragma unroll
-    for (int e = 0; e < 4; ++e) bars->lscr[t][e] = ls[e];
-    asm volatile("bar.sync 2, 128;" ::: "memory");
-    if (want_bias && t < 32) {
-      const int want = t >> 2, e = t & 3;
-      float acc = 0.f;
-      for (int u = 0; u < 128; ++u)
-        if ((((((u & 7) >> 1) ^ ((u >> 3) & 3)) << 1) | (u & 1)) == want) acc += bars->lscr[u][e];
-      const int n = ng * 32 + t;
-      if (n < g.N) dbias_base[(long long)sp * dbias_stride + n] = acc;
-    }
-  }
-
-  // ---- epilogue (once per CTA): TMEM -> fold the four hi/lo quadrants -> dW (or this split's partial) ----
-  if (warp >= 4 && warp < 8) {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    mbar_wait(&bars->acc_full, 0);
-    tc_fence_after_sync();
-    float* red = reinterpret_cast<float*>(St);               // all MMAs have completed: stage buffers are free
-    float* out = out_base + (long long)sp * split_stride;
-    for (int pr = 0; pr < npairs; ++pr) {
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + pr * 64;
-      uint32_t r0[32], r1[32];
-      tmem_ld_32x32b_x32(taddr, r0);
-      tmem_ld_32x32b_x32(taddr + 32, r1);
-      tmem_ld_wait();
-#pragma unroll
-      for (int cl = 0; cl < 32; ++cl) red[r * 33 + cl] = __uint_as_float(r0[cl]) + __uint_as_float(r1[cl]);
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (r < 64) {
-        const int k = (kc * 16 + 2 * pr + (r >> 5)) * 32 + (r & 31);
-        if (k < g.K) {
-#pragma unroll 4
-          for (int cl = 0; cl < 32; ++cl) {
-            const int n = ng * 32 + cl;
-            if (n < g.N) out[(long long)n * g.K + k] = red[r * 33 + cl] + red[(r + 64) * 33 + cl];
-          }
-        }
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after_sync(); tmem_dealloc(tmem_base, 512); }
 }
 
 static bool enabled() {
@@ -637,7 +474,7 @@ int dgrad_packed(const float* g, const float* packed, const float* mask_src, flo
 
 static void wgrad_plan(int M, int N, int K, int* S, int* tiles_per_split) {
   const int m_tiles = (M + 127) / 128;
-  const int base = ((N + 31) / 32) * (((K + 31) / 32 + 15) / 16);
+  const int base = ((N + 31) / 32) * ((K + 63) / 64);
   int want = (kNumSMs + base - 1) / base;
   if (want > m_tiles) want = m_tiles;
   if (want < 1) want = 1;
@@ -657,20 +494,15 @@ int wgrad(const float* g, const float* x, float* dw, float* dbias, float* ws, in
   int S, per;
   wgrad_plan(M, N, K, &S, &per);
   CUtensorMap tx, tg;
-  if (!make_2d(&tx, x, M, K, K, 128, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return DV_ERR_CUDA;
-  if (!make_2d(&tg, g, M, N, N, 128, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return DV_ERR_CUDA;
+  if (!make_2d(&tx, x, M, K, K, 128)) return DV_ERR_CUDA;
+  if (!make_2d(&tg, g, M, N, N, 128)) return DV_ERR_CUDA;
   static bool attr = false;
-  if (!attr) {
-    if (cudaFuncSetAttribute(linear_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes) != cudaSuccess) {
-      g_last_cuda_error = (int)cudaGetLastError();
-      return DV_ERR_CUDA;
-    }
-    attr = true;
-  }
+  const int rc = set_max_dynamic_smem(linear_wgrad_mma_kernel, kWgSmemBytes, &attr);
+  if (rc != DV_OK) return rc;
   WgGeom geo{M, N, K, (M + 127) / 128, per};
-  dim3 grid((N + 31) / 32, ((K + 31) / 32 + 15) / 16, S);
+  dim3 grid((N + 31) / 32, (K + 63) / 64, S);
   float* dbias_base = !dbias ? nullptr : (S > 1 ? ws + (size_t)S * N * K : dbias);
-  linear_wgrad_tc_kernel<<<grid, kThreads, kWgSmemBytes, st>>>(tx, tg, S > 1 ? ws : dw, (long long)N * K, dbias_base, (long long)N, geo);
+  linear_wgrad_mma_kernel<<<grid, kThreads, kWgSmemBytes, st>>>(tx, tg, S > 1 ? ws : dw, (long long)N * K, dbias_base, (long long)N, geo);
   *nsplit = S;
   return check_launch();
 }

@@ -1,5 +1,5 @@
-// Inline-PTX wrappers for the Blackwell (sm_100a) async machinery: mbarrier, TMA
-// (cp.async.bulk.tensor), tensor memory (tcgen05.alloc/ld/commit) and tcgen05.mma kind::tf32.
+// Inline-PTX wrappers for the Hopper (sm_90a) async machinery the tensor-core kernels use: mbarrier, TMA
+// (cp.async.bulk.tensor) and the warp-level tf32 tensor-core MMA (mma.sync m16n8k8).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -41,23 +41,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// 16-byte shared-memory load.  The operand tiles live in dynamic shared memory reached through an aligned-up pointer,
-// which the compiler treats as a GENERIC address (LD.E.128 with 64-bit address arithmetic per load); the explicit
-// ld.shared form (LDS.128, 32-bit addresses) measured 70.2 vs 72.5 us for the down kernel at (1024,16,32), the halo up
-// kernel is unchanged.  -DDV_SMEM_LDS=0 restores the generic loads.
-#ifndef DV_SMEM_LDS
-#define DV_SMEM_LDS 1
-#endif
-__device__ __forceinline__ uint4 lds128(const void* p) {
-#if DV_SMEM_LDS
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(smem_u32(p)) : "memory");
-  return v;
-#else
-  return *reinterpret_cast<const uint4*>(p);
-#endif
-}
-
 // one 32-bit word of shared memory (explicit ld.shared: 32-bit address arithmetic)
 __device__ __forceinline__ uint32_t lds32(uint32_t smem_addr) {
   uint32_t v;
@@ -65,22 +48,11 @@ __device__ __forceinline__ uint32_t lds32(uint32_t smem_addr) {
   return v;
 }
 
-// 16-byte shared-memory store / load by 32-bit shared address
-__device__ __forceinline__ void sts128(uint32_t smem_addr, float4 v) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(smem_addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+// Byte offset of fp32 element (row r, column c < 32) in a tile of 128-byte rows written by TMA with
+// CU_TENSOR_MAP_SWIZZLE_128B into a 1024-byte aligned buffer: the 16-byte chunk index is XOR-ed with (r & 7).
+__device__ __forceinline__ uint32_t swz128(int r, int c) {
+  return (uint32_t)(r * 128 + ((((c >> 2) ^ (r & 7)) << 4) | ((c & 3) << 2)));
 }
-__device__ __forceinline__ float4 lds128f(uint32_t smem_addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(smem_addr) : "memory");
-  return v;
-}
-
-// ---- proxy / tcgen05 fences -----------------------------------------------------------
-__device__ __forceinline__ void fence_proxy_async_smem() {   // generic-proxy smem writes -> async proxy (MMA/TMA)
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ---- TMA ------------------------------------------------------------------------------
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
@@ -104,123 +76,41 @@ __device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* m, int c0, in
   asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];"
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* m, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1) : "memory");
+
+// ---- tf32 tensor-core MMA -----------------------------------------------------------------
+// Error-compensated 3xTF32: x = hi + lo with hi = x rounded to the nearest tf32 and lo = x - hi (exact in fp32,
+// |lo| <= 2^-11 |x|), itself rounded to the nearest tf32; a*b ~ a_hi*b_hi + (a_hi*b_lo + a_lo*b_hi), the lo*lo term is
+// below fp32 rounding.  Rounding both planes to nearest (not truncating) keeps the residual error of a product near
+// 2^-22 of it and unbiased: a truncated split leaves an error of one sign in every product, which accumulates over
+// long reductions.
+// Nearest tf32, ties away from zero (what cvt.rna.tf32.f32 computes), as two full-rate integer operations on the
+// sign-magnitude bit pattern: add half a tf32 ulp, clear the 13 low mantissa bits.
+__device__ __forceinline__ float tf32_round(float x) {
+  return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
+}
+__device__ __forceinline__ void split_tf32(uint32_t x, uint32_t& hi, uint32_t& lo) {
+  const float h = tf32_round(__uint_as_float(x));
+  hi = __float_as_uint(h);
+  lo = __float_as_uint(tf32_round(__uint_as_float(x) - h));
 }
 
-// ---- tensor memory --------------------------------------------------------------------
-// One full warp allocates `ncols` (power of two >= 32) columns; the base address lands in *dst_smem.
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// 32 lanes x 32 consecutive columns: thread t of the warp gets lane (base_lane + t), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
+// D[16x8] += A[16x8] * B[8x8] (tf32 operands, fp32 accumulate).  With g = lane >> 2, t = lane & 3:
+//   a = {A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4]},  b = {B[t][g], B[t+4][g]},
+//   d = {D[g][2t], D[g][2t+1], D[g+8][2t], D[g+8][2t+1]}.
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> tensor memory: thread t of the warp writes lane (base_lane + t), columns [col, col+32)
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]),
-        "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]),
-        "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---- UMMA descriptors -------------------------------------------------------------------
-// K-major operand tile in shared memory, 128-byte rows, SWIZZLE_128B (what TMA writes with
-// CU_TENSOR_MAP_SWIZZLE_128B): 8-row x 128 B atoms, SBO = 1024 B between atoms along M/N.
-// (cute::UMMA::SmemDescriptor: start[0,14) LBO[16,30) SBO[32,46) version[46,48)=1 layout[61,64)=2)
-__device__ __forceinline__ uint64_t umma_desc_sw128_kmajor(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// kind::tf32, fp32 accumulate, both operands K-major (cute::UMMA::InstrDescriptor):
-// c_format[4,6)=1(F32) a_format[7,10)=2(TF32) b_format[10,13)=2 n_dim[17,23)=N>>3 m_dim[24,29)=M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem].  Call from ALL 32 lanes of the MMA warp with warp-uniform arguments:
-// the operands then live in uniform registers and one elected lane issues the instruction (calling it
-// from a single-lane branch makes the compiler emit a register->uniform-register broadcast loop per MMA).
-__device__ __forceinline__ void umma_tf32_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem: 128 lanes x K columns] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-// (implies tcgen05.fence::before_thread_sync)
-// (same calling convention: whole warp, the elected lane -- the one that issued the MMAs -- commits)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}"
-      ::"r"(smem_u32(bar)) : "memory");
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
-// Single-thread variants: the caller is already inside `if (elect_one())`, i.e. exactly one lane of the warp runs the
-// whole issue loop (barrier waits included), as CUTLASS does.
-__device__ __forceinline__ void umma_tf32_ss_1t(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_tf32_ts_1t(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_1t(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
+// main += a_hi * b_hi;  corr += a_hi * b_lo + a_lo * b_hi.  The correction products accumulate apart from the main
+// one, so they are not rounded at its magnitude.
+__device__ __forceinline__ void mma_3xtf32(float (&main)[4], float (&corr)[4], const uint32_t (&a_hi)[4],
+                                           const uint32_t (&a_lo)[4], const uint32_t (&b_hi)[2], const uint32_t (&b_lo)[2]) {
+  mma_tf32(main, a_hi, b_hi);
+  mma_tf32(corr, a_hi, b_lo);
+  mma_tf32(corr, a_lo, b_hi);
 }
 
 }  // namespace ptx

@@ -1,5 +1,5 @@
-"""disvae on B200: the reference's package surface (disvae/__init__.py:1-3) backed by
-hand-written sm_100a kernels (libdisvae_b200.so, C ABI in include/disvae_b200.h)."""
+"""disvae on H100: the reference's package surface (disvae/__init__.py:1-3) backed by
+hand-written sm_90a kernels (libdisvae_b200.so, C ABI in include/disvae_b200.h)."""
 from disvae.models.vae import init_specific_model
 from disvae.training import Trainer
 from disvae.evaluate import Evaluator

@@ -168,6 +168,6 @@ def require_cuda_f32(*tensors):
             continue
         if not t.is_cuda:
             raise RuntimeError("disvae_b200 runs on CUDA only: got a tensor on %s. Move the model and data to a "
-                               "B200 (`.to('cuda')`); there is no CPU path." % t.device)
+                               "GPU (`.to('cuda')`); there is no CPU path." % t.device)
         if t.dtype != torch.float32:
             raise RuntimeError("disvae_b200 computes in fp32; got %s" % t.dtype)

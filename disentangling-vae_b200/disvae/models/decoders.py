@@ -1,4 +1,4 @@
-"""Burgess decoder (reference disvae/models/decoders.py:16-84) on the sm_100a kernels."""
+"""Burgess decoder (reference disvae/models/decoders.py:16-84) on the sm_90a kernels."""
 from torch import nn
 
 from disvae import ops

@@ -1,4 +1,4 @@
-"""Burgess encoder (reference disvae/models/encoders.py:16-89) on the sm_100a kernels."""
+"""Burgess encoder (reference disvae/models/encoders.py:16-89) on the sm_90a kernels."""
 from torch import nn
 
 from disvae import ops

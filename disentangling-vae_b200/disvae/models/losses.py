@@ -1,4 +1,4 @@
-"""Disentanglement losses with the reference's API (disvae/models/losses.py) on the sm_100a
+"""Disentanglement losses with the reference's API (disvae/models/losses.py) on the sm_90a
 kernels: one fused reconstruction+KL kernel (ops.VaeLossFn), the beta-TCVAE decomposition kernel
 (ops.BtcvaeFn) and the FactorVAE heads.  Logged scalars are fetched with ONE device->host copy
 per recorded step instead of one `.item()` per value (losses.py:151,384-389,447,476-478).

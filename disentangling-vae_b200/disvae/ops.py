@@ -220,7 +220,7 @@ def _c(t):
 
 # ---------------------------------------------------------------------------------------
 # Weight-gradient lane: in a backward pass the weight gradient of a layer and the input gradient that continues the
-# chain are independent.  The MLP layers and the 4x4 / 8x8 conv layers occupy a fraction of the 148 SMs for ~15 us each
+# chain are independent.  The MLP layers and the 4x4 / 8x8 conv layers occupy a fraction of the SMs for a short time each
 # (launch-latency bound), so their weight-gradient kernels run on a second stream beside the dgrad chain and are joined
 # at the end of the node's backward.  Works inside CUDA-graph capture (fork/join from the capturing stream become graph
 # dependencies).  Tensors read on the side stream are kept alive until the join, so the caching allocator cannot hand

@@ -1,5 +1,5 @@
 /*
- * disvae_b200.h -- C ABI of libdisvae_b200.so: hand-written sm_100a kernels for the
+ * disvae_b200.h -- C ABI of libdisvae_b200.so: hand-written sm_90a kernels for the
  * disvae training hot path (BASELINE.json:north_star, SURVEY.md section 8).
  *
  * The reference (YannDubs/disentangling-vae) is pure Python on PyTorch and has NO
@@ -43,7 +43,7 @@ typedef enum DvStatus {
   DV_ERR_BAD_ARG = -2,       /* null pointer, bad enum */
   DV_ERR_WORKSPACE = -3,     /* workspace too small */
   DV_ERR_CUDA = -4,          /* a CUDA runtime call failed; see dv_last_cuda_error() */
-  DV_ERR_ARCH = -5           /* device is not sm_100 */
+  DV_ERR_ARCH = -5           /* device is not sm_90 */
 } DvStatus;
 
 enum { DV_ACT_NONE = 0, DV_ACT_RELU = 1, DV_ACT_SIGMOID = 2, DV_ACT_LEAKY = 3 };
@@ -51,10 +51,10 @@ enum { DV_DIST_BERNOULLI = 0, DV_DIST_GAUSSIAN = 1, DV_DIST_LAPLACE = 2 };
 
 /* ---- library probes ------------------------------------------------------------- */
 int dv_version(void);                 /* 10000*major + 100*minor + patch */
-int dv_built_arch(void);              /* 100 == compiled for sm_100a */
+int dv_built_arch(void);              /* 90 == compiled for sm_90a */
 const char* dv_status_string(int status);
 int dv_last_cuda_error(void);         /* cudaError_t of the last failing call on this thread */
-int dv_device_check(void);            /* DV_OK if the current device is compute capability 10.x */
+int dv_device_check(void);            /* DV_OK if the current device is compute capability 9.0 */
 /* how many kernels this library has launched in this process (for bench.py "gpu_launches") */
 long long dv_launch_count(void);
 
@@ -113,7 +113,7 @@ int dv_act_bwd(const float* dy, const float* y, float* g, long long n, int act, 
  * Replaces nn.Linear + activation: encoders.py:81-86, decoders.py:71-73, discriminator.py:63-68.
  * x[M,K], w[N,K] (torch layout), y[M,N].  slope is the LeakyReLU negative slope.
  */
-/* Shapes whose activation rows are 16-byte pitched run on the tensor cores (tcgen05, 3xTF32) and need
+/* Shapes whose activation rows are 16-byte pitched run on the tensor cores (mma.sync tf32, 3xTF32) and need
  * a scratch buffer for the hi/lo split weight planes; the query returns 0 when the FFMA path is used
  * (workspace may then be NULL). */
 size_t dv_linear_fwd_workspace_bytes(int M, int N, int K);
@@ -130,7 +130,7 @@ size_t dv_linear_wgrad_workspace_bytes(int M, int N, int K);
 int dv_linear_wgrad(const float* g, const float* x, float* dw, float* dbias, int M, int N, int K,
                     void* workspace, void* stream);
 /* Pre-packed weights: dv_linear_pack_multi splits n weight matrices (w[i]: [N[i], K[i]], HOST arrays of device
- * pointers / sizes) into the tcgen05 hi/lo operand planes of BOTH directions in one launch, into caller-owned
+ * pointers / sizes) into the tensor-core hi/lo operand planes of BOTH directions in one launch, into caller-owned
  * buffers of dv_linear_packed_floats(N, K) floats (16-byte aligned); dv_linear_fwd_packed / dv_linear_dgrad_packed are
  * dv_linear_fwd / dv_linear_dgrad on those planes (w is still passed: shapes that run on the CUDA cores read it).
  * One pack launch per network node per step instead of one per layer per direction. */

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep (ncu --set full) into a small markdown table for profiles/."""
+"""Summarise an .ncu-rep (ncu --set full) into a small markdown table."""
 import csv, subprocess, sys
 WANT = ["gpu__time_duration.sum", "launch__grid_size", "launch__block_size", "launch__registers_per_thread",
         "launch__shared_mem_per_block_dynamic", "dram__bytes_read.sum", "dram__bytes_write.sum",

@@ -1,4 +1,4 @@
-"""Quick guard before a long GPU run: the tcgen05 32->32 conv kernels must complete and be fp32-grade accurate
+"""Quick guard before a long GPU run: the tensor-core 32->32 conv kernels must complete and be fp32-grade accurate
 (SANITY_TIME=1 also times them at the bench shape).  Run under `timeout`: a hang here must not eat the test budget."""
 import os, sys, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

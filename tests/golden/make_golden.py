@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """Generate the golden fixtures in tests/golden/ from the UNMODIFIED reference.
 
-Run in the build container only (needs /root/reference, which does not exist on
-the GPU box):
+Needs a checkout of the reference: $DISVAE_REFERENCE, by default the location
+oracle/ship_reference.py reads (its DEFAULT_REF).  Running the tests does not:
 
-    python tests/golden/make_golden.py
+    DISVAE_REFERENCE=<reference checkout> python tests/golden/make_golden.py
 
 The reference is imported read-only with the two non-arithmetic shims of
 SURVEY.md Appendix C (an `imageio` stub; `np.product = np.prod`).  Every output
@@ -14,7 +14,7 @@ files.  Inputs are seeded; small ones are stored, big ones are re-derived from
 the seed in the tests and protected by a checksum stored here.
 
 Also copies two shipped checkpoints (reference DATA files, not source) so that
-trained / saturating weights are available on the GPU box:
+trained / saturating weights are available to the GPU tests:
 results/btcvae_dsprites/model.pt and results/VAE_mnist/model.pt.
 """
 import os
@@ -23,8 +23,12 @@ import sys
 import types
 from collections import defaultdict
 
-REF = os.environ.get("DISVAE_REFERENCE", "/root/reference")
 HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
+from oracle.ship_reference import REF  # noqa: E402  ($DISVAE_REFERENCE or the default checkout location)
+if not os.path.isfile(os.path.join(REF, "disvae", "training.py")):
+    sys.exit("make_golden.py: no reference checkout at %r; set DISVAE_REFERENCE to the directory of "
+             "YannDubs/disentangling-vae @ f0452191" % REF)
 
 sys.dont_write_bytecode = True
 sys.path.insert(0, REF)

@@ -1,6 +1,6 @@
 """Per-kernel parity: every C-ABI entry point against the oracle's plain-PyTorch CPU ops on the
 same seeded inputs.  Tolerance: the north_star's 1e-4 relative (fp32); most kernels are far
-inside it.  Run on the B200 box:  pytest -m gpu."""
+inside it.  Run on an H100:  pytest -m gpu."""
 import math
 
 import pytest
@@ -235,7 +235,7 @@ def test_linear_fwd_dgrad_wgrad(ops, M, N, K):
 
 @pytest.mark.parametrize("M,N,K", [(1024, 256, 512), (256, 1000, 1000), (300, 1000, 12), (77, 512, 256)])
 def test_linear_tensor_core_accuracy_vs_fp64(ops, M, N, K):
-    """The tcgen05 linear layers use the same error-compensated 3xTF32 scheme as the convolutions: <= 4e-6 of the
+    """The tensor-core linear layers use the same error-compensated 3xTF32 scheme as the convolutions: <= 4e-6 of the
     output scale against an fp64 reference (plain fp32 ~5e-7, single-pass tf32 ~5e-4)."""
     torch.manual_seed(M * 7 + N + K)
     x = torch.randn(M, K)

@@ -1,7 +1,7 @@
 """Model / loss / training-step parity of the CUDA path against (a) golden fixtures produced by
 the unmodified reference (tests/golden/make_golden.py) and (b) the oracle on the same seeded
 inputs at larger sizes.  Tolerance: 1e-4 relative fp32 on losses and reconstructions
-(BASELINE.json north_star).  Run on the B200 box: pytest -m gpu."""
+(BASELINE.json north_star).  Run on an H100: pytest -m gpu."""
 import logging
 import os
 from collections import OrderedDict, defaultdict

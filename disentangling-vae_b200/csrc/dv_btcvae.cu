@@ -755,7 +755,6 @@ int dv_btcvae_fwd_rows(const float* z, const float* mu, const float* logvar, int
   int rc;
   {
     // single-launch cluster path (D <= 16): columns split over the 4 CTAs of a cluster, rows over the clusters
-    static const int v4 = env_switch("DV_BTCVAE_V4", 1);
     const int dc = D == 10 ? 10 : 16;
     const int max_clusters = 32;                               // estimated 4-CTA cluster capacity of a 132-SM H100 (see above)
     int R = ((B + max_clusters - 1) / max_clusters + kRows - 1) / kRows * kRows;
@@ -766,7 +765,7 @@ int dv_btcvae_fwd_rows(const float* z, const float* mu, const float* logvar, int
     int S = G >= kF4Warps ? 1 : kF4Warps / G;
     if (S > NC / 32) S = NC / 32;
     if (S < 1) S = 1;
-    if (whole && v4 && D <= 16 && smem <= 200 * 1024 && R <= kF4MaxRows && G * S <= kF4MaxTasks) {
+    if (whole && D <= 16 && smem <= 200 * 1024 && R <= kF4MaxRows && G * S <= kF4MaxTasks) {
       const int nclus = (B + R - 1) / R;
       float4* pj = reinterpret_cast<float4*>(ws + kWsHeader);
       float* blockpart = ws + btcvae_part_offset_floats(B, D);

@@ -2,7 +2,6 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 #include "disvae_b200.h"
 
 #if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
@@ -42,17 +41,6 @@ inline int set_max_dynamic_smem(Kernel kernel, int bytes, bool* done) {
 // First 1024-byte aligned address at or after p (TMA destinations with the 128-byte swizzle need it).
 __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
-}
-
-// Environment toggles exist for A/B measurements only.  Each one is read ONCE per process through a C++11 local static
-// (`static const int v = env_switch(...)`: initialisation is thread-safe), so the entry points stay re-entrant.
-inline int env_switch(const char* name, int dflt) {          // "0..." -> 0, anything else set -> 1, unset -> dflt
-  const char* e = getenv(name);
-  return e ? (e[0] == '0' ? 0 : 1) : dflt;
-}
-inline int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
 }
 
 __device__ __forceinline__ float4 ldg4(const float* p) {

@@ -22,8 +22,8 @@
 //         32*CH FMAs); 16 streams per CTA, persistent CTAs, one ordered cross-stream reduction at the end, partials in
 //         the layout conv_wgrad_reduce_kernel already consumes (deterministic).
 //
-// Geometry handled here: square images of 32 or 64 pixels (lo W = H in {16, 32}), CH in {1, 3}; everything else keeps
-// the older paths.
+// Geometry handled here: square images of 32 or 64 pixels (lo W = H in {16, 32}), CH in {1, 3} -- every image-boundary
+// layer the shape check of dv_conv.cu accepts.
 #include "dv_common.cuh"
 
 namespace dv {
@@ -291,7 +291,7 @@ img_wgrad_kernel(const float* __restrict__ lo, const float* __restrict__ hi, flo
 // up: hi[b][c][2m+py][2n+px] = bias[c] + sum_{cl} sum_{(dm, kh) valid for py} sum_{(dn, kw) valid for px}
 //                                        lo[b][m+dm][n+dn][cl] * w[cl][c][kh][kw]
 //     py = 0: (dm, kh) in {(0,1), (-1,3)};  py = 1: (dm, kh) in {(+1,0), (0,2)}   (same for px / dn / kw)
-// weights wu[(tap*CH + c)*32 + cl] (the "up" section of conv_pack_kernel for CH < 32)
+// weights wu[(tap*CH + c)*32 + cl] (the "up" section of conv_pack_multi_kernel for CH < 32)
 // ------------------------------------------------------------------------------------------------------------
 template <int CH, int W>
 __global__ void __launch_bounds__(128, 2)
@@ -396,10 +396,6 @@ template <int CH, int W> constexpr size_t wgrad_smem() {
   return (tiles > red ? tiles : red) * sizeof(float);
 }
 
-bool shape_ok(int B, int H, int W, int CH) {
-  return B > 0 && H == W && (W == 16 || W == 32) && (CH == 1 || CH == 3);
-}
-
 template <typename K>
 static bool set_smem(K kernel, size_t bytes) {
   return bytes <= 48 * 1024 || cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) == cudaSuccess;
@@ -422,11 +418,15 @@ int conv_down(const float* hi, const float* wd, const float* bias, const float* 
   return check_launch();
 }
 
-int conv_wgrad(const float* lo, const float* hi, float* ws, int B, int H, int W, int CH, int max_split, int* nsplit, cudaStream_t st) {
+// CTAs of img_wgrad_kernel<CH, W>, one split-K partial each: persistent, as many as fit on the SMs (2 per SM for CH = 1)
+int wgrad_splits(int B, int H, int CH) {
   const int tiles = B * (H / 16);
   const int per_sm = (CH == 1) ? 2 : 1;
-  int grid = tiles < per_sm * kNumSMs ? tiles : per_sm * kNumSMs;
-  if (grid > max_split) grid = max_split;
+  return tiles < per_sm * kNumSMs ? tiles : per_sm * kNumSMs;
+}
+
+int conv_wgrad(const float* lo, const float* hi, float* ws, int B, int H, int W, int CH, cudaStream_t st) {
+  const int grid = wgrad_splits(B, H, CH);
 #define DV_IMG_WG(CHV, WV)                                                                     \
   do {                                                                                         \
     if (!set_smem(img_wgrad_kernel<CHV, WV>, wgrad_smem<CHV, WV>())) return DV_ERR_CUDA;       \
@@ -437,7 +437,6 @@ int conv_wgrad(const float* lo, const float* hi, float* ws, int B, int H, int W,
   else if (CH == 1 && W == 16) DV_IMG_WG(1, 16);
   else DV_IMG_WG(3, 16);
 #undef DV_IMG_WG
-  *nsplit = grid;
   return check_launch();
 }
 

@@ -11,7 +11,6 @@
 //   * warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 load fragments, issue mma.sync m16n8k8 and run
 //     the epilogue; warp 8 is the TMA producer.  mbarrier rings between them: raw-full (TMA transaction count) and
 //     raw-empty (one arrival per consumer warp).
-#include <stdlib.h>
 #include "dv_common.cuh"
 #include "dv_ptx.cuh"
 
@@ -49,7 +48,6 @@ struct DownGeom {
   int rows_per_tile;    // 128 / W image-rows of lo per tile
   int num_tiles;
   long long total_px;
-  int prefetch;         // L2-prefetch the next tile's hi rows (DV_TC_PREFETCH=0 switches it off)
 };
 constexpr int kDownStages = 5;
 struct DownBarriers {
@@ -90,7 +88,7 @@ conv_down32_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
       const int r0 = tile * g.rows_per_tile;
       const int b0 = r0 / g.H, i0 = r0 % g.H;
-      if (g.prefetch && tile + (int)gridDim.x < g.num_tiles) {
+      if (tile + (int)gridDim.x < g.num_tiles) {
         // the four taps (kh,kw) in {1,2}^2 touch every hi pixel of a tile exactly once: pull the NEXT tile into L2
         const int rn = (tile + gridDim.x) * g.rows_per_tile;
         const int bn = rn / g.H, in_ = rn % g.H;
@@ -217,7 +215,6 @@ static_assert(kWtSmem <= kSmemMax, "smem");
 
 struct WtGeom {
   int B, H, W, rows_per_tile, num_tiles, tiles_per_cta;
-  int prefetch;
 };
 
 __global__ void __launch_bounds__(kThreads, 1)
@@ -247,7 +244,7 @@ conv_wgrad32_mma_kernel(const __grid_constant__ CUtensorMap tmap_hi, const __gri
     for (int tile = t_begin; tile < t_end; ++tile, ++tseq) {
       const int r0 = tile * g.rows_per_tile;
       const int b0 = r0 / g.H, i0 = r0 % g.H;
-      if (g.prefetch && tile + 1 < t_end) {                  // pull the next tile's hi rows (and lo tile) into L2
+      if (tile + 1 < t_end) {                                // pull the next tile's hi rows (and lo tile) into L2
         const int rn = (tile + 1) * g.rows_per_tile;
         const int bn = rn / g.H, in_ = rn % g.H;
         for (int t4 = 0; t4 < 4; ++t4) tma_prefetch_4d(&tmap_hi, 0, (t4 & 1), 2 * in_ + (t4 >> 1), bn);
@@ -508,33 +505,11 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
   }
 }
 
-// ---- weight packing for the tensor-core kernels ------------------------------------------
-// w[cl][c][tap] ->  down: Wd[tap][row][c],  row <  32: hi (nearest tf32) of w[row][c][tap], row >= 32: lo
-//                   up  : Wu[tap][row][cl], row <  32: hi of w[cl][row][tap],          row >= 32: lo
-// wf != NULL: the same launch also writes the two CUDA-core layouts of conv_pack_kernel (dv_conv.cu): Wd[tap*32+c][cl]
-// and Wu[tap][cl][c] -- the fallbacks for geometries the tensor-core kernels do not take.
-__global__ void conv_pack_tc_kernel(const float* __restrict__ w, float* __restrict__ wd, float* __restrict__ wu,
-                                    float* __restrict__ wf) {
-  const int n = kLoCh * 32 * kTaps;
-  for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < n; idx += gridDim.x * blockDim.x) {
-    const int tap = idx % kTaps, c = (idx / kTaps) % 32, cl = idx / (kTaps * 32);
-    const float v = w[idx];
-    if (wf) {
-      wf[(tap * 32 + c) * kLoCh + cl] = v;
-      wf[n + (tap * kLoCh + cl) * 32 + c] = v;
-    }
-    const float hi = tf32_round(v);
-    const float lo = tf32_round(v - hi);
-    wd[(tap * 64 + cl) * 32 + c] = hi;
-    wd[(tap * 64 + 32 + cl) * 32 + c] = lo;
-    wu[(tap * 64 + c) * 32 + cl] = hi;
-    wu[(tap * 64 + 32 + c) * 32 + cl] = lo;
-  }
-}
-
-// every conv layer of a network node in ONE launch (blockIdx.y = layer): the CH == 32 layers get the four layouts of
-// conv_pack_tc_kernel at wp + {0 (CUDA-core), 32768 (tensor-core down), 65536 (tensor-core up)}, the image-boundary
-// layers (CH in {1,3}) the two layouts of conv_pack_kernel (dv_conv.cu): Wd[tap*CH + c][cl] and Wu[tap][c][cl]
+// ---- weight packing ----------------------------------------------------------------------
+// Every conv layer of a network node in ONE launch (blockIdx.y = layer), w[cl][c][tap] ->
+//   CH == 32:     down section Wd[tap][row][c] at wp,  row < 32: hi (nearest tf32) of w[row][c][tap], row >= 32: lo;
+//                 up section   Wu[tap][row][cl] at wp + 16*64*32,  row < 32: hi of w[cl][row][tap], row >= 32: lo
+//   CH in {1,3}:  the fp32 layout [tap*CH + c][cl] of the dv_conv_img.cu kernels, twice (down section, up section)
 constexpr int kPackMultiMax = 8;
 struct ConvPackTable {
   const float* w[kPackMultiMax];
@@ -549,11 +524,13 @@ __global__ void conv_pack_multi_kernel(ConvPackTable tab) {
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < n; idx += gridDim.x * blockDim.x) {
     const int tap = idx % kTaps, c = (idx / kTaps) % CH, cl = idx / (kTaps * CH);
     const float v = w[idx];
-    wp[(tap * CH + c) * kLoCh + cl] = v;
-    if (CH != 32) { wp[n + (tap * CH + c) * kLoCh + cl] = v; continue; }
-    wp[n + (tap * kLoCh + cl) * 32 + c] = v;
-    float* wd = wp + 2 * n;
-    float* wu = wd + kTaps * 64 * 32;
+    if (CH != 32) {
+      wp[(tap * CH + c) * kLoCh + cl] = v;
+      wp[n + (tap * CH + c) * kLoCh + cl] = v;
+      continue;
+    }
+    float* wd = wp;
+    float* wu = wp + kTaps * 64 * 32;
     const float hi = tf32_round(v);
     const float lo = tf32_round(v - hi);
     wd[(tap * 64 + cl) * 32 + c] = hi;
@@ -564,28 +541,6 @@ __global__ void conv_pack_multi_kernel(ConvPackTable tab) {
 }
 
 // ---- host side ---------------------------------------------------------------------------
-static int use_prefetch() {
-  static const int v = env_switch("DV_TC_PREFETCH", 1);
-  return v;
-}
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
 // NHWC activation [B][HH][WW][32] fp32; box = {32, bw, bh, bb} traversed with element strides {1, sw, sh, 1}, 128-byte swizzle
 static bool make_act_tmap(CUtensorMap* m, const float* base, int B, int HH, int WW, int bw, int bh, int bb, int stride) {
   EncodeTiledFn enc = get_encode();
@@ -622,10 +577,6 @@ int pack_multi(int n, const float* const* w, float* const* wp, const int* CH, cu
   }
   return DV_OK;
 }
-int pack_tc(const float* w, float* wd, float* wu, float* wf, cudaStream_t st) {
-  conv_pack_tc_kernel<<<64, 256, 0, st>>>(w, wd, wu, wf);
-  return check_launch();
-}
 
 // lo[B,H,W,32] = act(down(hi[B,2H,2W,32]) + bias) * [mask > 0]
 // colsum_part != NULL: the kernel also leaves per-CTA channel sums of `lo` in colsum_part[grid][32] and sets
@@ -636,7 +587,7 @@ int conv_down32_tc(const float* hi, const float* wd_packed, const float* bias, c
   if (nparts) *nparts = 0;
   if (W > 128 || 128 % W != 0) return DV_ERR_BAD_SHAPE;
   DownGeom g = {};
-  g.B = B; g.H = H; g.W = W; g.prefetch = use_prefetch();
+  g.B = B; g.H = H; g.W = W;
   g.rows_per_tile = 128 / W;
   const int TR = g.rows_per_tile < H ? g.rows_per_tile : H;
   if (H % TR != 0 || g.rows_per_tile % TR != 0) return DV_ERR_BAD_SHAPE;
@@ -655,20 +606,26 @@ int conv_down32_tc(const float* hi, const float* wd_packed, const float* bias, c
   return check_launch();
 }
 
-// partial sums of dw (and of lo, last row) per CTA into ws[grid][16*32+1][32]; returns the grid size in *nsplit
-int conv_wgrad32_tc(const float* lo, const float* hi, float* ws, int B, int H, int W, int* nsplit, cudaStream_t st) {
+// CTAs of conv_wgrad32_mma_kernel, one split-K partial each: at most one per SM, no empty CTA
+int wgrad_splits(int B, int H, int W) {
+  const int num_tiles = (int)(((long long)B * H * W + 127) / 128);
+  const int grid = num_tiles < kNumSMs ? num_tiles : kNumSMs;
+  const int tiles_per_cta = (num_tiles + grid - 1) / grid;
+  return (num_tiles + tiles_per_cta - 1) / tiles_per_cta;
+}
+
+// partial sums of dw (and of lo, last row) per CTA into ws[wgrad_splits(B, H, W)][16*32+1][32]
+int conv_wgrad32_tc(const float* lo, const float* hi, float* ws, int B, int H, int W, cudaStream_t st) {
   if (W > 128 || 128 % W != 0) return DV_ERR_BAD_SHAPE;
   WtGeom g = {};
-  g.B = B; g.H = H; g.W = W; g.prefetch = use_prefetch();
+  g.B = B; g.H = H; g.W = W;
   g.rows_per_tile = 128 / W;
   const int TR = g.rows_per_tile < H ? g.rows_per_tile : H;
   if (H % TR != 0 || g.rows_per_tile % TR != 0) return DV_ERR_BAD_SHAPE;
   const int TB = g.rows_per_tile / TR;
   g.num_tiles = (int)(((long long)B * H * W + 127) / 128);
-  int grid = g.num_tiles < kNumSMs ? g.num_tiles : kNumSMs;
+  const int grid = wgrad_splits(B, H, W);
   g.tiles_per_cta = (g.num_tiles + grid - 1) / grid;
-  grid = (g.num_tiles + g.tiles_per_cta - 1) / g.tiles_per_cta;   // no empty CTA
-  *nsplit = grid;
   CUtensorMap thi, tlo;
   if (!make_act_tmap(&thi, hi, B, 2 * H, 2 * W, 2 * W, 2 * TR, TB, 2)) return DV_ERR_CUDA;
   if (!make_act_tmap(&tlo, lo, B, H, W, W, TR, TB, 1)) return DV_ERR_CUDA;

@@ -184,12 +184,7 @@ static int wgrad_splits(int M, int N, int K) {
 }  // namespace dv
 
 namespace dv { namespace ltc {
-size_t fwd_workspace_bytes(int M, int N, int K);
-size_t dgrad_workspace_bytes(int M, int N, int K);
-int fwd(const float* x, const float* w, const float* bias, float* y, int M, int N, int K, int act, float slope, float* ws,
-        cudaStream_t st);
-int dgrad(const float* g, const float* w, const float* mask_src, float* dx, int M, int N, int K, int act, float slope, float* ws,
-          cudaStream_t st);
+bool nt_ok(int R);
 size_t packed_floats(int N, int K);
 int pack_multi(int n, const float* const* w, float* const* packed, const int* N, const int* K, cudaStream_t st);
 int fwd_packed(const float* x, const float* packed, const float* bias, float* y, int M, int N, int K, int act, float slope,
@@ -205,13 +200,14 @@ using namespace dv;
 
 extern "C" {
 
+// The tensor-core path packs w into the workspace (the layout of dv_linear_pack_multi) and runs on those planes.
 size_t dv_linear_fwd_workspace_bytes(int M, int N, int K) {
-  if (M <= 0 || N <= 0 || K <= 0) return 0;
-  return ltc::fwd_workspace_bytes(M, N, K);
+  if (M <= 0 || N <= 0 || K <= 0 || !ltc::nt_ok(K)) return 0;
+  return ltc::packed_floats(N, K) * sizeof(float);
 }
 size_t dv_linear_dgrad_workspace_bytes(int M, int N, int K) {
-  if (M <= 0 || N <= 0 || K <= 0) return 0;
-  return ltc::dgrad_workspace_bytes(M, N, K);
+  if (M <= 0 || N <= 0 || K <= 0 || !ltc::nt_ok(N)) return 0;
+  return ltc::packed_floats(N, K) * sizeof(float);
 }
 
 int dv_linear_fwd(const float* x, const float* w, const float* bias, float* y, int M, int N, int K,
@@ -219,9 +215,12 @@ int dv_linear_fwd(const float* x, const float* w, const float* bias, float* y, i
   if (!x || !w || !y) return DV_ERR_BAD_ARG;
   if (M <= 0 || N <= 0 || K <= 0) return DV_ERR_BAD_SHAPE;
   if (act < DV_ACT_NONE || act > DV_ACT_LEAKY) return DV_ERR_BAD_ARG;
-  if (ltc::fwd_workspace_bytes(M, N, K) > 0) {
+  if (ltc::nt_ok(K)) {
     if (!workspace) return DV_ERR_WORKSPACE;
-    return ltc::fwd(x, w, bias, y, M, N, K, act, slope, reinterpret_cast<float*>(workspace), as_stream(stream));
+    float* packed = reinterpret_cast<float*>(workspace);
+    const int rc = ltc::pack_multi(1, &w, &packed, &N, &K, as_stream(stream));
+    if (rc != DV_OK) return rc;
+    return ltc::fwd_packed(x, packed, bias, y, M, N, K, act, slope, as_stream(stream));
   }
   GemmEpilogue ep{bias, nullptr, act, slope};
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
@@ -233,9 +232,12 @@ int dv_linear_dgrad(const float* g, const float* w, const float* mask_src, float
                     int act, float slope, void* workspace, void* stream) {
   if (!g || !w || !dx) return DV_ERR_BAD_ARG;
   if (M <= 0 || N <= 0 || K <= 0) return DV_ERR_BAD_SHAPE;
-  if (ltc::dgrad_workspace_bytes(M, N, K) > 0) {
+  if (ltc::nt_ok(N)) {
     if (!workspace) return DV_ERR_WORKSPACE;
-    return ltc::dgrad(g, w, mask_src, dx, M, N, K, act, slope, reinterpret_cast<float*>(workspace), as_stream(stream));
+    float* packed = reinterpret_cast<float*>(workspace);
+    const int rc = ltc::pack_multi(1, &w, &packed, &N, &K, as_stream(stream));
+    if (rc != DV_OK) return rc;
+    return ltc::dgrad_packed(g, packed, mask_src, dx, M, N, K, act, slope, as_stream(stream));
   }
   GemmEpilogue ep{nullptr, mask_src, mask_src ? act : DV_ACT_NONE, slope};
   dim3 grid((K + BN - 1) / BN, (M + BM - 1) / BM);
@@ -261,7 +263,7 @@ int dv_linear_fwd_packed(const float* x, const float* w, const float* packed, co
   if (!x || !w || !y) return DV_ERR_BAD_ARG;
   if (M <= 0 || N <= 0 || K <= 0) return DV_ERR_BAD_SHAPE;
   if (act < DV_ACT_NONE || act > DV_ACT_LEAKY) return DV_ERR_BAD_ARG;
-  if (ltc::fwd_workspace_bytes(M, N, K) > 0) {
+  if (ltc::nt_ok(K)) {
     if (!packed) return DV_ERR_WORKSPACE;
     return ltc::fwd_packed(x, packed, bias, y, M, N, K, act, slope, as_stream(stream));
   }
@@ -272,7 +274,7 @@ int dv_linear_dgrad_packed(const float* g, const float* w, const float* packed, 
                            int K, int act, float slope, void* stream) {
   if (!g || !w || !dx) return DV_ERR_BAD_ARG;
   if (M <= 0 || N <= 0 || K <= 0) return DV_ERR_BAD_SHAPE;
-  if (ltc::dgrad_workspace_bytes(M, N, K) > 0) {
+  if (ltc::nt_ok(N)) {
     if (!packed) return DV_ERR_WORKSPACE;
     return ltc::dgrad_packed(g, packed, mask_src, dx, M, N, K, act, slope, as_stream(stream));
   }

@@ -12,8 +12,6 @@
 //   Row / column / K tails are handled by TMA out-of-bounds zero fill and guarded stores.
 #include "dv_common.cuh"
 #include "dv_ptx.cuh"
-#include <cstdlib>
-#include <cstring>
 
 namespace dv {
 namespace ltc {
@@ -270,41 +268,10 @@ linear_wgrad_mma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid
   }
 }
 
-// w[N][K] -> hi/lo planes.  transpose == 0: [N][Kp] (forward; Kp = K rounded up to 4 floats, TMA pitch is 16-byte);
-//                            transpose == 1: [K][Np] (the transposed copy the input-gradient GEMM reads).
-__global__ void linear_pack_kernel(const float* __restrict__ w, float* __restrict__ p_hi, float* __restrict__ p_lo,
-                                   int N, int K, int pitch, int transpose) {
-  __shared__ float tile[32][33];
-  const int n0 = blockIdx.y * 32, k0 = blockIdx.x * 32;
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;     // 32 x 8
-  for (int r = ty; r < 32; r += 8) {
-    const int n = n0 + r, k = k0 + tx;
-    const float v = (n < N && k < K) ? w[(long long)n * K + k] : 0.f;
-    if (transpose) {
-      tile[r][tx] = v;
-    } else if (n < N && k < pitch) {
-      const float hi = tf32_round(v);
-      p_hi[(long long)n * pitch + k] = hi;
-      p_lo[(long long)n * pitch + k] = tf32_round(v - hi);
-    }
-  }
-  if (!transpose) return;
-  __syncthreads();
-  for (int r = ty; r < 32; r += 8) {
-    const int k = k0 + r, n = n0 + tx;
-    if (k < K && n < pitch) {
-      const float v = tile[tx][r];
-      const float hi = tf32_round(v);
-      p_hi[(long long)k * pitch + n] = hi;
-      p_lo[(long long)k * pitch + n] = tf32_round(v - hi);
-    }
-  }
-}
-
-// Multi-tensor pack: every weight matrix of a network node (encoder MLP, decoder MLP, the 6-layer discriminator) in
+// Weight packing: every weight matrix of a network node (encoder MLP, decoder MLP, the 6-layer discriminator) in
 // ONE launch, both layouts at once -- packed[i] = [fwd hi | fwd lo | transposed hi | transposed lo] with pitches
-// round4(K) / round4(N).  Replaces one linear_pack_kernel launch per layer per direction (12 per VAE step, 22 per
-// FactorVAE step).
+// round4(K) / round4(N) (TMA row pitches are multiples of 16 bytes); the transposed copy is what the input-gradient
+// GEMM reads.
 constexpr int kPackMax = 8;
 struct PackTable {
   const float* w[kPackMax];
@@ -348,22 +315,6 @@ __global__ void linear_pack_multi_kernel(PackTable t) {
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
 // row-major [rows][cols] fp32 with a row pitch of `pitch` floats; box = {32 cols, box_rows}, 128-byte swizzle
 static bool make_2d(CUtensorMap* m, const float* base, long long rows, long long cols, long long pitch, int box_rows) {
   EncodeTiledFn enc = get_encode();
@@ -378,13 +329,6 @@ static bool make_2d(CUtensorMap* m, const float* base, long long rows, long long
 }
 
 static inline int round4(int v) { return (v + 3) & ~3; }
-
-static int pack(const float* w, float* p_hi, float* p_lo, int N, int K, int transpose, cudaStream_t st) {
-  const int pitch = transpose ? round4(N) : round4(K);
-  dim3 grid((round4(K) + 31) / 32, (round4(N) + 31) / 32);
-  linear_pack_kernel<<<grid, 256, 0, st>>>(w, p_hi, p_lo, N, K, pitch, transpose);
-  return check_launch();
-}
 
 // C[M,Nout] = epi(A[M,R] . B[Nout,R]^T);  b_hi/b_lo are packed planes with row pitch round4(R)
 static int launch_nt(const float* A, long long a_pitch, const float* b_hi, const float* b_lo, float* C, int M, int Nout, int R,
@@ -401,39 +345,8 @@ static int launch_nt(const float* A, long long a_pitch, const float* b_hi, const
   return check_launch();
 }
 
-static bool enabled() {
-  static const int v = [] { const char* e = getenv("DV_LINEAR_IMPL"); return (e && strcmp(e, "ffma") == 0) ? 0 : 1; }();
-  return v == 1;
-}
-// the tensor-core path needs 16-byte pitched activation rows for TMA: K % 4 == 0 (fwd) / N % 4 == 0 (dgrad)
-size_t fwd_workspace_bytes(int M, int N, int K) {
-  if (!enabled() || K % 4 != 0 || K < 32) return 0;
-  return (size_t)2 * N * K * sizeof(float);
-}
-size_t dgrad_workspace_bytes(int M, int N, int K) {
-  if (!enabled() || N % 4 != 0 || N < 32) return 0;
-  return (size_t)2 * K * N * sizeof(float);
-}
-
-int fwd(const float* x, const float* w, const float* bias, float* y, int M, int N, int K, int act, float slope, float* ws,
-        cudaStream_t st) {
-  float* hi = ws;
-  float* lo = ws + (size_t)N * K;
-  int rc = pack(w, hi, lo, N, K, 0, st);
-  if (rc != DV_OK) return rc;
-  Epilogue ep{bias, nullptr, act, slope};
-  return launch_nt(x, K, hi, lo, y, M, N, K, ep, st);
-}
-int dgrad(const float* g, const float* w, const float* mask_src, float* dx, int M, int N, int K, int act, float slope, float* ws,
-          cudaStream_t st) {
-  float* hi = ws;
-  float* lo = ws + (size_t)K * N;
-  int rc = pack(w, hi, lo, N, K, 1, st);
-  if (rc != DV_OK) return rc;
-  Epilogue ep{nullptr, mask_src, mask_src ? act : DV_ACT_NONE, slope};
-  return launch_nt(g, N, hi, lo, dx, M, K, N, ep, st);
-}
-
+// the NT GEMM reads its activation rows through TMA: they need a 16-byte pitch, R % 4 == 0 (R = K forward, N dgrad)
+bool nt_ok(int R) { return R % 4 == 0 && R >= 32; }
 
 size_t packed_floats(int N, int K) { return (size_t)2 * N * round4(K) + (size_t)2 * K * round4(N); }
 
@@ -456,7 +369,7 @@ int pack_multi(int n, const float* const* w, float* const* packed, const int* N,
   return DV_OK;
 }
 
-// the same two GEMMs on planes that dv_linear_pack_multi produced
+// forward and input-gradient GEMMs on planes written by pack_multi
 int fwd_packed(const float* x, const float* packed, const float* bias, float* y, int M, int N, int K, int act, float slope,
                cudaStream_t st) {
   const float* hi = packed;
@@ -482,7 +395,7 @@ static void wgrad_plan(int M, int N, int K, int* S, int* tiles_per_split) {
   *tiles_per_split = per;
   *S = (m_tiles + per - 1) / per;                             // no empty split
 }
-bool wgrad_ok(int M, int N, int K) { return enabled() && N % 4 == 0 && K % 4 == 0 && K >= 32 && M >= 32; }
+bool wgrad_ok(int M, int N, int K) { return N % 4 == 0 && K % 4 == 0 && K >= 32 && M >= 32; }
 size_t wgrad_workspace_bytes(int M, int N, int K) {
   int S, per;
   wgrad_plan(M, N, K, &S, &per);

@@ -1,5 +1,6 @@
 // Inline-PTX wrappers for the Hopper (sm_90a) async machinery the tensor-core kernels use: mbarrier, TMA
-// (cp.async.bulk.tensor) and the warp-level tf32 tensor-core MMA (mma.sync m16n8k8).
+// (cp.async.bulk.tensor) and the warp-level tf32 tensor-core MMA (mma.sync m16n8k8), and the host-side lookup of the
+// driver's tensor-map encoder.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -75,6 +76,22 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 __device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* m, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];"
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+
+// Host side: the driver's cuTensorMapEncodeTiled, looked up once per process through the runtime (no -lcuda);
+// nullptr if the driver does not provide it.
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+inline EncodeTiledFn get_encode() {
+  static const EncodeTiledFn fn = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    const bool ok = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
+                    qres == cudaDriverEntryPointSuccess;
+    return ok ? reinterpret_cast<EncodeTiledFn>(p) : nullptr;
+  }();
+  return fn;
 }
 
 // ---- tf32 tensor-core MMA -----------------------------------------------------------------

@@ -65,8 +65,12 @@ long long dv_launch_count(void);
  *           -> dv_conv_up / dv_conv_down (input grads), dv_conv_wgrad (+ bias grads).
  * w is the torch weight tensor itself, [32][CH][4][4] contiguous; w_packed is produced by
  * dv_conv_pack_weights (layout private to the library).  B images, lo is H x W.
- * hi_nchw != 0: hi is [B,CH,2H,2W] (model boundary; required for CH in {1,3});
- * hi_nchw == 0: hi is [B,2H,2W,CH] (required for CH == 32).
+ * hi_nchw != 0: hi is [B,CH,2H,2W];  hi_nchw == 0: hi is [B,2H,2W,CH].
+ * Shapes: the layers of the Burgess encoder and decoder on 32x32 and 64x64 images (vae.py:28).
+ * dv_conv_down, dv_conv_up and dv_conv_wgrad return DV_ERR_BAD_SHAPE for anything else:
+ *     CH       lo geometry (H == W)   layout of hi
+ *     1 or 3   16 or 32               NCHW (hi_nchw != 0)
+ *     32       4, 8 or 16             NHWC (hi_nchw == 0)
  * mask (optional, same shape/layout as the OUTPUT): out *= (mask > 0) -- the ReLU backward
  * of the layer that produced `mask`, fused into this epilogue.
  */
@@ -84,18 +88,20 @@ int dv_conv_pack_multi(int n, const void* const* w, void* const* w_packed, const
  * ReLU masks as bits (both optional, 32-channel NHWC outputs only, one 32-bit word per OUTPUT pixel, bit c =
  * channel c):  relu_bits_out receives [out > 0] of the stored tensor from the same epilogue -- kept by the
  * caller, it is the mask of the backward pass through the ReLU that follows this layer;  mask_bits is that
- * word form of `mask` (which must be passed as well: the CUDA-core fallbacks read the floats): the backward
- * epilogue then reads 4 bytes per pixel instead of 128 (autograd's threshold_backward, fused and compressed). */
+ * word form of `mask` (which must be passed as well): the backward epilogue then reads 4 bytes per pixel instead
+ * of 128 (autograd's threshold_backward, fused and compressed). */
 int dv_conv_down(const float* hi, const float* w_packed, const float* bias, const float* mask,
                  float* lo, int B, int H, int W, int CH, int hi_nchw, int act, float* colsum_out,
                  void* colsum_workspace, const unsigned* mask_bits, unsigned* relu_bits_out, void* stream);
-/* hi = act(up(lo) + bias) * [mask>0];  bias[CH] may be NULL.  act in {NONE, RELU, SIGMOID}.
- * mask_bits / relu_bits_out as above (CH == 32 only). */
+/* hi = act(up(lo) + bias) * [mask>0];  bias[CH] may be NULL.  act in {NONE, RELU, SIGMOID}; SIGMOID for
+ * CH in {1,3} only (DV_ERR_BAD_ARG otherwise).  mask, mask_bits and relu_bits_out as above, CH == 32 only
+ * (DV_ERR_BAD_ARG otherwise). */
 int dv_conv_up(const float* lo, const float* w_packed, const float* bias, const float* mask,
                float* hi, int B, int H, int W, int CH, int hi_nchw, int act, const unsigned* mask_bits,
                unsigned* relu_bits_out, void* stream);
 /* dw[32][CH][4][4] = sum_pixels lo (x) patch(hi);  dbias_lo[32] (optional) = sum_pixels lo.
- * Deterministic split-K: partials go to `workspace`, reduced in a fixed order. */
+ * Deterministic split-K: partials go to `workspace`, reduced in a fixed order.  The workspace query returns 0
+ * for a shape outside the table above. */
 size_t dv_conv_wgrad_workspace_bytes(int B, int H, int W, int CH);
 int dv_conv_wgrad(const float* lo, const float* hi, float* dw, float* dbias_lo, void* workspace,
                   size_t workspace_bytes, int B, int H, int W, int CH, int hi_nchw, void* stream);
@@ -113,9 +119,10 @@ int dv_act_bwd(const float* dy, const float* y, float* g, long long n, int act, 
  * Replaces nn.Linear + activation: encoders.py:81-86, decoders.py:71-73, discriminator.py:63-68.
  * x[M,K], w[N,K] (torch layout), y[M,N].  slope is the LeakyReLU negative slope.
  */
-/* Shapes whose activation rows are 16-byte pitched run on the tensor cores (mma.sync tf32, 3xTF32) and need
- * a scratch buffer for the hi/lo split weight planes; the query returns 0 when the FFMA path is used
- * (workspace may then be NULL). */
+/* The shape selects the kernel.  A reduction length (K forward, N input gradient) that is a multiple of 4 and at
+ * least 32 runs on the tensor cores (mma.sync tf32, 3xTF32); the call then packs w into `workspace`
+ * (dv_linear_packed_floats(N, K) floats, 16-byte aligned, the layout of dv_linear_pack_multi).  Other shapes run on
+ * the CUDA cores (FFMA); the query returns 0 for them and workspace may be NULL. */
 size_t dv_linear_fwd_workspace_bytes(int M, int N, int K);
 size_t dv_linear_dgrad_workspace_bytes(int M, int N, int K);
 int dv_linear_fwd(const float* x, const float* w, const float* bias, float* y, int M, int N, int K,

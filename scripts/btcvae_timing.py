@@ -35,7 +35,6 @@ for cold in (False, True):
     st, en = (timers[:, 0] - t0).float() / 1e3, (timers[:, 1] - t0).float() / 1e3
     print("   per-block global timer (us since the first block's entry): entry min/median/max %.2f %.2f %.2f | exit min/median/max %.2f %.2f %.2f"
           % (st.min(), st.median(), st.max(), en.min(), en.median(), en.max()))
-    v4 = os.environ.get("DV_BTCVAE_V4", "1") != "0"
-    names = ("(unused) | stage+fold | sweep | cluster.sync | finalise | exit sync" if v4 else "stage | bounds+fold | sweep | row stats | block sum | -")
+    names = "(unused) | stage+fold | sweep | cluster.sync | finalise | exit sync"
     print("cold" if cold else "warm", "event us %.2f" % us, "marks (clk since entry): %s =" % names, [int(m) for m in marks],
           " => us @1.9GHz:", [round(m / 1900, 2) for m in marks])

@@ -169,7 +169,7 @@ def test_library_loads_and_exports_every_declared_symbol():
     h = _native.lib()
     assert h.dv_built_arch() == 90 and h.dv_version() >= 100
     assert h.dv_status_string(-1).decode() == "unsupported shape"
-    assert h.dv_conv_packed_floats(32) == 2 * 32 * 32 * 16 + 2 * 16 * 64 * 32   # ffma + tensor-core (hi|lo) sections
+    assert h.dv_conv_packed_floats(32) == 2 * 16 * 64 * 32                       # tensor-core down, up sections (hi|lo)
     out = subprocess.run(["cuobjdump", "-lelf", _native.LIB_PATH], capture_output=True, text=True).stdout
     assert "sm_90a" in out
 

@@ -104,6 +104,10 @@ def test_conv_up_matches_conv_transpose2d(ops, B, H, CH, act):
     ref = F.conv_transpose2d(lo, w, b, stride=2, padding=1)
     ref = torch.relu(ref) if act == 1 else (torch.sigmoid(ref) if act == 2 else ref)
     wp = ops.conv_pack(w.to(dev()), CH)
+    if CH == 32 and act == 2:                                  # the sigmoid only ever follows the image layer
+        with pytest.raises(RuntimeError, match="bad argument"):
+            ops.conv_up(nhwc(lo).to(dev()), wp, b.to(dev()), None, B, H, H, CH, 0, act)
+        return
     hi = ops.conv_up(nhwc(lo).to(dev()), wp, b.to(dev()), None, B, H, H, CH, int(CH < 32), act)
     got = hi.cpu() if CH < 32 else nchw(hi.cpu())
     assert_close(got, ref, what="up")
@@ -115,9 +119,8 @@ def test_conv_up_matches_conv_transpose2d(ops, B, H, CH, act):
         hi3 = ops.conv_up(nhwc(lo).to(dev()), wp, None, nhwc(mask).to(dev()), B, H, H, CH, 0, 0,
                           mask_bits=relu_words(nhwc(mask).to(dev())))
         assert torch.equal(hi3, hi2)
-        if act != 2:
-            hi4, bits = ops.conv_up(nhwc(lo).to(dev()), wp, b.to(dev()), None, B, H, H, CH, 0, act, want_bits=True)
-            assert torch.equal(hi4, hi) and torch.equal(bits, relu_words(hi4))
+        hi4, bits = ops.conv_up(nhwc(lo).to(dev()), wp, b.to(dev()), None, B, H, H, CH, 0, act, want_bits=True)
+        assert torch.equal(hi4, hi) and torch.equal(bits, relu_words(hi4))
 
 
 @pytest.mark.parametrize("B,H,CH", CONV_CASES + [(64, 16, 32), (33, 32, 3)])
@@ -178,8 +181,8 @@ def test_conv32_kernels_fp32_grade_accuracy(ops, B, H):
 def test_conv_transpose_weight_gradient_is_same_kernel(ops):
     """dW of ConvTranspose2d(32 -> CH) == wgrad(lo = its input, hi = grad of its output)."""
     torch.manual_seed(3)
-    for CH in (3, 32):
-        B, H = 4, 8
+    for CH, H in ((3, 16), (32, 8)):                          # the decoder's last layer on 32x32 images, a 32->32 layer
+        B = 4
         lo = torch.randn(B, 32, H, H)
         w = torch.zeros(32, CH, 4, 4, requires_grad=True)
         g = torch.randn(B, CH, 2 * H, 2 * H)
@@ -187,6 +190,39 @@ def test_conv_transpose_weight_gradient_is_same_kernel(ops):
         hi = g.to(dev()) if CH < 32 else nhwc(g).to(dev())
         dw, _ = ops.conv_wgrad(nhwc(lo).to(dev()), hi, B, H, H, CH, int(CH < 32), False)
         assert_close(dw.cpu(), w.grad, what="convT dw CH=%d" % CH)
+
+
+def test_conv_entry_points_refuse_shapes_outside_the_burgess_layers():
+    """The conv entry points take exactly the layers of the Burgess networks on 32x32 and 64x64 images (CH in {1,3}:
+    lo 16 or 32; CH = 32: lo 4, 8 or 16; lo square) and refuse everything else before launching anything.  The image
+    layer's up kernel has no mask epilogue, so a float mask there is refused as well.  Every buffer is a real device
+    buffer of the size the geometry needs."""
+    from disvae import _native as N
+    L, st, p = N.lib(), N.stream(), (lambda t: t.data_ptr())
+    BAD_SHAPE, BAD_ARG = -1, -2
+
+    def buffers(B, H, W, CH):
+        hi = torch.randn(B * CH * 4 * H * W, device=dev())
+        lo = torch.randn(B * H * W * 32, device=dev())
+        wp = torch.zeros(L.dv_conv_packed_floats(CH), device=dev())
+        return hi, lo, wp
+
+    for B, H, W, CH in [(2, 8, 8, 3), (2, 64, 64, 1), (2, 32, 32, 32), (2, 8, 16, 32), (2, 32, 16, 3)]:
+        nchw = int(CH != 32)
+        hi, lo, wp = buffers(B, H, W, CH)
+        dw = torch.empty(32 * CH * 16, device=dev())
+        ws = torch.empty(2 * 132 * (16 * CH + 1) * 32, device=dev())
+        what = "B=%d H=%d W=%d CH=%d" % (B, H, W, CH)
+        assert L.dv_conv_down(p(hi), p(wp), None, None, p(lo), B, H, W, CH, nchw, 0, None, None, None, None, st) == BAD_SHAPE, what
+        assert L.dv_conv_up(p(lo), p(wp), None, None, p(hi), B, H, W, CH, nchw, 0, None, None, st) == BAD_SHAPE, what
+        assert L.dv_conv_wgrad_workspace_bytes(B, H, W, CH) == 0, what
+        assert L.dv_conv_wgrad(p(lo), p(hi), p(dw), None, p(ws), ws.numel() * 4, B, H, W, CH, nchw, st) == BAD_SHAPE, what
+    for CH in (1, 3):
+        B, H = 2, 16
+        hi, lo, wp = buffers(B, H, H, CH)
+        mask = torch.ones_like(hi)
+        assert L.dv_conv_up(p(lo), p(wp), None, p(mask), p(hi), B, H, H, CH, 1, 0, None, None, st) == BAD_ARG, CH
+    torch.cuda.synchronize()
 
 
 def test_channel_sum_and_transpose_and_act_bwd(ops):

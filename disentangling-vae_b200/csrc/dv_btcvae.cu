@@ -19,7 +19,6 @@
 //   * btcvae_bwd_kernel   -- rows role (g_z) and columns role (g_mu, g_logvar), same row-window semantics.
 // All exponent arithmetic is done in the log2 domain (c and hiv pre-multiplied by log2 e) so that each (i,j,d) costs
 // one MUFU.EX2 and no extra multiply; cross-lane merges are warp shuffles; every reduction has a fixed order.
-#include <stdlib.h>
 #include <cooperative_groups.h>
 #include "dv_common.cuh"
 
@@ -40,6 +39,13 @@ __device__ __forceinline__ float logw2(const LogW& w, int i, int j) {
   return (j == 1) ? w.ls : w.lm;
 }
 
+// A row's own Gaussian terms of one latent dim (natural-log units), added to the row's sums.
+__device__ __forceinline__ void add_row_gauss(float zz, float m, float lv, float& lq, float& lp) {
+  const float t = zz - m;
+  lq += -0.5f * (kLog2Pi + lv) - 0.5f * (t * t * expf(-lv));   // log N(z; mu, lv)   (math.py:48-51)
+  lp += -0.5f * kLog2Pi - 0.5f * (zz * zz);                      // log N(z; 0, 1)     (losses.py:531-532)
+}
+
 // rowstats is a structure of arrays [4 + D][B]: log_pz, log_qz, log_prod_qzi, log_q_zCx, P[d]
 // (natural-log units).  pj[d][b] = { c*log2e, hiv*log2e, mu, z } of batch row b.
 __global__ void btcvae_prep_kernel(const float* __restrict__ z, const float* __restrict__ mu, const float* __restrict__ logvar,
@@ -55,9 +61,7 @@ __global__ void btcvae_prep_kernel(const float* __restrict__ z, const float* __r
     const float cc = -0.5f * (kLog2Pi + lv);
     const float iv = expf(-lv);
     pj[(long long)d * B + row] = make_float4(cc * kLog2e, 0.5f * iv * kLog2e, m, zz);
-    const float t = zz - m;
-    lq += cc - 0.5f * (t * t * iv);                 // log N(z; mu, lv)      (math.py:48-51)
-    lp += -0.5f * kLog2Pi - 0.5f * (zz * zz);       // log N(z; 0, 0)        (losses.py:531-532)
+    add_row_gauss(zz, m, lv, lq, lp);
   }
   lq = warp_sum(lq); lp = warp_sum(lp);
   if (lane == 0) { rowstats[row] = lp; rowstats[3LL * B + row] = lq; }
@@ -74,14 +78,13 @@ __device__ __forceinline__ void lse_merge2(float& m, float& s, float m2, float s
 }
 
 // ------------------------------------------------------------------------------------------
-// Forward, second generation: (row-group x column-range) tiling.
-// The first kernel above streams every column's parameters through L1 for each group of 4 rows
-// (B/4 blocks x B*D*16 bytes x 2 sweeps = 82 MB of L2->SM traffic at (1024,10)) and is latency bound.
-// Here a block owns 32 rows (8 warps x 4 rows; the 8 lanes of a row split the columns) and ONE
-// column range of kJT columns whose parameters are staged once in shared memory (10 KB at D=10),
-// so both sweeps run out of shared memory with conflict-free 128-bit loads.  A block emits partial
-// logsumexp states (max, sum) per (row, dim) for its column range; btcvae_finalize_kernel merges
-// the ranges in a fixed order, forms the row statistics and the three means.  Grid: (B/32) x (B/kJT).
+// Forward for any D and any row window: (row-group x column-range) tiling.
+// A block owns 32 rows (8 warps x 4 rows; the 8 lanes of a row split the columns) and ONE column range
+// of kJT columns whose parameters are staged once in shared memory (10 KB at D=10, kJT=64), so every
+// row of the block reads them from shared memory with conflict-free 128-bit loads instead of from L2.
+// A block emits partial logsumexp states (max, sum) per (row, dim) for its column range;
+// btcvae_finalize_kernel merges the ranges in a fixed order, forms the row statistics and the three
+// means.  Grid: (nrows/32) x (B/kJT).
 // ------------------------------------------------------------------------------------------
 // JT = columns per block: 64 (8 per lane), or 16 (2 per lane) when (rows/32) x (B/64) blocks would leave most SMs idle
 // (B = 256: 32 blocks -> 128).
@@ -255,24 +258,23 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 
 // ------------------------------------------------------------------------------------------
-// Forward, version 4 (D <= 16): ONE launch, thread-block CLUSTERS of 4.
-// What limits version 3: every CTA stages the parameters of ALL B columns (176 KB per CTA of L2->smem
-// traffic, 176 KB smem CTAs) and every lane of a warp read a different column (LDS.128 with 32 distinct addresses =
-// 4 shared-memory wavefronts per 32 evaluations: the sweep was shared-memory-bandwidth bound).  Here
+// Forward for D <= 16 over the whole batch: ONE launch, thread-block CLUSTERS of 4.
 //   * a cluster of 4 CTAs owns R rows; CTA c of the cluster stages only ITS QUARTER of the columns (40 KB at
 //     (1024,10)) and sweeps those columns for all R rows; the four partial logsumexp states of every (row, dim) are
 //     merged through distributed shared memory after one cluster barrier -- no global-memory round trip, no second
 //     launch, nothing but the O(B*D) outputs touches HBM;
-//   * register blocking over ROWS: a lane owns columns (conflict-free LDS.128, odd float4 pitch) and applies each loaded
-//     column to RPT = 4 rows whose z_d and running sums it keeps in registers -- 4x less shared-memory traffic per
-//     evaluation (an LDS.128 is four shared-memory cycles whatever the addresses: broadcasting ACROSS lanes, the first
-//     attempt, bought nothing and its even pitch cost 2-way conflicts);
+//   * register blocking over ROWS: a lane owns columns and applies each loaded column to RPT rows whose z_d and
+//     running sums it keeps in registers, so one LDS.128 serves RPT evaluations.  An LDS.128 costs four shared-memory
+//     cycles whatever the addresses, so broadcasting one column ACROSS lanes would save nothing; lanes read
+//     consecutive columns instead, and the odd float4 pitch (DC + 1) keeps those reads conflict free where an even
+//     pitch gives 2-way conflicts;
 //   * the reference exponent is per CTA and per dimension (r_cd = max over the CTA's columns of c_jd + w_j, an
-//     upper bound of every term it sums), folded with the column weight into the staged constant as before
-//     (t = z - mu; arg = x'' - hiv*t*t; a += arg; s_d += ex2(arg)); partial sums of different CTAs are brought to
-//     the common exponent max_c r_cd in the merge.  log q(z): online logsumexp with one ex2 per column.
-//   * rows whose merged sum (nearly) underflows against the reference (outlier samples: best term > 60 nats below
-//     the column bound) are redone exactly (two passes straight from global memory) by the finalising warp.
+//     upper bound of every term it sums, so no ex2 and no sum can overflow), folded with the column weight into the
+//     staged constant (t = z - mu; arg = x'' - hiv*t*t; a += arg; s_d += ex2(arg)); partial sums of different CTAs
+//     are brought to the common exponent max_c r_cd in the merge.  log q(z): online logsumexp with one ex2 per column.
+//   * for an outlier sample (its best term > 60 nats below the column bound) ex2 flushes the terms against that bound
+//     to zero, so rows whose merged sum (nearly) underflows are redone exactly (two passes straight from global memory)
+//     by the finalising warp.
 // Rows of a cluster are finalised by its 4 CTAs round-robin (one warp per row: lanes = latent dims); the block's
 // contribution to the three means goes to `blockpart`, the last block adds them in block order (deterministic).
 // Clusters of 4 CTAs, rows spread over at most 32 of them (B = 1024: 32 rows per cluster).  32 is an estimate of how
@@ -283,6 +285,7 @@ constexpr int kF4Warps = kF4Threads / 32;
 constexpr int kF4Clus = 4;
 constexpr int kF4MaxTasks = 32;      // (row group of 4) x (column split) pairs per CTA
 constexpr int kF4MaxRows = 128;      // rows per cluster
+constexpr int kF4MaxSmem = 200 * 1024;   // dynamic shared memory opt-in (column stage)
 
 __device__ __forceinline__ void atomic_max_float(float* addr, float v) {   // shared memory; works for mixed signs
   if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
@@ -295,18 +298,9 @@ __global__ void __launch_bounds__(kF4Threads, 1)
 btcvae_fwd4_kernel(const float* __restrict__ z, const float* __restrict__ mu, const float* __restrict__ logvar, int ld,
                    int row_stride, int B, int D_rt, LogW lw, int R, int S, int NC, float4* __restrict__ pj_out,
                    float* __restrict__ rowstats, float* __restrict__ terms, float* __restrict__ blockpart,
-                   unsigned* __restrict__ counter, float* __restrict__ dbg) {
+                   unsigned* __restrict__ counter) {
   extern __shared__ float4 sp[];                               // [NC][DC+1]: {x'', hiv*log2e, mu, z} of this CTA's columns
   constexpr int DP = DC + 1;                                   // odd pitch: lanes over consecutive columns are conflict free
-  // DV_BTCVAE_TIMING=1: block 0 leaves its phase boundaries (SM clocks since kernel entry) in the workspace header
-  const long long t_start = dbg ? clock64() : 0;
-#define DV_F4_MARK(slot) do { if (dbg && blockIdx.x == 0 && threadIdx.x == 0) dbg[slot] = (float)(clock64() - t_start); } while (0)
-  // ... and every block its entry / exit time on the global nanosecond timer (dbg + 16 + 4*block: two 64-bit values)
-  if (dbg && threadIdx.x == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    reinterpret_cast<unsigned long long*>(dbg + 16)[2 * blockIdx.x] = t;
-  }
   __shared__ float s_ref[DC];                                  // r_cd (log2 units); -inf if the CTA owns no column
   __shared__ float s_rsum;                                     // sum_d r_cd
   __shared__ float s_tsx[kF4MaxTasks * kRows][DC];             // per (task, row) partial sums
@@ -365,7 +359,6 @@ btcvae_fwd4_kernel(const float* __restrict__ z, const float* __restrict__ mu, co
     }
     __syncthreads();
   }
-  DV_F4_MARK(1);
 
   // ---- phase 2: tasks = (group of RPT rows) x (column split); lanes = columns, RPT rows in registers ----
   {
@@ -435,7 +428,6 @@ btcvae_fwd4_kernel(const float* __restrict__ z, const float* __restrict__ mu, co
       }
     }
     __syncthreads();
-    DV_F4_MARK(2);
     // merge the column splits of every row in a fixed order -> this CTA's partial state
     for (int e = tid; e < R * (DC + 1); e += kF4Threads) {
       const int rr = e / (DC + 1), k = e - rr * (DC + 1);
@@ -452,7 +444,6 @@ btcvae_fwd4_kernel(const float* __restrict__ z, const float* __restrict__ mu, co
     }
   }
   cluster.sync();                                              // every CTA's s_sx / s_q / s_ref / s_rsum are final
-  DV_F4_MARK(3);
 
   // ---- phase 4: cluster rows round-robin over the 4 CTAs; one warp per row, lanes = latent dims ----
   for (int slot = warp; slot * kF4Clus + crank < R; slot += kF4Warps) {
@@ -493,31 +484,24 @@ btcvae_fwd4_kernel(const float* __restrict__ z, const float* __restrict__ mu, co
       for (int k = 0; k < D; ++k) {
         if (!((badmask >> k) & 1u)) continue;
         const float zk = z[(long long)i * D + k];
-        float mx = -INFINITY;
-        for (int j = lane; j < B; j += 32) {
+        auto term = [&](int j) {                               // m[i,j,k] + lw[i,j], log2 units
           const long long off = (long long)j * row_stride + (long long)k * ld;
           const float tt = zk - mu[off], lv = logvar[off];
-          mx = fmaxf(mx, (-0.5f * (kLog2Pi + lv) - 0.5f * (tt * tt) * expf(-lv)) * kLog2e + logw2(lw, i, j));
-        }
+          return (-0.5f * (kLog2Pi + lv) - 0.5f * (tt * tt) * expf(-lv)) * kLog2e + logw2(lw, i, j);
+        };
+        float mx = -INFINITY;
+        for (int j = lane; j < B; j += 32) mx = fmaxf(mx, term(j));
         mx = warp_max(mx);
         float sm = 0.f;
-        for (int j = lane; j < B; j += 32) {
-          const long long off = (long long)j * row_stride + (long long)k * ld;
-          const float tt = zk - mu[off], lv = logvar[off];
-          sm += exp2f((-0.5f * (kLog2Pi + lv) - 0.5f * (tt * tt) * expf(-lv)) * kLog2e + logw2(lw, i, j) - mx);
-        }
+        for (int j = lane; j < B; j += 32) sm += exp2f(term(j) - mx);
         sm = warp_sum(sm);
         if (lane == k) P2 = mx + log2f(sm);
       }
     }
-    // this row's own Gaussian terms: lanes over latent dims (same arithmetic as btcvae_prep_kernel)
     float lq = 0.f, lp = 0.f;
     for (int d = lane; d < D; d += 32) {
       const long long off = (long long)i * row_stride + (long long)d * ld;
-      const float m = mu[off], lv = logvar[off], zz = z[(long long)i * D + d];
-      const float tt = zz - m;
-      lq += -0.5f * (kLog2Pi + lv) - 0.5f * (tt * tt * expf(-lv));   // log N(z; mu, lv)   (math.py:48-51)
-      lp += -0.5f * kLog2Pi - 0.5f * (zz * zz);                      // log N(z; 0, 1)     (losses.py:531-532)
+      add_row_gauss(z[(long long)i * D + d], mu[off], logvar[off], lq, lp);
     }
     lq = warp_sum(lq); lp = warp_sum(lp);
     const float Pn = (lane < D) ? P2 * kLn2 : 0.f;
@@ -530,7 +514,6 @@ btcvae_fwd4_kernel(const float* __restrict__ z, const float* __restrict__ mu, co
     }
   }
   __syncthreads();
-  DV_F4_MARK(4);
   if (tid == 0) {
     float a = 0.f, b = 0.f, c = 0.f;
     for (int slot = 0; slot * kF4Clus + crank < R; ++slot) { a += s_means[slot][0]; b += s_means[slot][1]; c += s_means[slot][2]; }
@@ -539,13 +522,6 @@ btcvae_fwd4_kernel(const float* __restrict__ z, const float* __restrict__ mu, co
     is_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
   }
   cluster.sync();                                              // no CTA leaves while a peer may still read its shared memory
-  DV_F4_MARK(5);
-#undef DV_F4_MARK
-  if (dbg && threadIdx.x == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    reinterpret_cast<unsigned long long*>(dbg + 16)[2 * blockIdx.x + 1] = t;
-  }
   if (!is_last || warp != 0) return;
   __threadfence();
   float a = 0.f, b = 0.f, c = 0.f;
@@ -752,7 +728,6 @@ int dv_btcvae_fwd_rows(const float* z, const float* mu, const float* logvar, int
   float* ws = reinterpret_cast<float*>(workspace);
   cudaStream_t st = as_stream(stream);
   const LogW lw = make_logw(B, n_data, is_mss);
-  int rc;
   {
     // single-launch cluster path (D <= 16): columns split over the 4 CTAs of a cluster, rows over the clusters
     const int dc = D == 10 ? 10 : 16;
@@ -765,7 +740,7 @@ int dv_btcvae_fwd_rows(const float* z, const float* mu, const float* logvar, int
     int S = G >= kF4Warps ? 1 : kF4Warps / G;
     if (S > NC / 32) S = NC / 32;
     if (S < 1) S = 1;
-    if (whole && D <= 16 && smem <= 200 * 1024 && R <= kF4MaxRows && G * S <= kF4MaxTasks) {
+    if (whole && D <= 16 && smem <= kF4MaxSmem && R <= kF4MaxRows && G * S <= kF4MaxTasks) {
       const int nclus = (B + R - 1) / R;
       float4* pj = reinterpret_cast<float4*>(ws + kWsHeader);
       float* blockpart = ws + btcvae_part_offset_floats(B, D);
@@ -776,31 +751,23 @@ int dv_btcvae_fwd_rows(const float* z, const float* mu, const float* logvar, int
       attr[0].id = cudaLaunchAttributeClusterDimension;
       attr[0].val.clusterDim.x = kF4Clus; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
       cfg.attrs = attr; cfg.numAttrs = 1;
-      cudaError_t err = cudaSuccess;
-      static const int timing4 = [] { const char* e = getenv("DV_BTCVAE_TIMING"); return (e && e[0] == '1') ? 1 : 0; }();
-      float* dbg = timing4 ? blockpart + 4 * (nclus * kF4Clus) + 16 : nullptr;   // marks at dbg[0..5], per-block timers from dbg[16]
-#define DV_F4_CALL(DC, EXACT, RPT)                                                                                             \
-  do {                                                                                                                         \
-    static bool attr_set = false;                                                                                              \
-    if (!attr_set) {                                                                                                           \
-      if (cudaFuncSetAttribute(btcvae_fwd4_kernel<DC, EXACT, RPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != \
-          cudaSuccess) { g_last_cuda_error = (int)cudaGetLastError(); return DV_ERR_CUDA; }                                    \
-      attr_set = true;                                                                                                         \
-    }                                                                                                                          \
-    err = cudaLaunchKernelEx(&cfg, btcvae_fwd4_kernel<DC, EXACT, RPT>, z, mu, logvar, ld, row_stride, B, D, lw, R, S, NC, pj,  \
-                             rowstats, terms, blockpart, counter, dbg);                                                        \
-  } while (0)
-      if (D == 10) DV_F4_CALL(10, true, 4);
-      else if (D == 16) DV_F4_CALL(16, true, 2);
-      else DV_F4_CALL(16, false, 2);
-#undef DV_F4_CALL
-      if (err != cudaSuccess) { g_last_cuda_error = (int)err; cudaGetLastError(); return DV_ERR_CUDA; }
-      return check_launch();
+      auto launch = [&](auto kernel, bool* smem_set) -> int {
+        const int rc = set_max_dynamic_smem(kernel, kF4MaxSmem, smem_set);
+        if (rc != DV_OK) return rc;
+        const cudaError_t err = cudaLaunchKernelEx(&cfg, kernel, z, mu, logvar, ld, row_stride, B, D, lw, R, S, NC, pj,
+                                                   rowstats, terms, blockpart, counter);
+        if (err != cudaSuccess) { g_last_cuda_error = (int)err; cudaGetLastError(); return DV_ERR_CUDA; }
+        return check_launch();
+      };
+      static bool smem_set_10, smem_set_16, smem_set_16_any;
+      if (D == 10) return launch(btcvae_fwd4_kernel<10, true, 4>, &smem_set_10);
+      if (D == 16) return launch(btcvae_fwd4_kernel<16, true, 2>, &smem_set_16);
+      return launch(btcvae_fwd4_kernel<16, false, 2>, &smem_set_16_any);
     }
   }
   btcvae_prep_kernel<<<(B + 3) / 4, 128, 0, st>>>(z, mu, logvar, ld, row_stride, B, D,
                                                   reinterpret_cast<float4*>(ws + kWsHeader), rowstats);
-  rc = check_launch();
+  int rc = check_launch();
   if (rc != DV_OK) return rc;
   // small tiles only where the whole-batch rule reserved workspace for them
   const bool small = fwd2_small_tiles(B, nrows) && fwd2_small_tiles(B, B);

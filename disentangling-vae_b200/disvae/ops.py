@@ -500,31 +500,32 @@ class MlpFn(Function):
 # ---------------------------------------------------------------------------------------
 # reparameterisation (disvae/models/vae.py:65-68)
 # ---------------------------------------------------------------------------------------
-def _strides(mu, logvar):
-    """(ld, row_stride) if mu/logvar are [B,D] views with identical strides, else None."""
-    if mu.stride() == logvar.stride() and mu.dim() == 2:
-        return mu.stride(1), mu.stride(0)
-    return None
+def _mu_logvar(mu, logvar):
+    """-> (mu, logvar, ld, row_stride) as the C ABI takes them.  [B,D] views with identical strides (the two halves of
+    the encoder output) are passed as they are; anything else is made contiguous first."""
+    if mu.dim() != 2 or mu.stride() != logvar.stride():
+        mu, logvar = mu.contiguous(), logvar.contiguous()
+        if mu.dim() != 2 or mu.stride() != logvar.stride():
+            raise ValueError("mu and logvar must be [B, D] tensors of one shape, got %s and %s"
+                             % (tuple(mu.shape), tuple(logvar.shape)))
+    return mu, logvar, mu.stride(1), mu.stride(0)
 
 
 class ReparamFn(Function):
     @staticmethod
     def forward(ctx, mu, logvar, eps, seed, offset_dev):
         N.require_cuda_f32(mu, logvar, eps)
-        st = _strides(mu, logvar)
-        if st is None:
-            mu, logvar = mu.contiguous(), logvar.contiguous()
-            st = _strides(mu, logvar)
+        mu, logvar, ld, rs = _mu_logvar(mu, logvar)
         B, D = mu.shape
         z = _new((B, D), mu)
         if eps is not None:
             eps = _c(eps)
-            call("dv_reparam_fwd", ptr(mu), ptr(logvar), st[0], st[1], ptr(eps), 0, None, ptr(z), None, B, D, stream())
+            call("dv_reparam_fwd", ptr(mu), ptr(logvar), ld, rs, ptr(eps), 0, None, ptr(z), None, B, D, stream())
         else:
             eps = _new((B, D), mu)
-            call("dv_reparam_fwd", ptr(mu), ptr(logvar), st[0], st[1], None, seed, ptr(offset_dev), ptr(z), ptr(eps),
+            call("dv_reparam_fwd", ptr(mu), ptr(logvar), ld, rs, None, seed, ptr(offset_dev), ptr(z), ptr(eps),
                  B, D, stream())
-        ctx.st = st
+        ctx.st = (ld, rs)
         ctx.save_for_backward(logvar, eps)
         return z
 
@@ -549,29 +550,26 @@ class VaeLossFn(Function):
     def forward(ctx, recon, data, mu, logvar, dist):
         N.require_cuda_f32(recon, data, mu, logvar)
         recon, data = _c(recon), _c(data)
-        st = _strides(mu, logvar)
-        if st is None:
-            mu, logvar = mu.contiguous(), logvar.contiguous()
-            st = _strides(mu, logvar)
+        mu, logvar, ld, rs = _mu_logvar(mu, logvar)
         B, D = mu.shape
         n_img = recon.numel() // B
         ws = _zero_ws("vae_loss", N.lib().dv_vae_loss_workspace_bytes(B, n_img), recon.device)
         out = _new((2 + D,), recon)
-        call("dv_vae_loss_fwd", ptr(recon), ptr(data), n_img, B, dist, ptr(mu), ptr(logvar), st[0], st[1], D,
+        call("dv_vae_loss_fwd", ptr(recon), ptr(data), n_img, B, dist, ptr(mu), ptr(logvar), ld, rs, D,
              ptr(out), ptr(ws), stream())
-        ctx.meta = (n_img, B, D, dist, st)
+        ctx.meta = (n_img, B, D, dist, ld, rs)
         ctx.save_for_backward(recon, data, mu, logvar, out)
         return out
 
     @staticmethod
     def backward(ctx, g_out):
         recon, data, mu, logvar, out = ctx.saved_tensors
-        n_img, B, D, dist, st = ctx.meta
+        n_img, B, D, dist, ld, rs = ctx.meta
         g_out = _c(g_out)
         g_recon = torch.empty_like(recon) if ctx.needs_input_grad[0] else None
         g_mu = _new((B, D), mu) if ctx.needs_input_grad[2] else None
         g_lv = _new((B, D), mu) if ctx.needs_input_grad[3] else None
-        call("dv_vae_loss_bwd", ptr(recon), ptr(data), n_img, B, dist, ptr(mu), ptr(logvar), st[0], st[1], D,
+        call("dv_vae_loss_bwd", ptr(recon), ptr(data), n_img, B, dist, ptr(mu), ptr(logvar), ld, rs, D,
              ptr(out), ptr(g_out), ptr(g_recon), ptr(g_mu), ptr(g_lv), stream())
         return g_recon, None, g_mu, g_lv, None
 
@@ -585,18 +583,36 @@ class VaeLossFn(Function):
 _bt_pool = {}
 
 
+def _bt_new_workspace(B, D, device):
+    """A fresh beta-TCVAE workspace: only its 16-float header must start zero (include/disvae_b200.h)."""
+    ws = torch.empty((N.lib().dv_btcvae_workspace_bytes(B, D) + 3) // 4, dtype=torch.float32, device=device)
+    ws[:16].zero_()
+    return ws
+
+
 def _bt_workspace(B, D, device):
     key = (B, D, device.index)
     ent = _bt_pool.get(key)
     if ent is not None and not ent[1]:
         ent[1] = True
         return ent[0], key
-    nbytes = N.lib().dv_btcvae_workspace_bytes(B, D)
-    ws = torch.zeros((nbytes + 3) // 4, dtype=torch.float32, device=device)
+    ws = _bt_new_workspace(B, D, device)
     if ent is None:
         _bt_pool[key] = [ws, True]
         return ws, key
-    return ws, None                                            # pool buffer in flight: private, zero-filled
+    return ws, None                                            # pool buffer in flight: a private one
+
+
+def _btcvae_fwd(z, mu, logvar, n_data, is_mss, ws):
+    """dv_btcvae_fwd over the whole batch into workspace `ws` -> (rowstats [4+D, B], terms [3])."""
+    z = _c(z)
+    mu, logvar, ld, rs = _mu_logvar(mu, logvar)
+    B, D = z.shape
+    rowstats = _new((4 + D, B), z)
+    terms = _new((3,), z)
+    call("dv_btcvae_fwd", ptr(z), ptr(mu), ptr(logvar), ld, rs, B, D, int(n_data), int(bool(is_mss)),
+         ptr(rowstats), ptr(terms), ptr(ws), stream())
+    return rowstats, terms
 
 
 def _bt_release(key, ws):
@@ -611,17 +627,9 @@ class BtcvaeFn(Function):
     @staticmethod
     def forward(ctx, z, mu, logvar, n_data, is_mss):
         N.require_cuda_f32(z, mu, logvar)
-        z = _c(z)
-        st = _strides(mu, logvar)
-        if st is None:
-            mu, logvar = mu.contiguous(), logvar.contiguous()
-            st = _strides(mu, logvar)
         B, D = z.shape
         ws, key = _bt_workspace(B, D, z.device)
-        rowstats = _new((4 + D, B), z)
-        terms = _new((3,), z)
-        call("dv_btcvae_fwd", ptr(z), ptr(mu), ptr(logvar), st[0], st[1], B, D, int(n_data), int(bool(is_mss)),
-             ptr(rowstats), ptr(terms), ptr(ws), stream())
+        rowstats, terms = _btcvae_fwd(z, mu, logvar, n_data, is_mss, ws)
         if not (z.requires_grad or mu.requires_grad or logvar.requires_grad) or not torch.is_grad_enabled():
             _bt_release(key, ws)                               # no backward will come for it
             key = None
@@ -662,9 +670,7 @@ class BtcvaeGlobalFn(Function):
         gathered = parallel.all_gather_rows(torch.cat([z, mu, logvar], dim=1), group)       # [B, 3D]
         zg = gathered[:, :D].contiguous()
         mug, lvg = gathered[:, D:2 * D], gathered[:, 2 * D:]                                 # ld 1, row stride 3D
-        nbytes = N.lib().dv_btcvae_workspace_bytes(B, D)
-        ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=z.device)
-        ws[:16].zero_()
+        ws = _bt_new_workspace(B, D, z.device)
         rowstats = _new((4 + D, B), z)
         terms = _new((3,), z)
         call("dv_btcvae_fwd_rows", ptr(zg), ptr(mug), ptr(lvg), 1, 3 * D, B, D, rank * b, b, int(n_data), int(bool(is_mss)),
@@ -734,18 +740,8 @@ class LossCombineFn(Function):
 def btcvae_rowstats(z, mu, logvar, n_data, is_mss=True):
     """(log_pz, log_qz, log_prod_qzi, log_q_zCx) like losses.py:523-544 (no autograd)."""
     with torch.no_grad():
-        z = _c(z)
-        st = _strides(mu, logvar)
-        if st is None:
-            mu, logvar = mu.contiguous(), logvar.contiguous()
-            st = _strides(mu, logvar)
         B, D = z.shape
-        nbytes = N.lib().dv_btcvae_workspace_bytes(B, D)
-        ws = torch.zeros((nbytes + 3) // 4, dtype=torch.float32, device=z.device)
-        rowstats = _new((4 + D, B), z)
-        terms = _new((3,), z)
-        call("dv_btcvae_fwd", ptr(z), ptr(mu), ptr(logvar), st[0], st[1], B, D, int(n_data), int(bool(is_mss)),
-             ptr(rowstats), ptr(terms), ptr(ws), stream())
+        rowstats, _ = _btcvae_fwd(z, mu, logvar, n_data, is_mss, _bt_new_workspace(B, D, z.device))
     return rowstats[0], rowstats[1], rowstats[2], rowstats[3]
 
 

@@ -63,6 +63,8 @@ SIGNATURES = {
     "dv_latent_entropy_workspace_bytes": (SZ, [I, I, I]),
     "dv_latent_entropy": (I, [P, P, P, I, I, I, I, I, P, P, P, P]),
     "dv_permute_dims": (I, [P, P, ULL, P, P, I, I, P]),
+    "dv_permute_dims_workspace_bytes": (SZ, [I, I]),
+    "dv_permute_dims_rows": (I, [P, P, ULL, P, P, I, I, I, I, P, P]),
     "dv_factor_tc_fwd": (I, [P, I, P, P]),
     "dv_factor_tc_bwd": (I, [P, I, P, P]),
     "dv_factor_ce_fwd": (I, [P, P, I, P, P]),

@@ -153,6 +153,13 @@ class FactorKLoss(BaseLoss):
         self._perm_offset = None
         self._perm_queue = []          # injected permutations (parity tests), consumed FIFO
         self._fused_d = None           # FusedAdam over optimizer_d (built lazily once the discriminator is on CUDA)
+        # Data parallel only (no meaning for one process): False = every rank permutes its own second half-batch (the
+        # reference handed that shard as its batch, SURVEY.md 8e); True = every rank takes its rows of ONE permutation of
+        # the all-gathered second halves, so the "product of marginals" samples no longer depend on the number of ranks.
+        # DISVAE_GLOBAL_FACTOR=1 turns it on without touching main.py.
+        import os
+        self.global_batch = os.environ.get("DISVAE_GLOBAL_FACTOR") == "1"
+        self._gperm_offset = None
 
     def _step_d(self):
         """Discriminator Adam step: dv_adam_multi when optimizer_d is a plain CUDA Adam."""
@@ -174,9 +181,32 @@ class FactorKLoss(BaseLoss):
             self._perm_offset = torch.zeros(1, dtype=torch.int64, device=device)
         return self._perm_seed, self._perm_offset
 
+    def _global_perm_state(self, device):
+        """Key of the global permutation: rank 0's seed, unsalted (one process with the same seed draws the same
+        permutation), and an offset that advances by world*h*D on every rank."""
+        if self._gperm_offset is None or self._gperm_offset.device != device:
+            from disvae.parallel import broadcast_u64
+            self._gperm_seed = broadcast_u64(int(torch.initial_seed()) ^ 0x9E3779B97F4A7C15)
+            self._gperm_offset = torch.zeros(1, dtype=torch.int64, device=device)
+        return self._gperm_seed, self._gperm_offset
+
+    def _permute_global(self, latent_sample2, perms=None):
+        """This rank's rows [rank*h, (rank+1)*h) of the permutation of the second halves of all ranks, rank-major.
+        `perms`: injected global permutations [D, world*h]."""
+        import torch.distributed as dist
+        from disvae.parallel import all_gather_rows, check_equal_rows
+        h = latent_sample2.size(0)
+        check_equal_rows(h)                                      # before the gather: unequal sizes would hang it
+        z2_all = all_gather_rows(latent_sample2)
+        row0 = dist.get_rank() * h
+        if perms is not None:
+            return ops.permute_dims_rows(z2_all, row0, h, perms)
+        seed, off = self._global_perm_state(latent_sample2.device)
+        return ops.permute_dims_rows(z2_all, row0, h, None, seed, off)
+
     def call_optimize(self, data, model, optimizer, storer, eps1=None, eps2=None, perms=None, step_optimizers=True):
         """losses.py:243-313.  `eps1`/`eps2`/`perms` optionally inject the noise of the two
-        halves and the per-dimension permutations ([D, B/2] int64) for parity tests.
+        halves and the per-dimension permutations ([D, B/2] int64; [D, world*B/2] in global-batch mode) for parity tests.
         `step_optimizers=False` (data parallel): both backward passes run, neither optimizer steps -- the
         Trainer steps them after the gradients of all ranks are averaged."""
         storer = self._pre_call(model.training, storer)
@@ -207,7 +237,10 @@ class FactorKLoss(BaseLoss):
             latent_sample2 = model.sample_latent(data2, eps=eps2)
             if perms is None and self._perm_queue:
                 perms = self._perm_queue.pop(0)
-            if perms is None:
+            from disvae.parallel import is_distributed
+            if self.global_batch and is_distributed():
+                z_perm = self._permute_global(latent_sample2, perms)
+            elif perms is None:
                 seed, off = self._perm_state(latent_sample2.device)
                 z_perm = ops.permute_dims(latent_sample2, None, seed, off)
             else:

@@ -748,16 +748,38 @@ def btcvae_rowstats(z, mu, logvar, n_data, is_mss=True):
 # ---------------------------------------------------------------------------------------
 # FactorVAE heads (losses.py:265, 291-295, 483-508)
 # ---------------------------------------------------------------------------------------
+_PERM_MAX_B = 4096      # dv_permute_dims generates device permutations of at most this many rows
+
+
 def permute_dims(z, perms=None, seed=0, offset_dev=None):
     N.require_cuda_f32(z)
     z = _c(z.detach())
     B, D = z.shape
+    if perms is None and B > _PERM_MAX_B:
+        return permute_dims_rows(z, 0, B, None, seed, offset_dev)
     out = torch.empty_like(z)
     if perms is not None:
         perms = perms.to(device=z.device, dtype=torch.int64).contiguous()
         call("dv_permute_dims", ptr(z), ptr(perms), 0, None, ptr(out), B, D, stream())
     else:
         call("dv_permute_dims", ptr(z), None, seed, ptr(offset_dev), ptr(out), B, D, stream())
+    return out
+
+
+def permute_dims_rows(z, row0, nrows, perms=None, seed=0, offset_dev=None):
+    """Rows [row0, row0 + nrows) of permute_dims(z, perms, seed, offset_dev), at any batch size: the permutation is
+    the one of all B rows of z, and the device offset advances by B*D whatever the window."""
+    N.require_cuda_f32(z)
+    z = _c(z.detach())
+    B, D = z.shape
+    out = torch.empty((nrows, D), dtype=torch.float32, device=z.device)
+    if perms is not None:
+        perms = perms.to(device=z.device, dtype=torch.int64).contiguous()
+        call("dv_permute_dims_rows", ptr(z), ptr(perms), 0, None, ptr(out), B, D, row0, nrows, None, stream())
+    else:
+        nbytes = N.lib().dv_permute_dims_workspace_bytes(B, D)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=z.device) if nbytes else None
+        call("dv_permute_dims_rows", ptr(z), None, seed, ptr(offset_dev), ptr(out), B, D, row0, nrows, ptr(ws), stream())
     return out
 
 

@@ -105,10 +105,10 @@ def broadcast_parameters(module, src=0):
 
 
 # ---------------------------------------------------------------------------------------------------------
-# Row collectives for the global-batch beta-TCVAE estimator (SURVEY.md 8f-1): every rank contributes the same number
-# of rows.  NCCL: one all_gather_into_tensor / reduce_scatter_tensor.  gloo (CPU tests; CUDA tensors of ranks that
-# share one GPU in tests/ddp_worker.py) has neither for CUDA tensors nor reduce_scatter at all: staged through an
-# all_gather / all_reduce on the host, same results.
+# Row collectives for the global-batch beta-TCVAE estimator (SURVEY.md 8f-1) and FactorVAE permutation: every rank
+# contributes the same number of rows.  NCCL: one all_gather_into_tensor / reduce_scatter_tensor.  gloo (CPU tests;
+# CUDA tensors of ranks that share one GPU in tests/ddp_worker.py) has neither for CUDA tensors nor reduce_scatter at
+# all: staged through an all_gather / all_reduce on the host, same results.
 # ---------------------------------------------------------------------------------------------------------
 def _backend(group=None):
     return dist.get_backend(group)
@@ -126,6 +126,31 @@ def all_gather_rows(t, group=None):
     parts = [torch.empty_like(host) for _ in range(world)]
     dist.all_gather(parts, host, group=group)
     return torch.cat(parts, dim=0).to(t.device)
+
+
+def _small_tensor(values, group=None):
+    """int64 tensor for a small collective: on the current GPU for NCCL, on the host for gloo."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if _backend(group) == "nccl" else torch.device("cpu")
+    return torch.tensor(values, dtype=torch.int64, device=dev)
+
+
+def check_equal_rows(n, group=None):
+    """Raise RuntimeError unless every rank passes the same row count `n` (one MAX all-reduce of (n, -n)).  The row
+    collectives need equal blocks: all_gather_into_tensor with mismatched sizes hangs or mixes up rows."""
+    t = _small_tensor([n, -n], group)
+    dist.all_reduce(t, op=dist.ReduceOp.MAX, group=group)
+    hi, lo = int(t[0]), -int(t[1])
+    if hi != lo:
+        raise RuntimeError("data parallel: the ranks hold different numbers of rows (from %d to %d; this rank %d); "
+                           "the global-batch losses need equal shards" % (lo, hi, n))
+
+
+def broadcast_u64(value, src=0, group=None):
+    """Rank `src`'s unsigned 64-bit integer on every rank (e.g. a Philox key all ranks must share)."""
+    v = int(value) & 0xFFFFFFFFFFFFFFFF
+    t = _small_tensor([v - (1 << 64) if v >= (1 << 63) else v], group)
+    dist.broadcast(t, src=src, group=group)
+    return int(t[0]) & 0xFFFFFFFFFFFFFFFF
 
 
 def reduce_scatter_rows(t, group=None):

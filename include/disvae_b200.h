@@ -247,10 +247,24 @@ int dv_latent_entropy(const float* zs, const float* mean, const float* logvar, i
 /* ---- FactorVAE pieces ---------------------------------------------------------------------
  * dv_permute_dims replaces _permute_dims (losses.py:483-508): out[b][d] = z[perm[d][b]][d].
  * perms != NULL: int64 [D][B] (the reference's CPU randperm stream, trap T7).  perms == NULL:
- * per-dimension Philox-keyed random permutation generated on the device (B <= 4096).
+ * per-dimension Philox-keyed random permutation generated on the device (B <= 4096; larger B through
+ * dv_permute_dims_rows).
  */
 int dv_permute_dims(const float* z, const long long* perms, unsigned long long seed,
                     unsigned long long* offset_dev, float* out, int B, int D, void* stream);
+/* Row-window form of _permute_dims (losses.py:483-508) at any B, for the FactorVAE permutation of a half-batch
+ * all-gathered from several GPUs (SURVEY.md 8e): z holds all B rows, only rows [row0, row0 + nrows) of the permuted
+ * matrix are written, out[i][d] = z[pi_d(row0 + i)][d] for 0 <= i < nrows (out is [nrows][D]).
+ * perms != NULL: pi_d = perms[d] (int64 [D][B]).  perms == NULL: pi_d is the order that sorts the keys
+ * (philox4x32_10(*offset_dev + d*B + b, seed).x << 32) | b ascending -- the permutation dv_permute_dims draws --
+ * and *offset_dev advances by B*D whatever the window, so the windows of one call on every rank agree.
+ * Device permutations with B > 4096 sort through `workspace` (dv_permute_dims_workspace_bytes, 8-byte aligned,
+ * contents irrelevant); below that it may be NULL.  Deterministic, host-synchronisation free, graph-capturable.
+ * DV_ERR_BAD_SHAPE: B < 1, D < 1, row0 < 0, nrows < 1, row0 + nrows > B or B*D > INT_MAX. */
+size_t dv_permute_dims_workspace_bytes(int B, int D);   /* 0 when B <= 4096 */
+int dv_permute_dims_rows(const float* z, const long long* perms, unsigned long long seed,
+                         unsigned long long* offset_dev, float* out, int B, int D, int row0, int nrows,
+                         void* workspace, void* stream);
 /* tc[0] = mean(d_z[:,0] - d_z[:,1])  (losses.py:265) */
 int dv_factor_tc_fwd(const float* d_z, int h, float* tc, void* stream);
 int dv_factor_tc_bwd(const float* upstream, int h, float* g_d_z, void* stream);

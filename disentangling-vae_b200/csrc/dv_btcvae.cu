@@ -96,7 +96,9 @@ constexpr int kRG = 32;            // rows per block
 // (log2 units).  The bound max_j (c_j + w_j) >= every term, so exp2(term - ref) <= 2^60 never overflows;
 // the diagonal term (always part of the sum) keeps the row's total from underflowing; a block whose terms
 // all underflow against its own bound contributes (ref, 0), which the merge treats as the identity -- such
-// terms are < 2^-66 of the block bound and far below the diagonal term.  One MUFU.EX2, ~8 FP32 ops per (i,j,d).
+// terms are < 2^-66 of the block bound and, unless row i is an outlier, far below the diagonal term.  When every term
+// of a (row, dim) underflows, diagonal included, btcvae_finalize_kernel redoes it exactly.
+// One MUFU.EX2, ~8 FP32 ops per (i,j,d).
 template <int DC, bool EXACT, int kJT>
 __global__ void __launch_bounds__(kBtWarps * 32)
 btcvae_fwd2_kernel(int B, int D, int row0, int nrows, LogW lw, const float4* __restrict__ pj, float2* __restrict__ part) {
@@ -201,11 +203,31 @@ btcvae_fwd2_kernel(int B, int D, int row0, int nrows, LogW lw, const float4* __r
   if (jl == 0 && i_raw < row_end) part[((long long)js * (D + 1) + D) * B + i] = make_float2(am, as);
 }
 
+// Exact two-pass logsumexp_j (m[i,j,d] + lw[i,j]) in log2 units, from the column parameters pjd = pj[d][.].
+__device__ __forceinline__ float exact_lse2(int B, int i, const float4* __restrict__ pjd, LogW lw) {
+  const float zi = pjd[i].w;
+  auto term = [&](int j) {
+    const float4 p = pjd[j];
+    const float t = zi - p.z;
+    return p.x - p.y * (t * t) + logw2(lw, i, j);
+  };
+  float mx = -INFINITY;
+  for (int j = 0; j < B; ++j) mx = fmaxf(mx, term(j));
+  float s = 0.f;
+  for (int j = 0; j < B; ++j) s += exp2f(term(j) - mx);
+  return mx + log2f(s);
+}
+
 // merge the column ranges in a fixed order: 16 lanes per row (lane l owns dims l, l+16, ... and lane
 // D%16.. the log_qz slot), rowstats rows 1, 2, 4.. written per row; the last block forms the three means.
+// A (row, dim) whose terms all lie far below its blocks' reference exponents (an outlier sample) has lost them to
+// exp2f's underflow, the diagonal one included; a merged value more than 90 log2 units below the largest block
+// reference (or no value at all) is redone exactly from pj.  Terms flushed against a reference are < 2^-126 of it,
+// so a merged value above that bar has lost at most B * 2^-36 of itself.
 __global__ void __launch_bounds__(256)
-btcvae_finalize_kernel(int B, int D, int row0, int nrows, int JS, const float2* __restrict__ part,
-                       float* __restrict__ rowstats, float* __restrict__ terms, unsigned* __restrict__ counter) {
+btcvae_finalize_kernel(int B, int D, int row0, int nrows, int JS, LogW lw, const float4* __restrict__ pj,
+                       const float2* __restrict__ part, float* __restrict__ rowstats, float* __restrict__ terms,
+                       unsigned* __restrict__ counter) {
   __shared__ bool is_last;
   const int gl = threadIdx.x & 15;
   const int i = row0 + blockIdx.x * 16 + (threadIdx.x >> 4);
@@ -214,12 +236,15 @@ btcvae_finalize_kernel(int B, int D, int row0, int nrows, int JS, const float2* 
   if (i < row_end) {
     for (int d = gl; d <= D; d += 16) {
       float2 st = part[(long long)d * B + i];
-      float m = st.x, s = st.y;
+      float m = st.x, s = st.y, mref = st.x;
       for (int js = 1; js < JS; ++js) {
         st = part[((long long)js * (D + 1) + d) * B + i];
+        mref = fmaxf(mref, st.x);
         lse_merge2(m, s, st.x, st.y);
       }
-      const float v = (m + log2f(s)) * kLn2;
+      float v2 = m + log2f(s);
+      if (d < D && !(v2 > mref - 90.f)) v2 = exact_lse2(B, i, pj + (long long)d * B, lw);
+      const float v = v2 * kLn2;
       if (d < D) { rowstats[(long long)(4 + d) * B + i] = v; lprod += v; }
       else rowstats[1LL * B + i] = v;                         // log_qz
     }
@@ -283,6 +308,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
 constexpr int kF4Threads = 512;
 constexpr int kF4Warps = kF4Threads / 32;
 constexpr int kF4Clus = 4;
+constexpr int kF4MaxClusters = 32;   // the rows are spread over at most this many clusters
 constexpr int kF4MaxTasks = 32;      // (row group of 4) x (column split) pairs per CTA
 constexpr int kF4MaxRows = 128;      // rows per cluster
 constexpr int kF4MaxSmem = 200 * 1024;   // dynamic shared memory opt-in (column stage)
@@ -704,12 +730,15 @@ static bool fwd2_small_tiles(int B, int nrows) {
   return (long long)((nrows + kRG - 1) / kRG) * ((B + kJTBig - 1) / kJTBig) < kNumSMs && B <= 1024;
 }
 // header | float4 pj[D][B] | float2 part[ceil(B/JT)][D+1][B]
+// The cluster path keeps its per-CTA partial means (4 floats per CTA) where `part` goes; at tiny B * D that is more
+// than `part` itself.
 static long long btcvae_part_offset_floats(int B, int D) { return kWsHeader + 4LL * B * D; }
 size_t dv_btcvae_workspace_bytes(int B, int D) {
   const long long JS = (B + kJTSmall - 1) / kJTSmall;          // room for either column tile width when B is small
   const long long JS_big = (B + kJTBig - 1) / kJTBig;
   const long long js = fwd2_small_tiles(B, B) ? JS : JS_big;
-  return (size_t)(btcvae_part_offset_floats(B, D) + 2LL * js * (D + 1) * B) * sizeof(float);
+  const long long part = std::max(2LL * js * (D + 1) * B, 4LL * kF4Clus * kF4MaxClusters);
+  return (size_t)(btcvae_part_offset_floats(B, D) + part) * sizeof(float);
 }
 
 int dv_btcvae_fwd(const float* z, const float* mu, const float* logvar, int ld, int row_stride, int B, int D,
@@ -731,8 +760,8 @@ int dv_btcvae_fwd_rows(const float* z, const float* mu, const float* logvar, int
   {
     // single-launch cluster path (D <= 16): columns split over the 4 CTAs of a cluster, rows over the clusters
     const int dc = D == 10 ? 10 : 16;
-    const int max_clusters = 32;                               // estimated 4-CTA cluster capacity of a 132-SM H100 (see above)
-    int R = ((B + max_clusters - 1) / max_clusters + kRows - 1) / kRows * kRows;
+    // kF4MaxClusters: estimated 4-CTA cluster capacity of a 132-SM H100 (see above)
+    int R = ((B + kF4MaxClusters - 1) / kF4MaxClusters + kRows - 1) / kRows * kRows;
     const int NC = ((B + kF4Clus - 1) / kF4Clus + kJL - 1) / kJL * kJL;
     const size_t smem = (size_t)NC * (dc + 1) * sizeof(float4);
     const int rpt = (dc == 10) ? 4 : 2;                        // rows per thread (register budget)
@@ -788,7 +817,7 @@ int dv_btcvae_fwd_rows(const float* z, const float* mu, const float* logvar, int
 #undef DV_FWD2
   rc = check_launch();
   if (rc != DV_OK) return rc;
-  btcvae_finalize_kernel<<<(nrows + 15) / 16, 256, 0, st>>>(B, D, row0, nrows, JS, part, rowstats, terms,
+  btcvae_finalize_kernel<<<(nrows + 15) / 16, 256, 0, st>>>(B, D, row0, nrows, JS, lw, pjc, part, rowstats, terms,
                                                             reinterpret_cast<unsigned*>(ws));
   return check_launch();
 }

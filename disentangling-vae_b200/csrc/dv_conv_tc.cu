@@ -28,14 +28,16 @@ constexpr int kSmemMax = 232448;             // 227 KB per block on sm_90
 
 __device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers * 32) : "memory"); }
 
-// Four B fragments (hi and lo planes) of k slice ks for output columns nt*8 + g, from a packed-weight tap:
-// 64 rows x 128 B, rows [0,32) hi and [32,64) lo of the N-by-K (K contiguous) weight.
-__device__ __forceinline__ void load_b_tap(uint32_t tap_base, int nt, int ks, int g, int t, uint32_t (&bh)[2], uint32_t (&bl)[2]) {
-  const int n = nt * 8 + g;
-  bh[0] = lds32(tap_base + swz128(n, 8 * ks + t));
-  bh[1] = lds32(tap_base + swz128(n, 8 * ks + t + 4));
-  bl[0] = lds32(tap_base + swz128(32 + n, 8 * ks + t));
-  bl[1] = lds32(tap_base + swz128(32 + n, 8 * ks + t + 4));
+// The B fragments (hi and lo planes) of k slice ks for output columns nt*8 + g, from a packed-weight tap:
+// 64 rows x 128 B, rows [0,32) hi and [32,64) lo of the N-by-K (K contiguous) weight.  ONE ldmatrix .x4 instead of four
+// 32-bit loads: matrices {hi, k 0-3}, {hi, k 4-7}, {lo, k 0-3}, {lo, k 4-7} of the 8 columns; lane l gives the address
+// of row b_row = (l >> 4) * 32 + (l & 7) (+ 8 nt), column b_col = ((l >> 3) & 1) * 4 (b_lane_row / b_lane_col).
+__device__ __forceinline__ int b_lane_row(int lane) { return (lane >> 4) * 32 + (lane & 7); }
+__device__ __forceinline__ int b_lane_col(int lane) { return (lane & 8) >> 1; }
+__device__ __forceinline__ void load_b_tap(uint32_t tap_base, int nt, int ks, int b_row, int b_col, uint32_t (&bh)[2], uint32_t (&bl)[2]) {
+  uint32_t r[4];
+  ldsm_x4(tap_base + swz128(b_row + 8 * nt, 8 * ks + b_col), r);
+  bh[0] = r[0]; bh[1] = r[1]; bl[0] = r[2]; bl[1] = r[3];
 }
 
 // ------------------------------------------------------------------------------------------
@@ -106,6 +108,7 @@ conv_down32_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   }
 
   const int gq = lane >> 2, t = lane & 3;
+  const int b_row = b_lane_row(lane), b_col = b_lane_col(lane);
   const int r0 = warp * 16 + gq;                             // this thread's tile rows: r0 and r0 + 8
   const uint32_t bs = smem_u32(Bs), raw0 = smem_u32(Raw);
   float csum[4][2] = {};                                     // channel sums of the stored output (colsum_part)
@@ -129,7 +132,7 @@ conv_down32_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) {
           uint32_t bh[2], bl[2];
-          load_b_tap(b_base, nt, ks, gq, t, bh, bl);
+          load_b_tap(b_base, nt, ks, b_row, b_col, bh, bl);
           mma_3xtf32(mn[nt], corr[nt], ah, al, bh, bl);
         }
       }
@@ -406,6 +409,7 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
   }
 
   const int gq = lane >> 2, t = lane & 3;
+  const int b_row = b_lane_row(lane), b_col = b_lane_col(lane);
   const int HH = 2 * g.H, WW = 2 * g.W;
   const uint32_t bs = smem_u32(Bs), raw0 = smem_u32(Raw);
   // the two MMA rows of this thread (r = 16*warp + gq + 8h): centre pixel inside the resident box [TB][TR+2][W]
@@ -458,7 +462,7 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
 #pragma unroll
           for (int nt = 0; nt < 4; ++nt) {
             uint32_t bh[2], bl[2];
-            load_b_tap(b_base, nt, ks, gq, t, bh, bl);
+            load_b_tap(b_base, nt, ks, b_row, b_col, bh, bl);
             mma_3xtf32(mn[nt], corr[nt], ah, al, bh, bl);
           }
         }

@@ -49,6 +49,16 @@ __device__ __forceinline__ uint32_t lds32(uint32_t smem_addr) {
   return v;
 }
 
+// Four 8x8 b16 matrices (ldmatrix .x4): lane l gives the 16-byte row address of row l & 7 of matrix l >> 3, and
+// register j of lane l receives 32-bit word l & 3 of row l >> 2 of matrix j.  Read as 32-bit data, that is exactly the
+// tf32 m16n8k8 fragment layout: one instruction for a whole A fragment, or for the hi and lo B fragments of 8 columns.
+__device__ __forceinline__ void ldsm_x4(uint32_t smem_addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(smem_addr)
+               : "memory");
+}
+
 // Byte offset of fp32 element (row r, column c < 32) in a tile of 128-byte rows written by TMA with
 // CU_TENSOR_MAP_SWIZZLE_128B into a 1024-byte aligned buffer: the 16-byte chunk index is XOR-ed with (r & 7).
 __device__ __forceinline__ uint32_t swz128(int r, int c) {

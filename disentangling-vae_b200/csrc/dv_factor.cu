@@ -97,7 +97,7 @@ permute_merge_kernel(const unsigned long long* __restrict__ src, unsigned long l
     const unsigned long long k = s[i];
     int lo = p0, hi = p1;                              // ends as p0 + (keys of the partner run below k)
     while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
+      const int mid = (int)(((unsigned)lo + (unsigned)hi) >> 1);   // no int overflow for runs near INT_MAX
       if (s[mid] < k) lo = mid + 1; else hi = mid;
     }
     dst[(long long)d * B + pair0 + (i - run * w) + (lo - p0)] = k;
@@ -113,6 +113,12 @@ __global__ void permute_sorted_gather_kernel(const float* __restrict__ z, const 
     const long long src = (long long)(sorted[(long long)d * B + row0 + b] & 0xffffffffull);
     out[i] = z[src * D + d];
   }
+}
+// In place over the fully sorted keys of one dimension: key i becomes its row index as int64 (keys and idx alias).
+__global__ void sorted_index_column_kernel(unsigned long long* keys, int n) {
+  long long* idx = reinterpret_cast<long long*>(keys);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    idx[i] = (long long)(keys[i] & 0xffffffffull);
 }
 __global__ void advance_offset2_kernel(unsigned long long* offset_dev, unsigned long long by) { *offset_dev += by; }
 
@@ -238,6 +244,38 @@ int dv_permute_dims_rows(const float* z, const long long* perms, unsigned long l
   }
   if (rc != DV_OK) return rc;
   advance_offset2_kernel<<<1, 1, 0, st>>>(offset_dev, (unsigned long long)B * D);
+  return check_launch();
+}
+
+size_t dv_index_permutation_workspace_bytes(int N) {
+  return N > kPermMaxB ? (size_t)N * sizeof(unsigned long long) : 0;
+}
+
+int dv_index_permutation(int N, unsigned long long seed, unsigned long long* offset_dev, long long* out_idx,
+                         void* workspace, void* stream) {
+  if (N < 1) return DV_ERR_BAD_SHAPE;
+  if (!offset_dev || !out_idx || (reinterpret_cast<uintptr_t>(out_idx) & 7)) return DV_ERR_BAD_ARG;
+  int passes = 0;
+  for (long long w = kPermMaxB; w < N; w *= 2) ++passes;
+  if (passes > 0 && (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 7))) return DV_ERR_BAD_ARG;
+  // The key buffers ping-pong between out_idx (N x 8 bytes, like the keys) and the workspace; the tile pass writes to
+  // the one that makes the last merge pass land in out_idx, where the index column is then extracted in place.
+  unsigned long long* out_keys = reinterpret_cast<unsigned long long*>(out_idx);
+  unsigned long long* ws = static_cast<unsigned long long*>(workspace);
+  unsigned long long* buf[2] = {(passes & 1) ? ws : out_keys, (passes & 1) ? out_keys : ws};
+  cudaStream_t st = as_stream(stream);
+  permute_tile_sort_kernel<<<dim3((N + kPermMaxB - 1) / kPermMaxB, 1), 512, 0, st>>>(seed, offset_dev, buf[0], N, 1);
+  int rc = check_launch();
+  int cur = 0;
+  for (long long w = kPermMaxB; w < N && rc == DV_OK; w *= 2, cur ^= 1) {
+    permute_merge_kernel<<<dim3((N + 255) / 256, 1), 256, 0, st>>>(buf[cur], buf[cur ^ 1], N, 1, (int)w);
+    rc = check_launch();
+  }
+  if (rc != DV_OK) return rc;
+  sorted_index_column_kernel<<<(int)std::min<long long>((N + 255) / 256, 8 * kNumSMs), 256, 0, st>>>(out_keys, N);
+  rc = check_launch();
+  if (rc != DV_OK) return rc;
+  advance_offset2_kernel<<<1, 1, 0, st>>>(offset_dev, (unsigned long long)N);
   return check_launch();
 }
 

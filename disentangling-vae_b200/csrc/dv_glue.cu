@@ -3,15 +3,25 @@
 //
 //   dv_u8_to_f32          uint8 image batch -> fp32 / 255  (torchvision ToTensor semantics, utils/datasets.py:182,247,
 //                         364-367: `img.float().div(255)`), so a host batch travels over PCIe as bytes (4x less H2D)
+//   dv_gather_u8_to_f32   the same conversion of rows picked by an index list from a device-resident uint8 dataset:
+//                         one training batch per launch (disvae.data.DeviceLoader)
 //   dv_loss_combine_*     loss = sum_i ca[i]*a[i] + sum_j cb[j]*b[j] for two short device vectors (the fused loss kernel's
 //                         (rec, kl, ...) and the beta-TCVAE (mi, tc, dw_kl)): losses.py:151, 199-200, 381-382 as ONE
 //                         launch forward and ONE backward instead of ~10 scalar mul/add/select kernels and their
 //                         zero-filled gradient buffers
 //   dv_act_bwd_chansum    ConvTranspose2d output layer backward prologue: g = dy * act'(y) (decoders.py:82 sigmoid) fused
 //                         with the per-channel sum of g (that layer's bias gradient) -- one pass instead of two
+#include <algorithm>
 #include "dv_common.cuh"
 
 namespace dv {
+
+// torchvision ToTensor's byte -> float: true division, like Tensor.div(255) (not a multiply by 1/255)
+__device__ __forceinline__ float u8_to_unit(uint32_t b) { return (float)b / 255.0f; }
+__device__ __forceinline__ float4 u8x4_to_unit(uint32_t w) {
+  return make_float4(u8_to_unit(w & 0xffu), u8_to_unit((w >> 8) & 0xffu), u8_to_unit((w >> 16) & 0xffu),
+                     u8_to_unit(w >> 24));
+}
 
 __global__ void u8_to_f32_kernel(const uint8_t* __restrict__ src, float* __restrict__ dst, long long n) {
   const long long n16 = n >> 4;
@@ -19,19 +29,29 @@ __global__ void u8_to_f32_kernel(const uint8_t* __restrict__ src, float* __restr
   float4* d4 = reinterpret_cast<float4*>(dst);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += (long long)gridDim.x * blockDim.x) {
     const uint4 v = s4[i];
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      float4 o;
-      o.x = (float)(w[k] & 0xffu) / 255.0f;                    // true division, like Tensor.div(255)
-      o.y = (float)((w[k] >> 8) & 0xffu) / 255.0f;
-      o.z = (float)((w[k] >> 16) & 0xffu) / 255.0f;
-      o.w = (float)(w[k] >> 24) / 255.0f;
-      d4[4 * i + k] = o;
-    }
+    d4[4 * i + 0] = u8x4_to_unit(v.x);
+    d4[4 * i + 1] = u8x4_to_unit(v.y);
+    d4[4 * i + 2] = u8x4_to_unit(v.z);
+    d4[4 * i + 3] = u8x4_to_unit(v.w);
   }
   for (long long i = (n16 << 4) + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    dst[i] = (float)src[i] / 255.0f;
+    dst[i] = u8_to_unit(src[i]);
+}
+
+// dst row i = src row idx[i] / 255; one thread per 16-byte chunk of a destination row (row_bytes a multiple of 16).
+__global__ void __launch_bounds__(256)
+gather_u8_to_f32_kernel(const uint8_t* __restrict__ src, const long long* __restrict__ idx, int nrows, int chunks,
+                        float* __restrict__ dst) {
+  const long long n = (long long)nrows * chunks;
+  float4* d4 = reinterpret_cast<float4*>(dst);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long row = i / chunks, c = i - row * chunks;
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(src) + idx[row] * chunks + c);
+    d4[4 * i + 0] = u8x4_to_unit(v.x);
+    d4[4 * i + 1] = u8x4_to_unit(v.y);
+    d4[4 * i + 2] = u8x4_to_unit(v.z);
+    d4[4 * i + 3] = u8x4_to_unit(v.w);
+  }
 }
 
 struct Coefs { float a[8]; float b[8]; };
@@ -132,6 +152,17 @@ int dv_u8_to_f32(const unsigned char* src, float* dst, long long n, void* stream
   if (blocks < 1) blocks = 1;
   if (blocks > 8 * kNumSMs) blocks = 8 * kNumSMs;
   u8_to_f32_kernel<<<(int)blocks, 256, 0, as_stream(stream)>>>(src, dst, n);
+  return check_launch();
+}
+
+int dv_gather_u8_to_f32(const unsigned char* src, const long long* idx, int nrows, int row_bytes, float* dst,
+                        void* stream) {
+  if (!src || !idx || !dst) return DV_ERR_BAD_ARG;
+  if (nrows < 1 || row_bytes < 16 || (row_bytes & 15)) return DV_ERR_BAD_SHAPE;
+  if (((uintptr_t)src & 15) || ((uintptr_t)dst & 15) || ((uintptr_t)idx & 7)) return DV_ERR_BAD_ARG;
+  const int chunks = row_bytes >> 4;
+  const long long blocks = std::min<long long>(((long long)nrows * chunks + 255) / 256, 8 * kNumSMs);
+  gather_u8_to_f32_kernel<<<(int)blocks, 256, 0, as_stream(stream)>>>(src, idx, nrows, chunks, dst);
   return check_launch();
 }
 

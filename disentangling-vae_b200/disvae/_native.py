@@ -57,6 +57,7 @@ SIGNATURES = {
     "dv_btcvae_fwd_rows": (I, [P, P, P, I, I, I, I, I, I, LL, I, P, P, P, P]),
     "dv_btcvae_bwd_rows": (I, [I, I, I, I, LL, I, P, P, P, P, P, P, P]),
     "dv_u8_to_f32": (I, [P, P, LL, P]),
+    "dv_gather_u8_to_f32": (I, [P, P, I, I, P, P]),
     "dv_loss_combine_fwd": (I, [P, P, I, P, P, I, P, P]),
     "dv_loss_combine_bwd": (I, [P, P, I, I, P, I, P, P, P]),
     "dv_act_bwd_chansum": (I, [P, P, P, I, I, I, I, F, P, P, P]),
@@ -65,6 +66,8 @@ SIGNATURES = {
     "dv_permute_dims": (I, [P, P, ULL, P, P, I, I, P]),
     "dv_permute_dims_workspace_bytes": (SZ, [I, I]),
     "dv_permute_dims_rows": (I, [P, P, ULL, P, P, I, I, I, I, P, P]),
+    "dv_index_permutation_workspace_bytes": (SZ, [I]),
+    "dv_index_permutation": (I, [I, ULL, P, P, P, P]),
     "dv_factor_tc_fwd": (I, [P, I, P, P]),
     "dv_factor_tc_bwd": (I, [P, I, P, P]),
     "dv_factor_ce_fwd": (I, [P, P, I, P, P]),

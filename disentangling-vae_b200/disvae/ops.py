@@ -157,6 +157,33 @@ def u8_to_f32(src, out=None):
     return out
 
 
+def gather_u8_to_f32(src, idx, out=None):
+    """Rows src[idx] of a CUDA uint8 tensor [N, ...] as float32 / 255 (ToTensor on the device) in one launch;
+    idx = CUDA int64 indices in [0, N), repeats allowed; `out` = preallocated float32 [len(idx), ...]."""
+    if not src.is_cuda or src.dtype != torch.uint8:
+        raise RuntimeError("disvae_b200.gather_u8_to_f32 expects a CUDA uint8 tensor, got %s on %s" % (src.dtype, src.device))
+    if not idx.is_cuda or idx.dtype != torch.int64 or idx.dim() != 1:
+        raise RuntimeError("disvae_b200.gather_u8_to_f32 expects 1-d CUDA int64 indices, got %s %s on %s"
+                           % (idx.dtype, tuple(idx.shape), idx.device))
+    src, idx = _c(src), _c(idx)
+    if out is None:
+        out = torch.empty((idx.numel(),) + tuple(src.shape[1:]), dtype=torch.float32, device=src.device)
+    call("dv_gather_u8_to_f32", src.data_ptr(), idx.data_ptr(), idx.numel(), src[0].numel(), ptr(out), stream())
+    return out
+
+
+def index_permutation(n, seed, offset_dev, out=None):
+    """Philox-keyed permutation of [0, n) as CUDA int64 (the order dv_permute_dims_rows draws for one dimension);
+    reads the counter offset from the device tensor `offset_dev` and advances it by n."""
+    device = offset_dev.device
+    if out is None:
+        out = torch.empty(n, dtype=torch.int64, device=device)
+    nbytes = N.lib().dv_index_permutation_workspace_bytes(n)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=device) if nbytes else None
+    call("dv_index_permutation", n, seed, ptr(offset_dev), ptr(out), ptr(ws), stream())
+    return out
+
+
 def act_bwd(dy, y, act, slope=0.0):
     g = torch.empty_like(y)
     call("dv_act_bwd", ptr(dy), ptr(y), ptr(g), y.numel(), act, slope, stream())

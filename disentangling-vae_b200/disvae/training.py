@@ -43,6 +43,10 @@ class Trainer():
         self._grad_sync_d = None
         self._fused = None                        # FusedAdam over `optimizer` (built lazily on the device)
         self.use_cuda_graph = os.environ.get("DISVAE_CUDA_GRAPH", "1") != "0"
+        # DISVAE_DEVICE_DATA=1: a torch DataLoader passed to __call__ is replaced by a disvae.data.DeviceLoader over its
+        # dataset (decoded once, kept on the GPU; its own shuffle stream, hence opt-in)
+        self.device_data = os.environ.get("DISVAE_DEVICE_DATA", "0") == "1"
+        self._device_loaders = {}                 # id(DataLoader) -> (DataLoader, its DeviceLoader)
         self._graphs = {}                         # input shape -> (CUDAGraph, static input, static loss)
         self._eligible_steps = 0
         self.logger.info("Training Device: {}".format(self.device))
@@ -50,6 +54,8 @@ class Trainer():
     def __call__(self, data_loader, epochs=10, checkpoint_every=10):
         """training.py:64-102"""
         start = default_timer()
+        if self.device_data and isinstance(data_loader, torch.utils.data.DataLoader):
+            data_loader = self._device_loader(data_loader)
         self.model.train()
         for epoch in range(epochs):
             storer = defaultdict(list)
@@ -87,6 +93,14 @@ class Trainer():
         if self._fused:
             self._fused.flush_state()                         # optimizer.state[p]["step"] follows the device counter
         return epoch_loss.item() / len(data_loader)
+
+    def _device_loader(self, loader):
+        """The DeviceLoader standing in for `loader`, built (the dataset decoded and uploaded) once per loader."""
+        entry = self._device_loaders.get(id(loader))
+        if entry is None:
+            from disvae.data import device_loader_for
+            entry = self._device_loaders[id(loader)] = (loader, device_loader_for(loader, self.device))
+        return entry[1]
 
     def _loss_ring(self):
         if getattr(self, "_ring", None) is None:

@@ -220,6 +220,15 @@ int dv_btcvae_bwd_rows(int B, int D, int row0, int nrows, long long n_data, int 
  * uploaded as bytes (training.py:150; utils/datasets.py:182,247,364-367).  Both pointers 16-byte aligned.
  */
 int dv_u8_to_f32(const unsigned char* src, float* dst, long long n, void* stream);
+/* Device-resident dataset (disvae.data.DeviceLoader): replaces the per-item ToTensor of the reference's datasets
+ * (utils/datasets.py:182,206-210) and the collate of its DataLoader for one batch.  src is the dataset as uint8
+ * [N, row_bytes] on the device; dst row i = src row idx[i] / 255 (true division, bit-identical to dv_u8_to_f32 and to
+ * ToTensor), dst is fp32 [nrows, row_bytes].  idx: int64 device array of nrows entries in [0, N) (not checked: the
+ * kernel does not know N), repeats allowed.  One launch, 16-byte loads.
+ * DV_ERR_BAD_SHAPE: nrows < 1 or row_bytes not a positive multiple of 16 (every Burgess geometry is: 1024, 3072,
+ * 4096 or 12288 bytes).  DV_ERR_BAD_ARG: a NULL pointer, src or dst not 16-byte aligned, idx not 8-byte aligned. */
+int dv_gather_u8_to_f32(const unsigned char* src, const long long* idx, int nrows, int row_bytes, float* dst,
+                        void* stream);
 /* loss[0] = sum_{i<na} coef_a[i]*a[i] + sum_{j<nb} coef_b[j]*b[j]; a, b device vectors, coef_* HOST arrays (<= 8 each,
  * passed to the kernel by value).  The scalar combinations of losses.py:151 (rec + anneal*beta*kl), :199-200 is not
  * covered (|kl - C|), :381-382 (rec + alpha*mi + beta*tc + anneal*gamma*dw_kl).  Backward: g_a[0..na_total) (zeros past
@@ -264,6 +273,16 @@ int dv_permute_dims(const float* z, const long long* perms, unsigned long long s
 size_t dv_permute_dims_workspace_bytes(int B, int D);   /* 0 when B <= 4096 */
 int dv_permute_dims_rows(const float* z, const long long* perms, unsigned long long seed,
                          unsigned long long* offset_dev, float* out, int B, int D, int row0, int nrows,
+                         void* workspace, void* stream);
+/* Epoch order of a device-resident dataset: replaces the RandomSampler of the reference's DataLoader
+ * (utils/datasets.py:67-71, `shuffle=True`).  out_idx (int64 [N], 8-byte aligned) receives the Philox-keyed permutation
+ * of [0, N) that dv_permute_dims_rows draws for one dimension (D = 1): the order that sorts the keys
+ * (philox4x32_10(*offset_dev + i, seed).x << 32) | i ascending.  *offset_dev advances by N.  N up to INT_MAX.
+ * workspace: dv_index_permutation_workspace_bytes(N) bytes, 8-byte aligned, contents irrelevant (NULL allowed when
+ * that is 0, N <= 4096).  Deterministic, host-synchronisation free, graph-capturable.
+ * DV_ERR_BAD_SHAPE: N < 1.  DV_ERR_BAD_ARG: a NULL or misaligned pointer. */
+size_t dv_index_permutation_workspace_bytes(int N);
+int dv_index_permutation(int N, unsigned long long seed, unsigned long long* offset_dev, long long* out_idx,
                          void* workspace, void* stream);
 /* tc[0] = mean(d_z[:,0] - d_z[:,1])  (losses.py:265) */
 int dv_factor_tc_fwd(const float* d_z, int h, float* tc, void* stream);

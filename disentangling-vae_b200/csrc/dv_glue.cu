@@ -9,6 +9,9 @@
 //                         (rec, kl, ...) and the beta-TCVAE (mi, tc, dw_kl)): losses.py:151, 199-200, 381-382 as ONE
 //                         launch forward and ONE backward instead of ~10 scalar mul/add/select kernels and their
 //                         zero-filled gradient buffers
+//   dv_loss_combine_sched_*  the same with the annealing coefficient computed on the device from the loss's step counter
+//   dv_betab_loss_*       beta-VAE_B's rec + gamma*|kl - C(step)| (losses.py:199-200) with its autograd gradient
+//   dv_loss_record        the device loss log: a recording step's scalars into a ring row (also done by the two above)
 //   dv_act_bwd_chansum    ConvTranspose2d output layer backward prologue: g = dy * act'(y) (decoders.py:82 sigmoid) fused
 //                         with the per-channel sum of g (that layer's bias gradient) -- one pass instead of two
 #include <algorithm>
@@ -56,14 +59,128 @@ gather_u8_to_f32_kernel(const uint8_t* __restrict__ src, const long long* __rest
 
 struct Coefs { float a[8]; float b[8]; };
 
+// The arithmetic both combine kernels share, spelled out (an fma chain per vector, then one add) so that the host-
+// coefficient and the scheduled kernel round identically.
+__device__ __forceinline__ float combine_value(const float* a, int na, const float* b, int nb, const Coefs& c) {
+  float s = 0.f;
+  for (int i = 0; i < na; ++i) s = __fmaf_rn(c.a[i], a[i], s);  // fixed order: rec first, like rec + (...) in the reference
+  float t = 0.f;
+  for (int j = 0; j < nb; ++j) t = __fmaf_rn(c.b[j], b[j], t);
+  return __fadd_rn(s, t);
+}
+
 __global__ void loss_combine_fwd_kernel(const float* __restrict__ a, int na, const float* __restrict__ b, int nb, Coefs c,
                                         float* __restrict__ loss) {
   if (threadIdx.x != 0) return;
-  float s = 0.f;
-  for (int i = 0; i < na; ++i) s += c.a[i] * a[i];             // fixed order: rec first, like rec + (...) in the reference
-  float t = 0.f;
-  for (int j = 0; j < nb; ++j) t += c.b[j] * b[j];
-  loss[0] = s + t;
+  loss[0] = combine_value(a, na, b, nb, c);
+}
+
+// ---- annealed coefficients from a device step counter (dv_loss_combine_sched_*, dv_betab_loss_*, dv_loss_record) ----
+// linear_annealing(init, fin, step, steps_anneal) of losses.py in double, in Python's operation order:
+// min(init + (fin - init) * step / steps_anneal, fin), or fin outside training and when steps_anneal == 0.
+__device__ __forceinline__ double anneal_value(double init, double fin, long long step, long long steps_anneal,
+                                               int is_train) {
+  if (!is_train || steps_anneal == 0) return fin;
+  const double x = __dadd_rn(init, __ddiv_rn(__dmul_rn(__dsub_rn(fin, init), (double)step), (double)steps_anneal));
+  return fin < x ? fin : x;                                     // Python's min(x, fin) keeps x unless fin < x
+}
+
+// Thread 0: the step this launch computes for -- on a training step the counter is advanced first.
+__device__ __forceinline__ long long take_step(long long* step, int is_train) {
+  if (!is_train) return 0;
+  const long long s = *step + 1;
+  *step = s;
+  return s;
+}
+
+// Whole block: when `step` records (step % every == 1, losses.py's rule), concatenate the sources into ring row
+// ((step - 1) / every) % cap.  A NULL source (length 1) is `self_value`, the scalar the calling kernel just computed.
+__device__ void log_record(const dv_loss_log& L, long long step, float self_value) {
+  if (step % L.every != 1) return;
+  float* row = L.ring + ((step - 1) / L.every % L.cap) * (long long)L.ncols;
+  int off = 0;
+  for (int k = 0; k < L.nsrc; ++k) {
+    const float* src = L.src[k];
+    for (int i = threadIdx.x; i < L.len[k]; i += blockDim.x) row[off + i] = src ? src[i] : self_value;
+    off += L.len[k];
+  }
+}
+
+struct Sched {
+  double base[16];              // coefficient k: base[k], times the annealing value when bit k of `mask` is set
+  unsigned mask;
+  double init, fin;
+  long long steps_anneal;
+  int is_train;
+};
+
+__global__ void loss_combine_sched_fwd_kernel(const float* __restrict__ a, int na, const float* __restrict__ b, int nb,
+                                              Sched sc, long long* __restrict__ step, float* __restrict__ loss,
+                                              float* __restrict__ coefs, dv_loss_log log) {
+  long long s = 0;
+  float value = 0.f;
+  if (threadIdx.x == 0) {
+    s = take_step(step, sc.is_train);
+    const double v = anneal_value(sc.init, sc.fin, s, sc.steps_anneal, sc.is_train);
+    Coefs c = {};
+    for (int k = 0; k < na + nb; ++k) {
+      // (float)(anneal * base): what ctypes made of the Python product anneal_reg * coefficient
+      const float ck = __double2float_rn((sc.mask >> k) & 1u ? __dmul_rn(v, sc.base[k]) : sc.base[k]);
+      if (k < na) c.a[k] = ck; else c.b[k - na] = ck;
+      coefs[k] = ck;
+    }
+    value = combine_value(a, na, b, nb, c);
+    loss[0] = value;
+  }
+  if (!log.ring || !sc.is_train) return;
+  s = __shfl_sync(0xffffffffu, s, 0);
+  value = __shfl_sync(0xffffffffu, value, 0);
+  log_record(log, s, value);
+}
+
+__global__ void loss_combine_sched_bwd_kernel(const float* __restrict__ g, const float* __restrict__ coefs, int na,
+                                              int na_total, int nb, float* __restrict__ g_a, float* __restrict__ g_b) {
+  const float gv = g[0];
+  for (int i = threadIdx.x; i < na_total; i += blockDim.x) g_a[i] = i < na ? gv * coefs[i] : 0.f;
+  if (g_b)
+    for (int j = threadIdx.x; j < nb; j += blockDim.x) g_b[j] = gv * coefs[na + j];
+}
+
+struct BetaB { double gamma, c_init, c_fin; long long steps_anneal; int is_train; };
+
+// rec + gamma * |kl - C| with torch's rounding: kl - C and gamma * |.| in float, then the add (losses.py:199-200)
+__global__ void betab_loss_fwd_kernel(const float* __restrict__ rec_kl, BetaB p, long long* __restrict__ step,
+                                      float* __restrict__ loss, float* __restrict__ consts, dv_loss_log log) {
+  long long s = 0;
+  float value = 0.f;
+  if (threadIdx.x == 0) {
+    s = take_step(step, p.is_train);
+    const float C = __double2float_rn(anneal_value(p.c_init, p.c_fin, s, p.steps_anneal, p.is_train));
+    const float gm = __double2float_rn(p.gamma);
+    value = __fadd_rn(rec_kl[0], __fmul_rn(gm, fabsf(__fsub_rn(rec_kl[1], C))));
+    loss[0] = value;
+    consts[0] = C;
+    consts[1] = gm;
+  }
+  if (!log.ring || !p.is_train) return;
+  s = __shfl_sync(0xffffffffu, s, 0);
+  value = __shfl_sync(0xffffffffu, value, 0);
+  log_record(log, s, value);
+}
+
+// The gradient autograd gives the same expression: d rec = g, d kl = (g * gamma) * sgn(kl - C) with sgn(0) = 0, each
+// landing in a zero-filled [n] buffer (hence the + 0: -0 becomes +0 as it does there); zeros past the two.
+__global__ void betab_loss_bwd_kernel(const float* __restrict__ g, const float* __restrict__ rec_kl,
+                                      const float* __restrict__ consts, int n, float* __restrict__ g_out) {
+  const float gv = g[0];
+  const float d = __fsub_rn(rec_kl[1], consts[0]);
+  const float sg = (float)((d > 0.f) - (d < 0.f));
+  for (int i = threadIdx.x; i < n; i += blockDim.x)
+    g_out[i] = i == 0 ? __fadd_rn(0.f, gv) : i == 1 ? __fadd_rn(0.f, __fmul_rn(__fmul_rn(gv, consts[1]), sg)) : 0.f;
+}
+
+__global__ void loss_record_kernel(const long long* __restrict__ step, dv_loss_log log) {
+  log_record(log, *step, 0.f);
 }
 
 // g_a has na_total entries (the producing node's full output, e.g. 2 + latent_dim): zeros beyond the na weighted ones
@@ -183,6 +300,78 @@ int dv_loss_combine_bwd(const float* g, const float* coef_a, int na, int na_tota
   for (int i = 0; i < na; ++i) c.a[i] = coef_a[i];
   for (int j = 0; j < nb; ++j) c.b[j] = coef_b[j];
   loss_combine_bwd_kernel<<<1, 128, 0, as_stream(stream)>>>(g, na, na_total, nb, c, g_a, g_b);
+  return check_launch();
+}
+
+}  // extern "C"
+
+// A caller's log description -> the kernel argument (ring == NULL: no record).  self_ok: a NULL source of length 1 may
+// stand for the launch's own result.
+static int log_arg(const dv_loss_log* log, bool self_ok, dv_loss_log* out) {
+  *out = dv_loss_log{};
+  if (!log) return DV_OK;
+  if (!log->ring || log->cap < 1 || log->every < 1 || log->nsrc < 1 || log->nsrc > DV_LOSS_LOG_MAX_SRC) return DV_ERR_BAD_ARG;
+  int total = 0;
+  for (int k = 0; k < log->nsrc; ++k) {
+    if (log->len[k] < 0 || (!log->src[k] && !(self_ok && log->len[k] == 1))) return DV_ERR_BAD_ARG;
+    total += log->len[k];
+  }
+  if (total != log->ncols) return DV_ERR_BAD_SHAPE;
+  *out = *log;
+  return DV_OK;
+}
+
+extern "C" {
+
+int dv_loss_combine_sched_fwd(const float* a, int na, const float* b, int nb, const double* base, unsigned sched_mask,
+                              double init, double fin, long long steps_anneal, int is_train, long long* step, float* loss,
+                              float* coefs, const dv_loss_log* log, void* stream) {
+  if (!a || !base || !loss || !coefs || na < 1 || na > 8 || nb < 0 || nb > 8 || (nb > 0 && !b)) return DV_ERR_BAD_ARG;
+  if (steps_anneal < 0 || (is_train && !step) || (sched_mask >> (na + nb)) != 0) return DV_ERR_BAD_ARG;
+  Sched sc = {};
+  for (int k = 0; k < na + nb; ++k) sc.base[k] = base[k];       // HOST array: travels by value
+  sc.mask = sched_mask;
+  sc.init = init;
+  sc.fin = fin;
+  sc.steps_anneal = steps_anneal;
+  sc.is_train = is_train ? 1 : 0;
+  dv_loss_log L;
+  const int rc = log_arg(is_train ? log : nullptr, true, &L);
+  if (rc != DV_OK) return rc;
+  loss_combine_sched_fwd_kernel<<<1, 32, 0, as_stream(stream)>>>(a, na, b, nb, sc, step, loss, coefs, L);
+  return check_launch();
+}
+
+int dv_loss_combine_sched_bwd(const float* g, const float* coefs, int na, int na_total, int nb, float* g_a, float* g_b,
+                              void* stream) {
+  if (!g || !coefs || !g_a || na < 1 || na > 8 || na_total < na || nb < 0 || nb > 8) return DV_ERR_BAD_ARG;
+  loss_combine_sched_bwd_kernel<<<1, 128, 0, as_stream(stream)>>>(g, coefs, na, na_total, nb, g_a, nb > 0 ? g_b : nullptr);
+  return check_launch();
+}
+
+int dv_betab_loss_fwd(const float* rec_kl, double gamma, double c_init, double c_fin, long long steps_anneal, int is_train,
+                      long long* step, float* loss, float* consts, const dv_loss_log* log, void* stream) {
+  if (!rec_kl || !loss || !consts || steps_anneal < 0 || (is_train && !step)) return DV_ERR_BAD_ARG;
+  const BetaB p = {gamma, c_init, c_fin, steps_anneal, is_train ? 1 : 0};
+  dv_loss_log L;
+  const int rc = log_arg(is_train ? log : nullptr, true, &L);
+  if (rc != DV_OK) return rc;
+  betab_loss_fwd_kernel<<<1, 32, 0, as_stream(stream)>>>(rec_kl, p, step, loss, consts, L);
+  return check_launch();
+}
+
+int dv_betab_loss_bwd(const float* g, const float* rec_kl, const float* consts, int n, float* g_rec_kl, void* stream) {
+  if (!g || !rec_kl || !consts || !g_rec_kl || n < 2) return DV_ERR_BAD_ARG;
+  betab_loss_bwd_kernel<<<1, 128, 0, as_stream(stream)>>>(g, rec_kl, consts, n, g_rec_kl);
+  return check_launch();
+}
+
+int dv_loss_record(const long long* step, const dv_loss_log* log, void* stream) {
+  if (!step || !log) return DV_ERR_BAD_ARG;
+  dv_loss_log L;
+  const int rc = log_arg(log, false, &L);
+  if (rc != DV_OK) return rc;
+  loss_record_kernel<<<1, 32, 0, as_stream(stream)>>>(step, L);
   return check_launch();
 }
 

@@ -60,6 +60,11 @@ SIGNATURES = {
     "dv_gather_u8_to_f32": (I, [P, P, I, I, P, P]),
     "dv_loss_combine_fwd": (I, [P, P, I, P, P, I, P, P]),
     "dv_loss_combine_bwd": (I, [P, P, I, I, P, I, P, P, P]),
+    "dv_loss_combine_sched_fwd": (I, [P, I, P, I, P, I, DBL, DBL, LL, I, P, P, P, P, P]),
+    "dv_loss_combine_sched_bwd": (I, [P, P, I, I, I, P, P, P]),
+    "dv_betab_loss_fwd": (I, [P, DBL, DBL, DBL, LL, I, P, P, P, P, P]),
+    "dv_betab_loss_bwd": (I, [P, P, P, I, P, P]),
+    "dv_loss_record": (I, [P, P, P]),
     "dv_act_bwd_chansum": (I, [P, P, P, I, I, I, I, F, P, P, P]),
     "dv_latent_entropy_workspace_bytes": (SZ, [I, I, I]),
     "dv_latent_entropy": (I, [P, P, P, I, I, I, I, I, P, P, P, P]),
@@ -76,6 +81,15 @@ SIGNATURES = {
     "dv_adam_multi_max_tensors": (I, []),
     "dv_adam_multi": (I, [I, P, P, P, P, P, P, F, DBL, DBL, F, F, P]),
 }
+
+LOSS_LOG_MAX_SRC = 8
+
+
+class LossLog(ctypes.Structure):
+    """dv_loss_log: where a recording step's scalars go (device ring [cap][ncols]) and where they come from."""
+    _fields_ = [("ring", c_void_p), ("cap", c_int), ("ncols", c_int), ("every", c_int), ("nsrc", c_int),
+                ("src", c_void_p * LOSS_LOG_MAX_SRC), ("len", c_int * LOSS_LOG_MAX_SRC)]
+
 
 _lib = None
 GRAPH_LAUNCHES = 0       # kernels launched through CUDA-graph replays (dv_launch_count() only sees direct launches)

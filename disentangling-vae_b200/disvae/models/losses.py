@@ -73,14 +73,102 @@ def _kl_names(latent_dim):
     return ['kl_loss_' + str(i) for i in range(latent_dim)]
 
 
+def _flat_names(names, lens):
+    """The storer keys `_record` appends to, in its order, for values of `lens` entries each."""
+    flat = []
+    for name, n in zip(names, lens):
+        flat += [name] if isinstance(name, str) else list(name)[:n]
+    return flat
+
+
+class DeviceLossLog:
+    """The scalars of recording training steps kept on the device until the host asks for them.
+
+    A recording step's kernels write its values into one row of a device ring (ops: the `log` of the loss kernels,
+    dv_loss_record), so the step has no host synchronisation and can be replayed from a CUDA graph.  The host side knows
+    which steps record (`expect`: the reference's rule on n_train_steps) and for which storer; `flush` copies the ring
+    back once and appends every pending row to its storer with exactly the keys, order and values `_record` appends.
+    The ring is flushed before a new row could overwrite a pending one (every `capacity` recording steps at most)."""
+
+    def __init__(self, device, capacity=256):
+        self.device, self.capacity = device, capacity
+        self.ring = self.host = None
+        self.names = None               # keys of one row, in `_record`'s order
+        self.pending = []               # (row, storer) in step order
+
+    def spec(self, every, names, values):
+        """The _native.LossLog of one step: `values` as `_record` takes them, None for the loss the launch computes."""
+        from disvae import _native
+        lens = [1 if v is None else v.numel() for v in values]
+        self.layout(_flat_names(names, lens))
+        flat = self.names
+        if len(values) > _native.LOSS_LOG_MAX_SRC:
+            raise ValueError("at most %d logged values per step" % _native.LOSS_LOG_MAX_SRC)
+        log = _native.LossLog()
+        log.ring, log.cap, log.ncols, log.every, log.nsrc = self.ring.data_ptr(), self.capacity, len(flat), every, len(values)
+        for k, (v, n) in enumerate(zip(values, lens)):
+            if v is not None:
+                _native.require_cuda_f32(v)
+                if not v.is_contiguous():
+                    raise ValueError("logged values must be contiguous")
+            log.src[k] = None if v is None else v.data_ptr()
+            log.len[k] = n
+        return log
+
+    def layout(self, names):
+        """Keys of one row (the ring is allocated with the first layout; one log serves one loss)."""
+        if self.ring is None:
+            self.ring = torch.zeros(self.capacity, len(names), dtype=torch.float32, device=self.device)
+            self.host = torch.zeros(self.capacity, len(names), dtype=torch.float32)
+            if self.ring.is_cuda:
+                self.host = self.host.pin_memory()
+        if self.names is not None and names != self.names:
+            raise ValueError("one DeviceLossLog serves one loss: got keys %s after %s" % (names, self.names))
+        self.names = names
+
+    def expect(self, step, every, storer):
+        """Training step `step` is about to run with `storer`: note its row if it records.  The device writes the row of
+        every recording step, storer or not, so a row still pending is read back before it can be overwritten."""
+        if step % every != 1:
+            return
+        row = (step - 1) // every % self.capacity
+        if any(r == row for r, _ in self.pending):
+            self.flush()
+        if storer is not None:
+            self.pending.append((row, storer))
+
+    def flush(self):
+        """One copy of the ring to the host (after everything enqueued so far), then the pending rows into their storers."""
+        if not self.pending:
+            return
+        self.host.copy_(self.ring, non_blocking=True)
+        if self.ring.is_cuda:
+            done = torch.cuda.Event()
+            done.record()
+            done.synchronize()
+        rows = self.host.tolist()
+        for row, storer in self.pending:
+            for name, v in zip(self.names, rows[row]):
+                storer[name].append(v)
+        self.pending.clear()
+
+
 class BaseLoss(abc.ABC):
-    """losses.py:52-114: step counter, record-every-50 policy, common options."""
+    """losses.py:52-114: step counter, record-every-50 policy, common options.
+
+    Besides the host counter `n_train_steps` each loss owns an int64 device copy of it, advanced by the loss kernel of
+    every training step (ops.LossCombineSchedFn / BetaBLossFn), from which the annealing coefficients and the device
+    loss log are computed: a step replayed from a CUDA graph anneals and records like an eager one.  `_log` is the
+    DeviceLossLog of the Trainer step in progress (None otherwise: scalars go to the storer through `_record`)."""
 
     def __init__(self, record_loss_every=50, rec_dist="bernoulli", steps_anneal=0):
         self.n_train_steps = 0
         self.record_loss_every = record_loss_every
         self.rec_dist = rec_dist
         self.steps_anneal = steps_anneal
+        self._step_dev = None           # the device counter (created on the first training call)
+        self._step_dev_host = 0         # its value once the work enqueued so far has run
+        self._log = None
 
     @abc.abstractmethod
     def __call__(self, data, recon_data, latent_dist, is_train, storer, **kwargs):
@@ -89,9 +177,38 @@ class BaseLoss(abc.ABC):
     def _pre_call(self, is_train, storer):
         if is_train:
             self.n_train_steps += 1
+            if self._log is not None:                       # recorded on the device, handed to `storer` by the flush
+                self._log.expect(self.n_train_steps, self.record_loss_every, storer)
+                return None
         if not is_train or self.n_train_steps % self.record_loss_every == 1:
             return storer
         return None
+
+    def _step_counter(self, device, advancing):
+        """The device step counter, holding what the host counter held before this step: n_train_steps - 1 when the
+        launch about to be enqueued advances it (`advancing`, after _pre_call), n_train_steps otherwise.  Re-written
+        only when the two have drifted apart (n_train_steps set by hand), so never inside a captured step."""
+        want = self.n_train_steps - 1 if advancing else self.n_train_steps
+        if self._step_dev is None or self._step_dev.device != device:
+            self._step_dev = torch.full((1,), want, dtype=torch.int64, device=device)
+        elif self._step_dev_host != want:
+            self._step_dev.fill_(want)
+        self._step_dev_host = self.n_train_steps
+        return self._step_dev
+
+    def _log_spec(self, is_train, names, values):
+        """The device loss log of this call (None: none -- outside a Trainer step, or not training)."""
+        if not is_train or self._log is None:
+            return None
+        return self._log.spec(self.record_loss_every, names, values)
+
+    def _combine(self, out, b, coef_a, coef_b, annealed, is_train, log):
+        """ops.LossCombineSchedFn: coefficient number `annealed` (coef_a, then coef_b) is multiplied by
+        linear_annealing(0, 1, step, steps_anneal) on the device."""
+        step = self._step_counter(out.device, True) if is_train else None
+        loss, _ = ops.LossCombineSchedFn.apply(out, b, coef_a, coef_b, 1 << annealed, (0, 1, self.steps_anneal),
+                                               is_train, step, log)
+        return loss
 
     def _rec_kl(self, data, recon_data, latent_dist):
         """(recon_loss, kl_total, per-dim kl vector) from the fused kernel."""
@@ -114,10 +231,10 @@ class BetaHLoss(BaseLoss):
         storer = self._pre_call(is_train, storer)
         out = self._rec_kl_vec(data, recon_data, latent_dist)
         rec_loss, kl_loss, kl_dims = out[0], out[1], out[2:]
-        anneal_reg = linear_annealing(0, 1, self.n_train_steps, self.steps_anneal) if is_train else 1
-        loss = ops.LossCombineFn.apply(out, None, [1.0, anneal_reg * self.beta], None)     # rec + anneal * (beta * kl)
-        _record(storer, ['recon_loss', 'kl_loss', _kl_names(kl_dims.numel()), 'loss'],
-                [rec_loss, kl_loss, kl_dims, loss])
+        names = ['recon_loss', 'kl_loss', _kl_names(kl_dims.numel()), 'loss']
+        log = self._log_spec(is_train, names, [rec_loss, kl_loss, kl_dims, None])
+        loss = self._combine(out, None, [1.0, self.beta], None, 1, is_train, log)     # rec + anneal * (beta * kl)
+        _record(storer, names, [rec_loss, kl_loss, kl_dims, loss])
         return loss
 
 
@@ -132,12 +249,15 @@ class BetaBLoss(BaseLoss):
 
     def __call__(self, data, recon_data, latent_dist, is_train, storer, **kwargs):
         storer = self._pre_call(is_train, storer)
-        rec_loss, kl_loss, kl_dims = self._rec_kl(data, recon_data, latent_dist)
-        C = (linear_annealing(self.C_init, self.C_fin, self.n_train_steps, self.steps_anneal)
-             if is_train else self.C_fin)
-        loss = rec_loss + self.gamma * (kl_loss - C).abs()
-        _record(storer, ['recon_loss', 'kl_loss', _kl_names(kl_dims.numel()), 'loss'],
-                [rec_loss, kl_loss, kl_dims, loss])
+        out = self._rec_kl_vec(data, recon_data, latent_dist)
+        rec_loss, kl_loss, kl_dims = out[0], out[1], out[2:]
+        names = ['recon_loss', 'kl_loss', _kl_names(kl_dims.numel()), 'loss']
+        log = self._log_spec(is_train, names, [rec_loss, kl_loss, kl_dims, None])
+        assert not (is_train and self.steps_anneal) or self.C_fin > self.C_init     # linear_annealing's own check
+        step = self._step_counter(out.device, True) if is_train else None
+        # rec + gamma * |kl - C| with C = linear_annealing(C_init, C_fin, step, steps_anneal) (C_fin outside training)
+        loss, _ = ops.BetaBLossFn.apply(out, self.gamma, (self.C_init, self.C_fin, self.steps_anneal), is_train, step, log)
+        _record(storer, names, [rec_loss, kl_loss, kl_dims, loss])
         return loss
 
 
@@ -217,12 +337,11 @@ class FactorKLoss(BaseLoss):
         recon_batch, latent_dist, latent_sample1 = model(data1, eps=eps1)
         out = self._rec_kl_vec(data1, recon_batch, latent_dist)
         rec_loss, kl_loss, kl_dims = out[0], out[1], out[2:]
-        anneal_reg = linear_annealing(0, 1, self.n_train_steps, self.steps_anneal) if model.training else 1
 
         if not model.training:
             d_z = self.discriminator(latent_sample1)
             tc_loss = ops.FactorTcFn.apply(d_z)
-            vae_loss = ops.LossCombineFn.apply(out, tc_loss, [1.0, 1.0], [anneal_reg * self.gamma])
+            vae_loss = self._combine(out, tc_loss, [1.0, 1.0], [self.gamma], 2, False, None)
             _record(storer, ['recon_loss', 'kl_loss', _kl_names(kl_dims.numel()), 'loss', 'tc_loss'],
                     [rec_loss, kl_loss, kl_dims, vae_loss, tc_loss])
             return vae_loss
@@ -249,7 +368,7 @@ class FactorKLoss(BaseLoss):
             d_all = self.discriminator(torch.cat([latent_sample1, z_perm]))
         d_z, d_z_perm = d_all[:half], d_all[half:]
         tc_loss = ops.FactorTcFn.apply(d_z)                      # mean(d_z[:,0] - d_z[:,1])
-        vae_loss = ops.LossCombineFn.apply(out, tc_loss, [1.0, 1.0], [anneal_reg * self.gamma])   # rec + kl + anneal*gamma*tc
+        vae_loss = self._combine(out, tc_loss, [1.0, 1.0], [self.gamma], 2, True, None)   # rec + kl + anneal*gamma*tc
 
         optimizer.zero_grad()
         with ops.mlp_input_grad_only():                          # the discriminator's own gradients of this pass are zeroed below
@@ -263,8 +382,12 @@ class FactorKLoss(BaseLoss):
             optimizer.step()
             self._step_d()
 
-        _record(storer, ['recon_loss', 'kl_loss', _kl_names(kl_dims.numel()), 'loss', 'tc_loss', 'discrim_loss'],
-                [rec_loss, kl_loss, kl_dims, vae_loss, tc_loss, d_tc_loss])
+        names = ['recon_loss', 'kl_loss', _kl_names(kl_dims.numel()), 'loss', 'tc_loss', 'discrim_loss']
+        values = [rec_loss, kl_loss, kl_dims, vae_loss, tc_loss, d_tc_loss]
+        log = self._log_spec(True, names, values)
+        if log is not None:                                      # the discriminator loss exists only now: own launch
+            ops.loss_record(self._step_dev, log)
+        _record(storer, names, values)
         return vae_loss
 
 
@@ -296,11 +419,11 @@ class BtcvaeLoss(BaseLoss):
         else:
             terms = ops.btcvae_terms(latent_sample, latent_dist[0], latent_dist[1], self.n_data, self.is_mss)
         mi_loss, tc_loss, dw_kl_loss = terms[0], terms[1], terms[2]
-        anneal_reg = linear_annealing(0, 1, self.n_train_steps, self.steps_anneal) if is_train else 1
+        names = ['recon_loss', 'loss', 'mi_loss', 'tc_loss', 'dw_kl_loss', 'kl_loss', _kl_names(kl_dims.numel())]
+        log = self._log_spec(is_train, names, [rec_loss, None, mi_loss, tc_loss, dw_kl_loss, kl_loss, kl_dims])
         # rec + (alpha*mi + beta*tc + anneal*gamma*dw_kl) as one launch (the kl entries of `out` only feed the log)
-        loss = ops.LossCombineFn.apply(out, terms, [1.0], [self.alpha, self.beta, anneal_reg * self.gamma])
-        _record(storer, ['recon_loss', 'loss', 'mi_loss', 'tc_loss', 'dw_kl_loss', 'kl_loss', _kl_names(kl_dims.numel())],
-                [rec_loss, loss, mi_loss, tc_loss, dw_kl_loss, kl_loss, kl_dims])
+        loss = self._combine(out, terms, [1.0], [self.alpha, self.beta, self.gamma], 3, is_train, log)
+        _record(storer, names, [rec_loss, loss, mi_loss, tc_loss, dw_kl_loss, kl_loss, kl_dims])
         return loss
 
 

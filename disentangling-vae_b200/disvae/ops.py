@@ -764,6 +764,79 @@ class LossCombineFn(Function):
         return g_a, g_b, None, None
 
 
+def _log_arg(log):
+    import ctypes
+    return ctypes.byref(log) if log is not None else None
+
+
+class LossCombineSchedFn(Function):
+    """LossCombineFn whose coefficients are formed on the device, so that a captured CUDA graph anneals: coefficient k is
+    float(base[k] * linear_annealing(init, fin, step, steps_anneal)) when bit k of `sched_mask` is set (k counts coef_a,
+    then coef_b), float(base[k]) otherwise.  On a training step the kernel first advances the int64 device counter `step`
+    and anneals with the new value; otherwise `step` is not read (None allowed) and the annealing value is `fin`.
+    `log` (a _native.LossLog, or None): the device loss log written by the same launch on a recording step.
+    -> (loss, coefs): coefs [na + nb] are the float coefficients the kernel used (not differentiable)."""
+
+    @staticmethod
+    def forward(ctx, a, b, coef_a, coef_b, sched_mask, anneal, is_train, step, log):
+        import ctypes
+        N.require_cuda_f32(a, b)
+        a = _c(a)
+        b = _c(b) if b is not None else None
+        na, nb = len(coef_a), (len(coef_b) if b is not None else 0)
+        base = (ctypes.c_double * (na + nb))(*(list(coef_a) + (list(coef_b) if nb else [])))
+        init, fin, steps_anneal = anneal
+        loss, coefs = _new((), a), _new((na + nb,), a)
+        call("dv_loss_combine_sched_fwd", ptr(a), na, ptr(b), nb, base, int(sched_mask), float(init), float(fin),
+             int(steps_anneal), int(bool(is_train)), ptr(step), ptr(loss), ptr(coefs), _log_arg(log), stream())
+        ctx.meta = (na, nb, a.numel(), tuple(b.shape) if b is not None else None)
+        ctx.save_for_backward(coefs)
+        ctx.mark_non_differentiable(coefs)
+        return loss, coefs
+
+    @staticmethod
+    def backward(ctx, g, _g_coefs):
+        coefs, = ctx.saved_tensors
+        na, nb, na_total, b_shape = ctx.meta
+        g = _c(g)
+        g_a = _new((na_total,), g)
+        g_b = _new(b_shape, g) if nb else None
+        call("dv_loss_combine_sched_bwd", ptr(g), ptr(coefs), na, na_total, nb, ptr(g_a), ptr(g_b), stream())
+        return g_a, g_b, None, None, None, None, None, None, None
+
+
+class BetaBLossFn(Function):
+    """beta-VAE_B's rec + gamma * |kl - C| (losses.py:199-200) from the fused loss kernel's output `out` = (rec, kl, ..),
+    with C = linear_annealing(c_init, c_fin, step, steps_anneal) formed on the device like LossCombineSchedFn's
+    coefficients (C_fin outside training).  Forward and backward are bit-identical to that torch expression and its
+    autograd gradient.  -> (loss, consts): consts = (C, gamma) as floats (not differentiable)."""
+
+    @staticmethod
+    def forward(ctx, out, gamma, c_anneal, is_train, step, log):
+        N.require_cuda_f32(out)
+        out = _c(out)
+        c_init, c_fin, steps_anneal = c_anneal
+        loss, consts = _new((), out), _new((2,), out)
+        call("dv_betab_loss_fwd", ptr(out), float(gamma), float(c_init), float(c_fin), int(steps_anneal),
+             int(bool(is_train)), ptr(step), ptr(loss), ptr(consts), _log_arg(log), stream())
+        ctx.save_for_backward(out, consts)
+        ctx.mark_non_differentiable(consts)
+        return loss, consts
+
+    @staticmethod
+    def backward(ctx, g, _g_consts):
+        out, consts = ctx.saved_tensors
+        g = _c(g)
+        g_out = torch.empty_like(out)
+        call("dv_betab_loss_bwd", ptr(g), ptr(out), ptr(consts), out.numel(), ptr(g_out), stream())
+        return g_out, None, None, None, None, None
+
+
+def loss_record(step, log):
+    """The device loss log on its own (dv_loss_record), predicated on the counter `step` as it stands."""
+    call("dv_loss_record", ptr(step), _log_arg(log), stream())
+
+
 def btcvae_rowstats(z, mu, logvar, n_data, is_mss=True):
     """(log_pz, log_qz, log_prod_qzi, log_q_zCx) like losses.py:523-544 (no autograd)."""
     with torch.no_grad():

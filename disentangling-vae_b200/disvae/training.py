@@ -17,6 +17,7 @@ from tqdm import trange
 
 from disvae import _native
 from disvae.fused import FusedAdam
+from disvae.models.losses import DeviceLossLog
 from disvae.parallel import FlatGradSync, is_distributed
 from disvae.utils.modelIO import save_model
 
@@ -49,6 +50,7 @@ class Trainer():
         self._device_loaders = {}                 # id(DataLoader) -> (DataLoader, its DeviceLoader)
         self._graphs = {}                         # input shape -> (CUDAGraph, static input, static loss)
         self._eligible_steps = 0
+        self._loss_log = None                     # DeviceLossLog of the training steps (built on the first GPU step)
         self.logger.info("Training Device: {}".format(self.device))
 
     def __call__(self, data_loader, epochs=10, checkpoint_every=10):
@@ -92,6 +94,7 @@ class Trainer():
                 t.update()
         if self._fused:
             self._fused.flush_state()                         # optimizer.state[p]["step"] follows the device counter
+        self._flush_loss_log()                                # this epoch's recorded scalars -> storer
         return epoch_loss.item() / len(data_loader)
 
     def _device_loader(self, loader):
@@ -119,7 +122,7 @@ class Trainer():
             self.optimizer.step()
 
     # -- whole-step CUDA graph ------------------------------------------------------------------
-    def _graph_eligible(self, data, storer):
+    def _graph_eligible(self, data):
         lf = self.loss_f
         if not (self.use_cuda_graph and self.device.type == "cuda" and self.model.training):
             return False
@@ -138,25 +141,25 @@ class Trainer():
                 return False
         if getattr(lf, "global_batch", False) and is_distributed():
             return False                                      # collectives inside the loss node: run eagerly
-        if lf.steps_anneal != 0 and lf.n_train_steps < lf.steps_anneal:
-            return False                                      # host-side annealing coefficient still moving
-        if storer is not None and (lf.n_train_steps + 1) % lf.record_loss_every == 1:
-            return False                                      # this step logs scalars (host sync): run eagerly
+        # annealing and recording steps are eligible: the coefficients and the loss log follow the loss's device counter
         if self._fused is None:
             self._fused = FusedAdam(self.optimizer) if FusedAdam.supports(self.optimizer) else False
         return bool(self._fused)
 
-    def _graph_step(self, data):
+    def _graph_step(self, data, storer):
         """fwd + loss + bwd (+ Adam when not data-parallel) of one batch as ONE CUDA graph launch (static
         shapes).  Data-parallel: the graph ends after the backward pass; its static gradient tensors are
         gathered into the flat buffer (one kernel), all-reduced (one NCCL call) and consumed by the fused
-        Adam launch with grad_scale = 1/world."""
+        Adam launch with grad_scale = 1/world.  The loss's device step counter advances inside the graph (annealing
+        coefficients, the device loss log of recording steps); the host counter follows here."""
         key = (tuple(data.shape), str(data.dtype))
         entry = self._graphs.get(key)
         ddp = is_distributed()
+        lf = self.loss_f
         if entry is None:
             static_x = torch.empty(data.shape, dtype=torch.float32, device=self.device)
             self._fill_static(static_x, data)
+            lf._step_counter(static_x.device, False)         # exists and is in step before capture: nothing to re-write in it
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             steps_before = self.loss_f.n_train_steps
@@ -182,7 +185,7 @@ class Trainer():
                         self._fused.step()
                         self._fused.host_steps -= 1               # capture executed nothing
                 static_loss = loss.detach()
-            self.loss_f.n_train_steps = steps_before
+            self.loss_f.n_train_steps = self.loss_f._step_dev_host = steps_before    # capture executed nothing
             flat = None
             if ddp:
                 params = [p for p in self.model.parameters() if p.grad is not None]
@@ -199,6 +202,9 @@ class Trainer():
             self._graphs[key] = entry
         g, static_x, static_loss, n_kernels, flat = entry
         self._fill_static(static_x, data)
+        lf._step_counter(static_x.device, False)             # (re-written only if n_train_steps was set by hand)
+        if self._loss_log is not None:
+            self._loss_log.expect(lf.n_train_steps + 1, lf.record_loss_every, storer)   # before the replay writes its row
         g.replay()
         _native.GRAPH_LAUNCHES += n_kernels
         if flat is not None:
@@ -213,6 +219,7 @@ class Trainer():
                 self.loss_f._fused_d.step(grad_scale=1.0 / dist.get_world_size())
                 self.loss_f._fused_d.host_steps -= 1
         self.loss_f.n_train_steps += 1
+        self.loss_f._step_dev_host += 1                       # the replay advanced the device counter
         self._fused.host_steps += 1
         if getattr(self.loss_f, "_fused_d", None):
             self.loss_f._fused_d.host_steps += 1
@@ -228,11 +235,24 @@ class Trainer():
             static_x.copy_(data, non_blocking=True)
 
     def _step(self, data, storer):
-        """One optimisation step; returns the loss as a detached 0-dim device tensor."""
-        if self._graph_eligible(data, storer):
+        """One optimisation step; returns the loss as a detached 0-dim device tensor.  On the GPU the scalars of a
+        recording step go to the device loss log (eager and graph steps alike) and reach `storer` at the next flush:
+        the end of the epoch, `_train_iteration`, or a full log."""
+        if self.device.type != "cuda":
+            return self._run_step(data, storer)
+        if self._loss_log is None:
+            self._loss_log = DeviceLossLog(self.device)
+        self.loss_f._log = self._loss_log
+        try:
+            return self._run_step(data, storer)
+        finally:
+            self.loss_f._log = None
+
+    def _run_step(self, data, storer):
+        if self._graph_eligible(data):
             self._eligible_steps += 1
             if self._eligible_steps > 2 or (tuple(data.shape), str(data.dtype)) in self._graphs:   # 2 eager warm-up steps first
-                return self._graph_step(data)
+                return self._graph_step(data, storer)
         data = data.to(self.device, non_blocking=True)
         if data.dtype == torch.uint8:                         # bytes over PCIe, ToTensor's /255 on the device
             from disvae import ops
@@ -258,8 +278,14 @@ class Trainer():
         return loss.detach()
 
     def _train_iteration(self, data, storer):
-        """training.py:137-164 (returns a Python float, i.e. synchronises)."""
-        return self._step(data, storer).item()
+        """training.py:137-164 (returns a Python float, i.e. synchronises; `storer` holds this step's scalars)."""
+        loss = self._step(data, storer).item()
+        self._flush_loss_log()
+        return loss
+
+    def _flush_loss_log(self):
+        if self._loss_log is not None:
+            self._loss_log.flush()
 
     # -- data parallel ---------------------------------------------------------------------
     def _sync_grads(self):

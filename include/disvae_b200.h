@@ -231,12 +231,52 @@ int dv_gather_u8_to_f32(const unsigned char* src, const long long* idx, int nrow
                         void* stream);
 /* loss[0] = sum_{i<na} coef_a[i]*a[i] + sum_{j<nb} coef_b[j]*b[j]; a, b device vectors, coef_* HOST arrays (<= 8 each,
  * passed to the kernel by value).  The scalar combinations of losses.py:151 (rec + anneal*beta*kl), :199-200 is not
- * covered (|kl - C|), :381-382 (rec + alpha*mi + beta*tc + anneal*gamma*dw_kl).  Backward: g_a[0..na_total) (zeros past
+ * covered (|kl - C|: dv_betab_loss_fwd below), :381-382 (rec + alpha*mi + beta*tc + anneal*gamma*dw_kl).  The training
+ * path uses the scheduled form below.  Backward: g_a[0..na_total) (zeros past
  * na), g_b[0..nb) from the upstream scalar g[0]. */
 int dv_loss_combine_fwd(const float* a, const float* coef_a, int na, const float* b, const float* coef_b, int nb,
                         float* loss, void* stream);
 int dv_loss_combine_bwd(const float* g, const float* coef_a, int na, int na_total, const float* coef_b, int nb,
                         float* g_a, float* g_b, void* stream);
+
+/* ---- annealed loss combinations and the device loss log (graph-capturable training steps) ----------
+ * Each loss owns an int64 device step counter (`step`).  On a training step (is_train != 0) the forward kernels first
+ * advance it by one, then anneal with the new value -- so a captured CUDA graph sees the step of every replay.
+ * The annealing value is linear_annealing (losses.py:511-518) in double, in Python's operation order:
+ *   A(step) = min(init + (fin - init) * step / steps_anneal, fin),  A = fin when steps_anneal == 0 or !is_train,
+ * and a coefficient is (float)(A * base), which is what ctypes made of the host product: bit-identical to the
+ * host-coefficient entry points above given the same step.
+ *
+ * Device loss log: on a training step whose counter value s satisfies s % every == 1 (the reference's record rule,
+ * losses.py:105-114), a kernel writes the concatenation of its sources into row ((s - 1) / every) % cap of ring
+ * [cap][ncols] (fp32, device).  The host reads rows back later; no host synchronisation inside the step.
+ * src[k] is a device pointer to len[k] floats; in the forward entry points a NULL src[k] of length 1 stands for the
+ * loss that launch computes.  sum(len) must equal ncols.  log == NULL (or !is_train): nothing is recorded. */
+#define DV_LOSS_LOG_MAX_SRC 8
+typedef struct dv_loss_log {
+  float* ring;
+  int cap, ncols, every, nsrc;
+  const float* src[DV_LOSS_LOG_MAX_SRC];
+  int len[DV_LOSS_LOG_MAX_SRC];
+} dv_loss_log;
+/* loss[0] = sum_{i<na} c[i]*a[i] + sum_{j<nb} c[na+j]*b[j] with c[k] = (float)(A * base[k]) if bit k of sched_mask is set,
+ * else (float)base[k]; base is a HOST array of na + nb doubles (na, nb <= 8).  coefs[na + nb] (device) receives the c[k]
+ * used; the backward reads them: g_a[0..na_total) (zeros past na), g_b[0..nb) from the upstream scalar g[0]. */
+int dv_loss_combine_sched_fwd(const float* a, int na, const float* b, int nb, const double* base, unsigned sched_mask,
+                              double init, double fin, long long steps_anneal, int is_train, long long* step, float* loss,
+                              float* coefs, const dv_loss_log* log, void* stream);
+int dv_loss_combine_sched_bwd(const float* g, const float* coefs, int na, int na_total, int nb, float* g_a, float* g_b,
+                              void* stream);
+/* beta-VAE_B (losses.py:199-200): loss = rec + gamma * |kl - C| with rec = rec_kl[0], kl = rec_kl[1] (the output of
+ * dv_vae_loss_fwd) and C = (float)A(step) for (init, fin) = (c_init, c_fin); rounded like the torch expression (kl - C
+ * and gamma * |.| in float, gamma = (float)gamma).  consts[2] (device) receives (C, gamma).  Backward: g_rec_kl[0] = g,
+ * g_rec_kl[1] = (g * gamma) * sign(kl - C) with sign(0) = 0 -- torch's abs backward -- and zeros up to n. */
+int dv_betab_loss_fwd(const float* rec_kl, double gamma, double c_init, double c_fin, long long steps_anneal, int is_train,
+                      long long* step, float* loss, float* consts, const dv_loss_log* log, void* stream);
+int dv_betab_loss_bwd(const float* g, const float* rec_kl, const float* consts, int n, float* g_rec_kl, void* stream);
+/* The log alone (no NULL sources), predicated on the counter as it stands: for scalars computed after the loss
+ * combination (FactorVAE's discriminator loss). */
+int dv_loss_record(const long long* step, const dv_loss_log* log, void* stream);
 /* g = dy * act'(y) over an NCHW tensor [B, C <= 4, hw] fused with chansum[c] = sum_{b,hw} g (the bias gradient of the
  * ConvTranspose2d that produced y; decoders.py:82).  workspace: dv_channel_sum_workspace_bytes(). */
 int dv_act_bwd_chansum(const float* dy, const float* y, float* g, int B, int C, int hw, int act, float slope,

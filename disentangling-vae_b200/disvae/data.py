@@ -142,11 +142,16 @@ class DeviceLoader:
             perm = torch.cat([perm, perm[:self.n_padded - self.n]])
         return perm[:self.n_padded]
 
-    def __iter__(self):
+    def epoch_indices(self):
+        """The dataset indices of each batch of the next epoch (CUDA int64 views of one permutation); what `iter()`
+        gathers.  Advances the epoch like `iter()`."""
         order = self.order(self.epoch)
         self.epoch += 1
         for start, size in self.windows:
-            idx = order[start:start + size]
+            yield order[start:start + size]
+
+    def __iter__(self):
+        for idx in self.epoch_indices():
             yield ops.gather_u8_to_f32(self.data, idx), idx
 
     def __len__(self):

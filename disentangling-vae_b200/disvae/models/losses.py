@@ -153,6 +153,11 @@ class DeviceLossLog:
         self.pending.clear()
 
 
+def permutation_key(seed, salt=0):
+    """Philox key of FactorVAE's latent permutations in a process seeded with `seed` (`salt`: parallel.rank_salt())."""
+    return ((int(seed) ^ 0x9E3779B97F4A7C15) + salt) & 0xFFFFFFFFFFFFFFFF
+
+
 class BaseLoss(abc.ABC):
     """losses.py:52-114: step counter, record-every-50 policy, common options.
 
@@ -297,9 +302,14 @@ class FactorKLoss(BaseLoss):
     def _perm_state(self, device):
         if self._perm_offset is None or self._perm_offset.device != device:
             from disvae.parallel import rank_salt
-            self._perm_seed = ((int(torch.initial_seed()) ^ 0x9E3779B97F4A7C15) + rank_salt()) & 0xFFFFFFFFFFFFFFFF
-            self._perm_offset = torch.zeros(1, dtype=torch.int64, device=device)
+            self.seed_permutations(permutation_key(torch.initial_seed(), rank_salt()), device)
         return self._perm_seed, self._perm_offset
+
+    def seed_permutations(self, key, device):
+        """Fix the Philox key of the latent permutations (what the first training step would take from
+        torch.initial_seed(); permutation_key) and start its counter at 0 on `device`."""
+        self._perm_seed = int(key)
+        self._perm_offset = torch.zeros(1, dtype=torch.int64, device=device)
 
     def _global_perm_state(self, device):
         """Key of the global permutation: rank 0's seed, unsalted (one process with the same seed draws the same

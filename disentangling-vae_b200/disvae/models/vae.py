@@ -21,6 +21,11 @@ def init_specific_model(model_type, img_size, latent_dim):
     return model
 
 
+def noise_key(seed, salt=0):
+    """Philox key of the reparameterisation noise of a process seeded with `seed` (`salt`: parallel.rank_salt())."""
+    return (int(seed) + salt) & 0xFFFFFFFFFFFFFFFF
+
+
 class VAE(nn.Module):
     def __init__(self, img_size, encoder, decoder, latent_dim):
         super().__init__()
@@ -42,9 +47,14 @@ class VAE(nn.Module):
         if self._rng_offset is None or self._rng_offset.device != device:
             from disvae.parallel import rank_salt
             # identically seeded replicas (main.py's set_seed) must still draw different noise for their shards
-            self._rng_seed = (int(torch.initial_seed()) + rank_salt()) & 0xFFFFFFFFFFFFFFFF
-            self._rng_offset = torch.zeros(1, dtype=torch.int64, device=device)
+            self.seed_noise(noise_key(torch.initial_seed(), rank_salt()), device)
         return self._rng_seed, self._rng_offset
+
+    def seed_noise(self, key, device):
+        """Fix the Philox key of the reparameterisation noise (what the first training step would take from
+        torch.initial_seed(); noise_key) and start its counter at 0 on `device`."""
+        self._rng_seed = int(key)
+        self._rng_offset = torch.zeros(1, dtype=torch.int64, device=device)
 
     def reparameterize(self, mean, logvar, eps=None):
         """vae.py:52-71.  Training: mean + exp(0.5*logvar) * eps with eps ~ N(0,1) drawn on the

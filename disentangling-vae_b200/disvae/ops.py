@@ -4,6 +4,9 @@ PyTorch is plumbing here: it owns device memory, streams and the autograd tape b
 big nodes (encoder, decoder, discriminator, loss heads).  Every FLOP of the hot path runs in
 libdisvae_b200.so.  All functions require CUDA fp32 tensors and raise otherwise.
 """
+import contextlib
+import os as _os
+
 import torch
 from torch.autograd import Function
 
@@ -17,27 +20,62 @@ DISC_SLOPE = 0.2    # discriminator.py:10
 # ---------------------------------------------------------------------------------------
 # persistent, zero-initialised scratch (kernels that use a "last block done" counter leave
 # it at zero, so one buffer per device can be reused across calls on the same stream)
+#
+# Every per-process resource below -- this scratch, the beta-TCVAE workspaces and the weight-gradient side stream -- is
+# keyed by the current owner as well as the device.  The owner is None except inside `owner(token)`: disvae.sweep runs
+# each member's eager steps and graph capture under its own token, so members whose graphs replay concurrently never
+# share a split-K partial buffer, a "last block done" counter or a side stream.
 # ---------------------------------------------------------------------------------------
 _persist = {}
+_in_graph = set()      # keys of _persist whose current buffer was handed out during a CUDA-graph capture
+_retired = {}          # owner -> such buffers after a larger one replaced them: the graph still reads their addresses
+_owner = None
+
+
+@contextlib.contextmanager
+def owner(token):
+    """Kernels called inside use the scratch, workspaces and side stream of `token` (any hashable; None = the
+    process-wide set a lone Trainer uses)."""
+    global _owner
+    old, _owner = _owner, token
+    try:
+        yield
+    finally:
+        _owner = old
+
+
+def release(token):
+    """Drop the scratch, workspaces and side stream of owner `token` (once nothing that uses them can run again)."""
+    for table in (_persist, _bt_pool, _side_streams):
+        for k in [k for k in table if k[-1] == token]:
+            del table[k]
+    _in_graph.difference_update([k for k in _in_graph if k[-1] == token])
+    _retired.pop(token, None)
+
+
+def _persistent(key, nbytes, device, alloc):
+    k = (key, device.index, _owner)
+    buf = _persist.get(k)
+    if buf is None or buf.numel() * 4 < nbytes:
+        # A buffer only eager kernels used is freed: each key is used on one stream, and the caching allocator hands the
+        # block only to later work on that stream.  One a captured graph baked in must outlive the graph: kept.
+        if k in _in_graph:
+            _retired.setdefault(_owner, []).append(buf)
+            _in_graph.discard(k)
+        buf = alloc((nbytes + 3) // 4, dtype=torch.float32, device=device)
+        _persist[k] = buf
+    if torch.cuda.is_current_stream_capturing():
+        _in_graph.add(k)
+    return buf
 
 
 def _zero_ws(key, nbytes, device):
-    k = (key, device.index)
-    buf = _persist.get(k)
-    if buf is None or buf.numel() * 4 < nbytes:
-        buf = torch.zeros((nbytes + 3) // 4, dtype=torch.float32, device=device)
-        _persist[k] = buf
-    return buf
+    return _persistent(key, nbytes, device, torch.zeros)
 
 
 def _scratch(key, nbytes, device):
     """Non-zeroed scratch, grown on demand (channel sums, wgrad partials)."""
-    k = (key, device.index)
-    buf = _persist.get(k)
-    if buf is None or buf.numel() * 4 < nbytes:
-        buf = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=device)
-        _persist[k] = buf
-    return buf
+    return _persistent(key, nbytes, device, torch.empty)
 
 
 def _new(shape, like):
@@ -253,9 +291,6 @@ def _c(t):
 # dependencies).  Tensors read on the side stream are kept alive until the join, so the caching allocator cannot hand
 # their memory to the main stream meanwhile.  DISVAE_SIDE_STREAM=0 switches it off (same kernels, same results).
 # ---------------------------------------------------------------------------------------
-import contextlib
-import os as _os
-
 _side_streams = {}
 
 
@@ -265,9 +300,10 @@ class _WgradLane:
         self.keep = []
         if self.enabled:
             self.main = torch.cuda.current_stream(device)
-            side = _side_streams.get(device.index)
+            key = (device.index, _owner)
+            side = _side_streams.get(key)
             if side is None:
-                side = _side_streams[device.index] = torch.cuda.Stream(device)
+                side = _side_streams[key] = torch.cuda.Stream(device)
             self.side = side
 
     def run(self, fn, *reads):
@@ -618,7 +654,7 @@ def _bt_new_workspace(B, D, device):
 
 
 def _bt_workspace(B, D, device):
-    key = (B, D, device.index)
+    key = (B, D, device.index, _owner)
     ent = _bt_pool.get(key)
     if ent is not None and not ent[1]:
         ent[1] = True

@@ -51,6 +51,8 @@ class Trainer():
         self._graphs = {}                         # input shape -> (CUDAGraph, static input, static loss)
         self._eligible_steps = 0
         self._loss_log = None                     # DeviceLossLog of the training steps (built on the first GPU step)
+        self._resident_input = None               # fp32 device batch a caller refills in place (disvae.sweep): a graph
+                                                  # captured on it reads it directly instead of a copy
         self.logger.info("Training Device: {}".format(self.device))
 
     def __call__(self, data_loader, epochs=10, checkpoint_every=10):
@@ -62,12 +64,19 @@ class Trainer():
         for epoch in range(epochs):
             storer = defaultdict(list)
             mean_epoch_loss = self._train_epoch(data_loader, storer, epoch)
-            self.logger.info('Epoch: {} Average loss per image: {:.2f}'.format(epoch + 1, mean_epoch_loss))
-            self.losses_logger.log(epoch, storer)
-            if self.gif_visualizer is not None:
-                self.gif_visualizer()
-            if epoch % checkpoint_every == 0:
-                save_model(self.model, self.save_dir, filename="model-{}.pt".format(epoch))
+            self._end_epoch(epoch, storer, mean_epoch_loss, checkpoint_every)
+        self._end_training(start)
+
+    def _end_epoch(self, epoch, storer, mean_epoch_loss, checkpoint_every):
+        """training.py:84-90: epoch log line, train_losses.log rows, GIF frame, checkpoint."""
+        self.logger.info('Epoch: {} Average loss per image: {:.2f}'.format(epoch + 1, mean_epoch_loss))
+        self.losses_logger.log(epoch, storer)
+        if self.gif_visualizer is not None:
+            self.gif_visualizer()
+        if epoch % checkpoint_every == 0:
+            save_model(self.model, self.save_dir, filename="model-{}.pt".format(epoch))
+
+    def _end_training(self, start):
         if self.gif_visualizer is not None:
             self.gif_visualizer.save_reset()
         self.model.eval()
@@ -76,26 +85,13 @@ class Trainer():
 
     def _train_epoch(self, data_loader, storer, epoch):
         """training.py:104-135; the epoch loss is accumulated on the device."""
-        kwargs = dict(desc="Epoch {}".format(epoch + 1), leave=False, disable=not self.is_progress_bar)
         on_gpu = self.device.type == "cuda"
-        # own accumulator, updated in place: `loss` may be the CUDA graph's static output tensor, which the next
-        # replay overwrites -- never keep a reference to it across steps
-        epoch_loss = torch.zeros((), dtype=torch.float32, device=self.device)
         batches = _Prefetcher(data_loader, self.device) if on_gpu else data_loader
-        ring = self._loss_ring() if on_gpu else None
-        with trange(len(data_loader), **kwargs) as t:
-            for i, (data, _) in enumerate(batches):
-                loss = self._step(data, storer)
-                epoch_loss += loss
-                if ring is not None:
-                    ring.push(loss)                           # async D2H of this step's loss (4 bytes)
-                if self.is_progress_bar and i % self.sync_every == 0:
-                    t.set_postfix(loss=ring.latest() if ring is not None else loss.item())
-                t.update()
-        if self._fused:
-            self._fused.flush_state()                         # optimizer.state[p]["step"] follows the device counter
-        self._flush_loss_log()                                # this epoch's recorded scalars -> storer
-        return epoch_loss.item() / len(data_loader)
+        tally = _EpochTally(self, len(data_loader), epoch)
+        with tally.bar:
+            for data, _ in batches:
+                tally.add(self._step(data, storer))
+        return tally.close()
 
     def _device_loader(self, loader):
         """The DeviceLoader standing in for `loader`, built (the dataset decoded and uploaded) once per loader."""
@@ -157,8 +153,11 @@ class Trainer():
         ddp = is_distributed()
         lf = self.loss_f
         if entry is None:
-            static_x = torch.empty(data.shape, dtype=torch.float32, device=self.device)
-            self._fill_static(static_x, data)
+            if data is self._resident_input:
+                static_x = data                               # the caller refills this very tensor before each step
+            else:
+                static_x = torch.empty(data.shape, dtype=torch.float32, device=self.device)
+                self._fill_static(static_x, data)
             lf._step_counter(static_x.device, False)         # exists and is in step before capture: nothing to re-write in it
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
@@ -201,7 +200,8 @@ class Trainer():
             entry = (g, static_x, static_loss, _native.lib().dv_launch_count() - launches_before, flat)
             self._graphs[key] = entry
         g, static_x, static_loss, n_kernels, flat = entry
-        self._fill_static(static_x, data)
+        if data is not static_x:
+            self._fill_static(static_x, data)
         lf._step_counter(static_x.device, False)             # (re-written only if n_train_steps was set by hand)
         if self._loss_log is not None:
             self._loss_log.expect(lf.n_train_steps + 1, lf.record_loss_every, storer)   # before the replay writes its row
@@ -334,6 +334,36 @@ class Trainer():
         return loss.detach()
 
 
+class _EpochTally:
+    """One epoch of a Trainer's bookkeeping: the running loss (on the device), the host loss ring behind the progress
+    bar, and at the end the optimizer step counters and the device loss log brought up to date."""
+
+    def __init__(self, trainer, n_batches, epoch):
+        self.tr, self.n, self.i = trainer, n_batches, 0
+        # own accumulator, updated in place: `loss` may be the CUDA graph's static output tensor, which the next
+        # replay overwrites -- never keep a reference to it across steps
+        self.loss = torch.zeros((), dtype=torch.float32, device=trainer.device)
+        self.ring = trainer._loss_ring() if trainer.device.type == "cuda" else None
+        self.bar = trange(n_batches, desc="Epoch {}".format(epoch + 1), leave=False, disable=not trainer.is_progress_bar)
+
+    def add(self, loss):
+        self.loss += loss
+        if self.ring is not None:
+            self.ring.push(loss)                              # async D2H of this step's loss (4 bytes)
+        if self.tr.is_progress_bar and self.i % self.tr.sync_every == 0:
+            self.bar.set_postfix(loss=self.ring.latest() if self.ring is not None else loss.item())
+        self.bar.update()
+        self.i += 1
+
+    def close(self):
+        """-> the mean loss of the epoch's batches (synchronises)."""
+        self.bar.close()
+        if self.tr._fused:
+            self.tr._fused.flush_state()                      # optimizer.state[p]["step"] follows the device counter
+        self.tr._flush_loss_log()                             # this epoch's recorded scalars -> storer
+        return self.loss.item() / self.n
+
+
 class _Prefetcher:
     """Iterates a loader of (data, label) batches one step ahead: the host->device copy of batch i+1 is issued
     on a copy stream while step i runs (two device buffers, reused).  Pageable host tensors still work (the copy
@@ -434,7 +464,10 @@ class LossesLogger(object):
     def __init__(self, file_path_name):
         if os.path.isfile(file_path_name):
             os.remove(file_path_name)
-        self.logger = logging.getLogger("losses_logger")
+        # a logger of its own, not the shared named one: several Trainers in one process (disvae.sweep) each write
+        # only their own file
+        self.logger = logging.Logger("losses_logger")
+        self.logger.parent = logging.getLogger("losses_logger")
         self.logger.setLevel(1)
         file_handler = logging.FileHandler(file_path_name)
         file_handler.setLevel(1)

@@ -30,6 +30,16 @@ class FusedAdam:
                 n += 1
         return 0 < n
 
+    @staticmethod
+    def lazy(holder, attr, optimizer):
+        """`holder.<attr>`: the FusedAdam over `optimizer`, built at the first call (once the parameters are on the
+        device); False where `supports` says no, and the caller keeps `optimizer.step()`."""
+        fused = getattr(holder, attr)
+        if fused is None:
+            fused = FusedAdam(optimizer) if FusedAdam.supports(optimizer) else False
+            setattr(holder, attr, fused)
+        return fused
+
     def __init__(self, optimizer):
         assert FusedAdam.supports(optimizer)
         self.optimizer = optimizer

@@ -289,10 +289,9 @@ class FactorKLoss(BaseLoss):
     def _step_d(self):
         """Discriminator Adam step: dv_adam_multi when optimizer_d is a plain CUDA Adam."""
         from disvae.fused import FusedAdam
-        if self._fused_d is None:
-            self._fused_d = FusedAdam(self.optimizer_d) if FusedAdam.supports(self.optimizer_d) else False
-        if self._fused_d:
-            self._fused_d.step()
+        fused = FusedAdam.lazy(self, "_fused_d", self.optimizer_d)
+        if fused:
+            fused.step()
         else:
             self.optimizer_d.step()
 
@@ -337,8 +336,8 @@ class FactorKLoss(BaseLoss):
     def call_optimize(self, data, model, optimizer, storer, eps1=None, eps2=None, perms=None, step_optimizers=True):
         """losses.py:243-313.  `eps1`/`eps2`/`perms` optionally inject the noise of the two
         halves and the per-dimension permutations ([D, B/2] int64; [D, world*B/2] in global-batch mode) for parity tests.
-        `step_optimizers=False` (data parallel): both backward passes run, neither optimizer steps -- the
-        Trainer steps them after the gradients of all ranks are averaged."""
+        `step_optimizers=False`: both backward passes run, neither optimizer steps -- the Trainer steps them
+        itself (under data parallelism after the gradients of all ranks are averaged)."""
         storer = self._pre_call(model.training, storer)
         half = data.size(0) // 2
         parts = data.split(half)

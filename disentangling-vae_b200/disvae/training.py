@@ -9,7 +9,7 @@ torch.distributed (one process per GPU) gradients are averaged with one flat all
 """
 import logging
 import os
-from collections import defaultdict
+from collections import defaultdict, namedtuple
 from timeit import default_timer
 
 import torch
@@ -18,7 +18,7 @@ from tqdm import trange
 from disvae import _native
 from disvae.fused import FusedAdam
 from disvae.models.losses import DeviceLossLog
-from disvae.parallel import FlatGradSync, is_distributed
+from disvae.parallel import FlatGradSync, broadcast_parameters, is_distributed
 from disvae.utils.modelIO import save_model
 
 TRAIN_LOSSES_LOGFILE = "train_losses.log"
@@ -48,7 +48,7 @@ class Trainer():
         # dataset (decoded once, kept on the GPU; its own shuffle stream, hence opt-in)
         self.device_data = os.environ.get("DISVAE_DEVICE_DATA", "0") == "1"
         self._device_loaders = {}                 # id(DataLoader) -> (DataLoader, its DeviceLoader)
-        self._graphs = {}                         # input shape -> (CUDAGraph, static input, static loss)
+        self._graphs = {}                         # (input shape, dtype) -> _Graph of the captured step
         self._eligible_steps = 0
         self._loss_log = None                     # DeviceLossLog of the training steps (built on the first GPU step)
         self._resident_input = None               # fp32 device batch a caller refills in place (disvae.sweep): a graph
@@ -106,16 +106,69 @@ class Trainer():
             self._ring = _HostLossRing(self.device)
         return self._ring
 
-    # -- optimizer ---------------------------------------------------------------------------
-    def _optimizer_step(self, grad_scale=1.0):
-        """Adam through dv_adam_multi when `optimizer` is a plain torch.optim.Adam on CUDA parameters,
-        else the optimizer's own step()."""
-        if self._fused is None:
-            self._fused = FusedAdam(self.optimizer) if FusedAdam.supports(self.optimizer) else False
-        if self._fused:
-            self._fused.step(grad_scale)
+    # -- the pieces of a training step ----------------------------------------------------------
+    def _device_batch(self, data, out=None):
+        """`data` as the fp32 batch on the device, written into `out` when given.  uint8 batches (SURVEY.md 8f-3) are
+        uploaded as bytes and converted by dv_u8_to_f32 (ToTensor's /255), float batches are copied."""
+        if data.dtype == torch.uint8:
+            from disvae import ops
+            return ops.u8_to_f32(data.to(self.device, non_blocking=True), out=out)
+        if out is None:
+            return data.to(self.device, non_blocking=True)
+        return out.copy_(data, non_blocking=True)
+
+    def _discarded_forward(self, x):
+        """FactorVAE: the full-batch forward pass whose result the reference discards (training.py:153), kept for its
+        noise draw."""
+        if hasattr(self.loss_f, "call_optimize"):
+            with torch.no_grad():
+                self.model(x)
+
+    def _forward_backward(self, x, storer, **inject):
+        """Forward pass, loss and backward pass of the fp32 device batch `x`; returns the detached loss.  Afterwards
+        every `p.grad` (FactorVAE: the discriminator's too) holds this process's gradient.  `inject` forwards
+        eps1/eps2/perms to FactorKLoss.call_optimize."""
+        if hasattr(self.loss_f, "call_optimize"):             # several optimizers (training.py:160-162): both backward passes
+            disc = self.loss_f.discriminator
+            if is_distributed() and self._grad_sync_d is None:
+                broadcast_parameters(disc)                    # replicas must start from identical discriminators
+                self._grad_sync_d = FlatGradSync(list(disc.parameters()))
+            loss = self.loss_f.call_optimize(x, self.model, self.optimizer, storer, step_optimizers=False, **inject)
         else:
-            self.optimizer.step()
+            recon_batch, latent_dist, latent_sample = self.model(x)
+            loss = self.loss_f(x, recon_batch, latent_dist, self.model.training, storer, latent_sample=latent_sample)
+            self.optimizer.zero_grad()
+            loss.backward()
+        return loss.detach()
+
+    def _average_grads(self):
+        """Data parallel: the rank-average of the model's and the discriminator's gradients, in place (one flat
+        all-reduce each).  No-op in one process."""
+        if not is_distributed():
+            return
+        if self._grad_sync is None:
+            self._grad_sync = FlatGradSync(list(self.model.parameters()))
+        self._grad_sync.sync()
+        if self._grad_sync_d is not None:
+            self._grad_sync_d.sync()
+
+    def _optimizers(self):
+        """(optimizer, its FusedAdam or False) of each network a step updates: the model and, for FactorVAE, the
+        discriminator."""
+        pairs = [(self.optimizer, FusedAdam.lazy(self, "_fused", self.optimizer))]
+        lf = self.loss_f
+        if hasattr(lf, "call_optimize"):
+            pairs.append((lf.optimizer_d, FusedAdam.lazy(lf, "_fused_d", lf.optimizer_d)))
+        return pairs
+
+    def _optimizer_steps(self, grad_scale=1.0):
+        """The Adam step of each network: dv_adam_multi on the gradients times `grad_scale` when FusedAdam takes the
+        optimizer over (a plain torch.optim.Adam on CUDA parameters), else the optimizer's own step()."""
+        for opt, fused in self._optimizers():
+            if fused:
+                fused.step(grad_scale)
+            else:
+                opt.step()
 
     # -- whole-step CUDA graph ------------------------------------------------------------------
     def _graph_eligible(self, data):
@@ -131,108 +184,82 @@ class Trainer():
                 return False
             if is_distributed() and self._grad_sync_d is None:
                 return False                                  # the discriminators are broadcast by the first eager step
-            if lf._fused_d is None:
-                lf._fused_d = FusedAdam(lf.optimizer_d) if FusedAdam.supports(lf.optimizer_d) else False
-            if not lf._fused_d:
+            if not FusedAdam.lazy(lf, "_fused_d", lf.optimizer_d):
                 return False
         if getattr(lf, "global_batch", False) and is_distributed():
             return False                                      # collectives inside the loss node: run eagerly
         # annealing and recording steps are eligible: the coefficients and the loss log follow the loss's device counter
-        if self._fused is None:
-            self._fused = FusedAdam(self.optimizer) if FusedAdam.supports(self.optimizer) else False
-        return bool(self._fused)
+        return bool(FusedAdam.lazy(self, "_fused", self.optimizer))
+
+    def _capture(self, data):
+        """The _Graph of a training step on batches like `data`: the discarded forward (FactorVAE), forward + loss +
+        backward and, in one process, the Adam steps.  Capture executes nothing, so the host step counters that the
+        step's code advances are put back; each replay advances them (`_graph_step`)."""
+        if data is self._resident_input:
+            static_x = data                                   # the caller refills this very tensor before each step
+        else:
+            static_x = self._device_batch(data, out=torch.empty(data.shape, dtype=torch.float32, device=self.device))
+        lf, ddp = self.loss_f, is_distributed()
+        adams = [fused for _, fused in self._optimizers()]
+        lf._step_counter(static_x.device, False)             # exists and is in step before capture: nothing to re-write in it
+        counters = (lf.n_train_steps, lf._step_dev_host, [f.host_steps for f in adams])
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        launches_before = _native.lib().dv_launch_count()
+        with torch.cuda.graph(g):
+            self._discarded_forward(static_x)
+            static_loss = self._forward_backward(static_x, None)
+            if not ddp:                                       # data parallel: the optimizers step after the average
+                self._optimizer_steps()
+        n_kernels = _native.lib().dv_launch_count() - launches_before
+        lf.n_train_steps, lf._step_dev_host = counters[:2]
+        for f, n in zip(adams, counters[2]):
+            f.host_steps = n
+        reduce = None
+        if ddp:
+            params = [p for p in self.model.parameters() if p.grad is not None]
+            if hasattr(lf, "call_optimize"):                  # one flat buffer (one all-reduce) for both networks
+                params += [p for p in lf.discriminator.parameters() if p.grad is not None]
+            static_grads = [p.grad.view(-1) for p in params]  # written by every replay
+            flat = torch.zeros(sum(t.numel() for t in static_grads), dtype=torch.float32, device=self.device)
+            off, views = 0, []
+            for p in params:                                  # Adam reads the all-reduced flat views
+                views.append(flat[off:off + p.numel()].view_as(p))
+                off += p.numel()
+            reduce = (flat, static_grads, params, views)
+        return _Graph(g, static_x, static_loss, n_kernels, reduce, () if ddp else tuple(adams))
 
     def _graph_step(self, data, storer):
         """fwd + loss + bwd (+ Adam when not data-parallel) of one batch as ONE CUDA graph launch (static
         shapes).  Data-parallel: the graph ends after the backward pass; its static gradient tensors are
         gathered into the flat buffer (one kernel), all-reduced (one NCCL call) and consumed by the fused
         Adam launch with grad_scale = 1/world.  The loss's device step counter advances inside the graph (annealing
-        coefficients, the device loss log of recording steps); the host counter follows here."""
+        coefficients, the device loss log of recording steps); the host counters follow here."""
         key = (tuple(data.shape), str(data.dtype))
         entry = self._graphs.get(key)
-        ddp = is_distributed()
-        lf = self.loss_f
         if entry is None:
-            if data is self._resident_input:
-                static_x = data                               # the caller refills this very tensor before each step
-            else:
-                static_x = torch.empty(data.shape, dtype=torch.float32, device=self.device)
-                self._fill_static(static_x, data)
-            lf._step_counter(static_x.device, False)         # exists and is in step before capture: nothing to re-write in it
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            steps_before = self.loss_f.n_train_steps
-            launches_before = _native.lib().dv_launch_count()
-            factor = hasattr(self.loss_f, "call_optimize")
-            with torch.cuda.graph(g):
-                if factor:
-                    with torch.no_grad():
-                        self.model(static_x)                      # the discarded full-batch forward of training.py:153:
-                                                                  # kept for its noise draw (same stream as the eager path)
-                    if ddp:                                       # both backward passes; the optimizers step after the average
-                        loss = self.loss_f.call_optimize(static_x, self.model, self.optimizer, None, step_optimizers=False)
-                    else:
-                        loss = self.loss_f.call_optimize(static_x, self.model, _StepProxy(self.optimizer, self._optimizer_step), None)
-                        self._fused.host_steps -= 1               # capture executed nothing
-                        self.loss_f._fused_d.host_steps -= 1
-                else:
-                    recon, latent_dist, z = self.model(static_x)
-                    loss = self.loss_f(static_x, recon, latent_dist, True, None, latent_sample=z)
-                    self.optimizer.zero_grad(set_to_none=True)
-                    loss.backward()
-                    if not ddp:
-                        self._fused.step()
-                        self._fused.host_steps -= 1               # capture executed nothing
-                static_loss = loss.detach()
-            self.loss_f.n_train_steps = self.loss_f._step_dev_host = steps_before    # capture executed nothing
-            flat = None
-            if ddp:
-                params = [p for p in self.model.parameters() if p.grad is not None]
-                if factor:                                        # one flat buffer (one all-reduce) for both networks
-                    params += [p for p in self.loss_f.discriminator.parameters() if p.grad is not None]
-                static_grads = [p.grad for p in params]           # written by every replay
-                flat_buf = torch.zeros(sum(t.numel() for t in static_grads), dtype=torch.float32, device=self.device)
-                off, views = 0, []
-                for p in params:                                  # Adam reads the all-reduced flat views
-                    views.append(flat_buf[off:off + p.numel()].view_as(p))
-                    off += p.numel()
-                flat = (flat_buf, [t.view(-1) for t in static_grads], params, views)
-            entry = (g, static_x, static_loss, _native.lib().dv_launch_count() - launches_before, flat)
-            self._graphs[key] = entry
-        g, static_x, static_loss, n_kernels, flat = entry
-        if data is not static_x:
-            self._fill_static(static_x, data)
-        lf._step_counter(static_x.device, False)             # (re-written only if n_train_steps was set by hand)
+            entry = self._graphs[key] = self._capture(data)
+        elif data is not entry.static_x:
+            self._device_batch(data, out=entry.static_x)
+        lf = self.loss_f
+        lf._step_counter(entry.static_x.device, False)       # (re-written only if n_train_steps was set by hand)
         if self._loss_log is not None:
             self._loss_log.expect(lf.n_train_steps + 1, lf.record_loss_every, storer)   # before the replay writes its row
-        g.replay()
-        _native.GRAPH_LAUNCHES += n_kernels
-        if flat is not None:
+        entry.graph.replay()
+        _native.GRAPH_LAUNCHES += entry.n_kernels
+        if entry.reduce is not None:
             import torch.distributed as dist
-            torch.cat(flat[1], out=flat[0])
-            dist.all_reduce(flat[0], op=dist.ReduceOp.SUM)
-            for p, v in zip(flat[2], flat[3]):                    # (an eager step in between re-binds .grad)
+            flat, static_grads, params, views = entry.reduce
+            torch.cat(static_grads, out=flat)
+            dist.all_reduce(flat, op=dist.ReduceOp.SUM)
+            for p, v in zip(params, views):                   # (an eager step in between re-binds .grad)
                 p.grad = v
-            self._fused.step(grad_scale=1.0 / dist.get_world_size())
-            self._fused.host_steps -= 1
-            if hasattr(self.loss_f, "call_optimize"):
-                self.loss_f._fused_d.step(grad_scale=1.0 / dist.get_world_size())
-                self.loss_f._fused_d.host_steps -= 1
-        self.loss_f.n_train_steps += 1
-        self.loss_f._step_dev_host += 1                       # the replay advanced the device counter
-        self._fused.host_steps += 1
-        if getattr(self.loss_f, "_fused_d", None):
-            self.loss_f._fused_d.host_steps += 1
-        return static_loss
-
-    def _fill_static(self, static_x, data):
-        """The graph's input buffer <- this step's batch.  uint8 batches (SURVEY.md 8f-3) are uploaded as bytes and
-        converted by dv_u8_to_f32 straight into the buffer (ToTensor's /255), float batches are copied."""
-        if data.dtype == torch.uint8:
-            from disvae import ops
-            ops.u8_to_f32(data.to(self.device, non_blocking=True), out=static_x)
-        else:
-            static_x.copy_(data, non_blocking=True)
+            self._optimizer_steps(grad_scale=1.0 / dist.get_world_size())
+        lf.n_train_steps += 1                                 # the replay's work on the host counters
+        lf._step_dev_host += 1
+        for f in entry.adams:
+            f.host_steps += 1
+        return entry.static_loss
 
     def _step(self, data, storer):
         """One optimisation step; returns the loss as a detached 0-dim device tensor.  On the GPU the scalars of a
@@ -253,29 +280,14 @@ class Trainer():
             self._eligible_steps += 1
             if self._eligible_steps > 2 or (tuple(data.shape), str(data.dtype)) in self._graphs:   # 2 eager warm-up steps first
                 return self._graph_step(data, storer)
-        data = data.to(self.device, non_blocking=True)
-        if data.dtype == torch.uint8:                         # bytes over PCIe, ToTensor's /255 on the device
-            from disvae import ops
-            data = ops.u8_to_f32(data)
-        recon_batch, latent_dist, latent_sample = self.model(data)
-        try:
-            loss = self.loss_f(data, recon_batch, latent_dist, self.model.training, storer, latent_sample=latent_sample)
-        except ValueError:
-            # losses with several optimizers (FactorVAE) announce themselves by raising from __call__
-            # (training.py:160-162, losses.py:240-241).  Only the loss call is inside the `try`: a ValueError from
-            # anywhere else in the step (a kernel-side shape check, the optimizer) must surface, not be rerouted.
-            if not hasattr(self.loss_f, "call_optimize"):
-                raise
-            if is_distributed():
-                loss = self._factor_step_distributed(data, storer)
-            else:
-                loss = self.loss_f.call_optimize(data, self.model, _StepProxy(self.optimizer, self._optimizer_step), storer)
-            return loss.detach()
-        self.optimizer.zero_grad()
-        loss.backward()
-        self._sync_grads()
-        self._optimizer_step()
-        return loss.detach()
+        x = self._device_batch(data)
+        self._discarded_forward(x)
+        loss = self._forward_backward(x, storer)
+        if self.model.training or not hasattr(self.loss_f, "call_optimize"):
+            # (outside training FactorVAE only evaluates: no backward pass, no update, losses.py:276-278)
+            self._average_grads()
+            self._optimizer_steps()
+        return loss
 
     def _train_iteration(self, data, storer):
         """training.py:137-164 (returns a Python float, i.e. synchronises; `storer` holds this step's scalars)."""
@@ -287,51 +299,20 @@ class Trainer():
         if self._loss_log is not None:
             self._loss_log.flush()
 
-    # -- data parallel ---------------------------------------------------------------------
-    def _sync_grads(self):
-        if not is_distributed():
-            return
-        if self._grad_sync is None:
-            self._grad_sync = FlatGradSync(list(self.model.parameters()))
-        self._grad_sync.sync()
-
-    def _factor_step_distributed(self, data, storer):
-        """FactorVAE step with the optimizer updates deferred until gradients are averaged."""
-        loss = self._factor_grads_distributed(data, storer)
-        self._optimizer_step()
-        self.loss_f._step_d()
-        return loss
-
-    def _factor_grads_distributed(self, data, storer, **inject):
-        """Both backward passes of losses.py:243-313 on this rank's shard, then the rank-average of the VAE and the
-        discriminator gradients (two flat all-reduces); no optimizer steps."""
-        lf = self.loss_f
-        if self._grad_sync_d is None:
-            from disvae.parallel import broadcast_parameters
-            broadcast_parameters(lf.discriminator)                # replicas must start from identical discriminators
-            self._grad_sync_d = FlatGradSync(list(lf.discriminator.parameters()))
-        loss = lf.call_optimize(data, self.model, self.optimizer, storer, step_optimizers=False, **inject)
-        self._sync_grads()
-        self._grad_sync_d.sync()
-        return loss
-
     def _grads_only(self, data, storer=None, **inject):
         """Forward + loss + backward (+ the data-parallel gradient average) of one batch WITHOUT an optimizer step:
         afterwards every `p.grad` (and, for FactorVAE, the discriminator's) holds exactly what the optimizers would
         consume.  Used by the parity checks (bench.py `parity` / `ddp_parity`, tests); `inject` forwards
         eps1/eps2/perms to FactorKLoss.call_optimize."""
-        data = data.to(self.device, non_blocking=True)
-        lf = self.loss_f
-        if hasattr(lf, "call_optimize"):
-            if is_distributed():
-                return self._factor_grads_distributed(data, storer, **inject).detach()
-            return lf.call_optimize(data, self.model, self.optimizer, storer, step_optimizers=False, **inject).detach()
-        recon_batch, latent_dist, latent_sample = self.model(data)
-        loss = lf(data, recon_batch, latent_dist, self.model.training, storer, latent_sample=latent_sample)
-        self.optimizer.zero_grad()
-        loss.backward()
-        self._sync_grads()
-        return loss.detach()
+        loss = self._forward_backward(self._device_batch(data), storer, **inject)
+        self._average_grads()
+        return loss
+
+
+# One captured training step (Trainer._graphs): the graph, its input buffer and loss, the native kernels one replay runs,
+# under data parallelism the flat all-reduce buffers (flat, static grads, params, views of flat), and the FusedAdams
+# whose steps the graph holds.
+_Graph = namedtuple("_Graph", "graph static_x static_loss n_kernels reduce adams")
 
 
 class _EpochTally:
@@ -358,8 +339,9 @@ class _EpochTally:
     def close(self):
         """-> the mean loss of the epoch's batches (synchronises)."""
         self.bar.close()
-        if self.tr._fused:
-            self.tr._fused.flush_state()                      # optimizer.state[p]["step"] follows the device counter
+        for fused in (self.tr._fused, getattr(self.tr.loss_f, "_fused_d", None)):
+            if fused:
+                fused.flush_state()                           # optimizer.state[p]["step"] follows the device counter
         self.tr._flush_loss_log()                             # this epoch's recorded scalars -> storer
         return self.loss.item() / self.n
 
@@ -442,20 +424,6 @@ class _HostLossRing:
             if self.events[k] is not None and self.events[k].query():
                 return float(self.host[k])
         return float("nan")
-
-
-class _StepProxy:
-    """What FactorKLoss.call_optimize sees as `optimizer`: zero_grad() of the real one, step() through
-    the Trainer's fused Adam."""
-
-    def __init__(self, optimizer, step_fn):
-        self._opt, self._step = optimizer, step_fn
-
-    def zero_grad(self, *a, **k):
-        return self._opt.zero_grad(*a, **k)
-
-    def step(self):
-        return self._step()
 
 
 class LossesLogger(object):

@@ -96,8 +96,7 @@ def main():
                                   for k, p in named.items())
 
     loss2 = mean_over_ranks(tr._grads_only(x, None, **inject).item())   # same gradients again ...
-    tr._optimizer_step()                                                 # ... and the two deferred optimizer steps
-    lf._step_d()
+    tr._optimizer_steps()                                                # ... and the two deferred optimizer steps
     rep["step_loss_rel"] = abs(loss2 - o_loss) / abs(o_loss)
     m_err = v_err = 0.0
     for k, p in named.items():

@@ -7,7 +7,8 @@ scripts/gpu_multi.sh as
 
 With N visible GPUs every rank takes its own device over NCCL; with fewer GPUs than ranks (the single-GPU test box) all
 ranks share cuda:0 and the collectives run over gloo on CUDA tensors -- the host-side logic under test
-(FlatGradSync, Trainer._factor_grads_distributed, the graph path's flat gather + all-reduce + fused Adam) is the same.
+(FlatGradSync, the FactorVAE discriminator broadcast and gradient average of Trainer._forward_backward /
+_average_grads, the graph path's flat gather + all-reduce + fused Adam) is the same.
 
 Checked on every rank, verdict gathered on rank 0 (exit code 0/1, one "DDP_WORKER {json}" line):
   * rank r's loss == oracle loss on shard r                                   (1e-4)
@@ -157,8 +158,7 @@ def main():
         tr.use_cuda_graph = True
     else:
         loss2 = tr._grads_only(x, None, **inject).item()             # same gradients again ...
-        tr._optimizer_step()                                         # ... and the two deferred optimizer steps
-        lf._step_d()
+        tr._optimizer_steps()                                        # ... and the two deferred optimizer steps
     if glob:
         allv = [None] * world
         dist.all_gather_object(allv, loss2)

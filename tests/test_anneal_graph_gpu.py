@@ -110,7 +110,7 @@ def test_annealed_recording_steps_replay_bit_identical(loss_name, rec_dist, img,
     assert list(st_e.items()) == list(st_h.items())
     # every step after the two eager warm-up steps was a replay: the third step captured (its launches count once as
     # direct ones) and replayed; from the fourth on nothing launches directly and each step replays n_kernels
-    n_kernels = next(iter(tr_g._graphs.values()))[3]
+    n_kernels = next(iter(tr_g._graphs.values())).n_kernels
     assert n_kernels > 0
     # counts[k] is noted when batch k is drawn: the prefetcher draws one batch ahead, so after steps 0 .. k-2; the
     # last entry is noted after the epoch

@@ -474,6 +474,37 @@ def test_train_epoch_mean_identical_in_graph_and_eager_mode(tmp_path):
     assert steps_e == steps_g == 15.0                  # FusedAdam.flush_state at every epoch end (ADVICE r1)
 
 
+def test_factor_discriminator_adam_step_count_at_epoch_end(tmp_path):
+    """FactorVAE: at every epoch end optimizer_d.state[p]["step"] counts the discriminator's Adam steps, as torch's Adam
+    would report them -- after eager steps and after graph replays alike (its FusedAdam's counter is flushed too)."""
+    import disvae
+    from disvae.models.losses import get_loss_f
+
+    def run(use_graph):
+        torch.manual_seed(SEED)
+        m = disvae.init_specific_model("Burgess", (1, 32, 32), 10)
+        opt = torch.optim.Adam(m.parameters(), lr=5e-4)
+        lf = get_loss_f("factor", rec_dist="bernoulli", reg_anneal=0, factor_G=6.4, latent_dim=10, lr_disc=1e-4,
+                        device=torch.device(DEV))
+        tr = disvae.Trainer(m, opt, lf, device=torch.device(DEV), logger=logging.getLogger("t"), save_dir=str(tmp_path),
+                            is_progress_bar=False)
+        tr.use_cuda_graph = use_graph
+        m.train()
+        g = torch.Generator().manual_seed(5)
+        loader = [(torch.rand(64, 1, 32, 32, generator=g), None) for _ in range(5)]
+        counts = []
+        for e in range(2):
+            tr._train_epoch(loader, None, e)
+            counts.append(({float(opt.state[p]["step"]) for p in m.parameters()},
+                           {float(lf.optimizer_d.state[p]["step"]) for p in lf.discriminator.parameters()}))
+        return counts, tr
+
+    counts_e, _ = run(False)
+    counts_g, tr_g = run(True)
+    assert len(tr_g._graphs) == 1, "graph path was not taken"
+    assert counts_e == counts_g == [({5.0}, {5.0}), ({10.0}, {10.0})]
+
+
 def test_uint8_batches_train_like_float_batches(tmp_path):
     """SURVEY.md 8f-3: a uint8 host batch (bytes over PCIe, /255 on the device by dv_u8_to_f32 -- in graph mode straight
     into the captured input buffer) walks exactly the trajectory of the same batch converted by ToTensor on the host."""

@@ -18,39 +18,34 @@ def rank_salt():
     return (dist.get_rank() * 0xD1342543DE82EF95) & 0xFFFFFFFFFFFFFFFF
 
 
-class FlatGradSync:
-    """Packs the gradients of `params` into one contiguous buffer, all-reduces it (sum) and
-    scatters the mean back.  The buffer is allocated once; `.grad` tensors are re-pointed to
-    views of it so the copy-in happens only the first time."""
+class GradAverage:
+    """The rank average of the gradients of `params` (in order: the model's, then FactorVAE's discriminator's) through
+    one flat fp32 buffer.  A call gathers every `.grad` into the buffer (a missing one as zeros), all-reduces it (sum)
+    and re-points every `.grad` to its view; it returns 1/world, the scale that turns those sums into the mean."""
 
-    def __init__(self, params, group=None):
+    def __init__(self, params):
         self.params = [p for p in params if p.requires_grad]
-        self.group = group
-        self.numel = sum(p.numel() for p in self.params)
         p0 = self.params[0]
-        self.flat = torch.zeros(self.numel, dtype=p0.dtype, device=p0.device)
-        self.views = []
-        off = 0
+        self.flat = torch.zeros(sum(p.numel() for p in self.params), dtype=torch.float32, device=p0.device)
+        self.views, off = [], 0
         for p in self.params:
             self.views.append(self.flat[off:off + p.numel()].view_as(p))
             off += p.numel()
 
-    def world_size(self):
-        return dist.get_world_size(self.group) if is_distributed() else 1
-
-    def sync(self):
-        """Average gradients over ranks in place.  No-op for world_size 1."""
-        ws = self.world_size()
-        if ws == 1:
-            return
+    def __call__(self):
+        grads = [p.grad for p in self.params]
+        if all(g is not None and g.data_ptr() != v.data_ptr() for g, v in zip(grads, self.views)):
+            torch.cat([g.reshape(-1) for g in grads], out=self.flat)       # one kernel
+        else:                                   # some gradient missing, or already in the buffer (accumulated into it)
+            for g, v in zip(grads, self.views):
+                if g is None:
+                    v.zero_()
+                elif g.data_ptr() != v.data_ptr():
+                    v.copy_(g)
+        dist.all_reduce(self.flat, op=dist.ReduceOp.SUM)
         for p, v in zip(self.params, self.views):
-            if p.grad is None:
-                v.zero_()
-            elif p.grad.data_ptr() != v.data_ptr():
-                v.copy_(p.grad)
-                p.grad = v
-        dist.all_reduce(self.flat, op=dist.ReduceOp.SUM, group=self.group)
-        self.flat.mul_(1.0 / ws)
+            p.grad = v
+        return 1.0 / dist.get_world_size()
 
 
 def shard_batch(data, rank=None, world_size=None):

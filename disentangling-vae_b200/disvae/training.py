@@ -18,7 +18,7 @@ from tqdm import trange
 from disvae import _native
 from disvae.fused import FusedAdam
 from disvae.models.losses import DeviceLossLog
-from disvae.parallel import FlatGradSync, broadcast_parameters, is_distributed
+from disvae.parallel import GradAverage, broadcast_parameters, is_distributed
 from disvae.utils.modelIO import save_model
 
 TRAIN_LOSSES_LOGFILE = "train_losses.log"
@@ -40,8 +40,7 @@ class Trainer():
         self.losses_logger = LossesLogger(os.path.join(self.save_dir, TRAIN_LOSSES_LOGFILE))
         self.gif_visualizer = gif_visualizer
         self.sync_every = 50                      # progress-bar refresh (host sync) period
-        self._grad_sync = None
-        self._grad_sync_d = None
+        self._grad_avg = None                     # GradAverage of the data-parallel steps (`_setup_data_parallel`)
         self._fused = None                        # FusedAdam over `optimizer` (built lazily on the device)
         self.use_cuda_graph = os.environ.get("DISVAE_CUDA_GRAPH", "1") != "0"
         # DISVAE_DEVICE_DATA=1: a torch DataLoader passed to __call__ is replaced by a disvae.data.DeviceLoader over its
@@ -124,15 +123,24 @@ class Trainer():
             with torch.no_grad():
                 self.model(x)
 
+    def _setup_data_parallel(self):
+        """Once, before the first data-parallel forward pass: FactorVAE's discriminator is broadcast from rank 0
+        (replicas must start from identical discriminators) and the GradAverage of the model's and the discriminator's
+        parameters is built."""
+        if self._grad_avg is not None or not is_distributed():
+            return
+        params = list(self.model.parameters())
+        if hasattr(self.loss_f, "call_optimize"):
+            broadcast_parameters(self.loss_f.discriminator)
+            params += list(self.loss_f.discriminator.parameters())
+        self._grad_avg = GradAverage(params)
+
     def _forward_backward(self, x, storer, **inject):
         """Forward pass, loss and backward pass of the fp32 device batch `x`; returns the detached loss.  Afterwards
         every `p.grad` (FactorVAE: the discriminator's too) holds this process's gradient.  `inject` forwards
         eps1/eps2/perms to FactorKLoss.call_optimize."""
+        self._setup_data_parallel()
         if hasattr(self.loss_f, "call_optimize"):             # several optimizers (training.py:160-162): both backward passes
-            disc = self.loss_f.discriminator
-            if is_distributed() and self._grad_sync_d is None:
-                broadcast_parameters(disc)                    # replicas must start from identical discriminators
-                self._grad_sync_d = FlatGradSync(list(disc.parameters()))
             loss = self.loss_f.call_optimize(x, self.model, self.optimizer, storer, step_optimizers=False, **inject)
         else:
             recon_batch, latent_dist, latent_sample = self.model(x)
@@ -142,15 +150,9 @@ class Trainer():
         return loss.detach()
 
     def _average_grads(self):
-        """Data parallel: the rank-average of the model's and the discriminator's gradients, in place (one flat
-        all-reduce each).  No-op in one process."""
-        if not is_distributed():
-            return
-        if self._grad_sync is None:
-            self._grad_sync = FlatGradSync(list(self.model.parameters()))
-        self._grad_sync.sync()
-        if self._grad_sync_d is not None:
-            self._grad_sync_d.sync()
+        """-> the scale the optimizers apply to the gradients: 1.0 in one process.  Data parallel: every `p.grad` of
+        the model and the discriminator becomes the sum over ranks (one flat all-reduce) and the scale is 1/world."""
+        return self._grad_avg() if is_distributed() else 1.0
 
     def _optimizers(self):
         """(optimizer, its FusedAdam or False) of each network a step updates: the model and, for FactorVAE, the
@@ -162,13 +164,19 @@ class Trainer():
         return pairs
 
     def _optimizer_steps(self, grad_scale=1.0):
-        """The Adam step of each network: dv_adam_multi on the gradients times `grad_scale` when FusedAdam takes the
-        optimizer over (a plain torch.optim.Adam on CUDA parameters), else the optimizer's own step()."""
+        """The Adam step of each network on its gradients times `grad_scale`: dv_adam_multi when FusedAdam takes the
+        optimizer over (a plain torch.optim.Adam on CUDA parameters), else the optimizer's own step() after scaling its
+        gradients in place."""
         for opt, fused in self._optimizers():
             if fused:
                 fused.step(grad_scale)
-            else:
-                opt.step()
+                continue
+            if grad_scale != 1.0:
+                for group in opt.param_groups:
+                    for p in group["params"]:
+                        if p.grad is not None:
+                            p.grad.mul_(grad_scale)
+            opt.step()
 
     # -- whole-step CUDA graph ------------------------------------------------------------------
     def _graph_eligible(self, data):
@@ -182,8 +190,6 @@ class Trainer():
             # parallelism the graph ends after the second backward pass (gradient average + both Adam steps follow it)
             if getattr(lf, "_perm_queue", None):
                 return False
-            if is_distributed() and self._grad_sync_d is None:
-                return False                                  # the discriminators are broadcast by the first eager step
             if not FusedAdam.lazy(lf, "_fused_d", lf.optimizer_d):
                 return False
         if getattr(lf, "global_batch", False) and is_distributed():
@@ -215,26 +221,15 @@ class Trainer():
         lf.n_train_steps, lf._step_dev_host = counters[:2]
         for f, n in zip(adams, counters[2]):
             f.host_steps = n
-        reduce = None
-        if ddp:
-            params = [p for p in self.model.parameters() if p.grad is not None]
-            if hasattr(lf, "call_optimize"):                  # one flat buffer (one all-reduce) for both networks
-                params += [p for p in lf.discriminator.parameters() if p.grad is not None]
-            static_grads = [p.grad.view(-1) for p in params]  # written by every replay
-            flat = torch.zeros(sum(t.numel() for t in static_grads), dtype=torch.float32, device=self.device)
-            off, views = 0, []
-            for p in params:                                  # Adam reads the all-reduced flat views
-                views.append(flat[off:off + p.numel()].view_as(p))
-                off += p.numel()
-            reduce = (flat, static_grads, params, views)
-        return _Graph(g, static_x, static_loss, n_kernels, reduce, () if ddp else tuple(adams))
+        grads = tuple(p.grad for p in self._grad_avg.params) if ddp else None   # written by every replay
+        return _Graph(g, static_x, static_loss, n_kernels, grads, () if ddp else tuple(adams))
 
     def _graph_step(self, data, storer):
         """fwd + loss + bwd (+ Adam when not data-parallel) of one batch as ONE CUDA graph launch (static
-        shapes).  Data-parallel: the graph ends after the backward pass; its static gradient tensors are
-        gathered into the flat buffer (one kernel), all-reduced (one NCCL call) and consumed by the fused
-        Adam launch with grad_scale = 1/world.  The loss's device step counter advances inside the graph (annealing
-        coefficients, the device loss log of recording steps); the host counters follow here."""
+        shapes).  Data-parallel: the graph ends after the backward pass; `.grad` is bound to its static gradient
+        tensors, then the gradient average and the Adam steps follow as in an eager step.  The loss's device step
+        counter advances inside the graph (annealing coefficients, the device loss log of recording steps); the host
+        counters follow here."""
         key = (tuple(data.shape), str(data.dtype))
         entry = self._graphs.get(key)
         if entry is None:
@@ -247,14 +242,10 @@ class Trainer():
             self._loss_log.expect(lf.n_train_steps + 1, lf.record_loss_every, storer)   # before the replay writes its row
         entry.graph.replay()
         _native.GRAPH_LAUNCHES += entry.n_kernels
-        if entry.reduce is not None:
-            import torch.distributed as dist
-            flat, static_grads, params, views = entry.reduce
-            torch.cat(static_grads, out=flat)
-            dist.all_reduce(flat, op=dist.ReduceOp.SUM)
-            for p, v in zip(params, views):                   # (an eager step in between re-binds .grad)
-                p.grad = v
-            self._optimizer_steps(grad_scale=1.0 / dist.get_world_size())
+        if entry.grads is not None:
+            for p, grad in zip(self._grad_avg.params, entry.grads):
+                p.grad = grad
+            self._optimizer_steps(self._average_grads())
         lf.n_train_steps += 1                                 # the replay's work on the host counters
         lf._step_dev_host += 1
         for f in entry.adams:
@@ -285,8 +276,7 @@ class Trainer():
         loss = self._forward_backward(x, storer)
         if self.model.training or not hasattr(self.loss_f, "call_optimize"):
             # (outside training FactorVAE only evaluates: no backward pass, no update, losses.py:276-278)
-            self._average_grads()
-            self._optimizer_steps()
+            self._optimizer_steps(self._average_grads())
         return loss
 
     def _train_iteration(self, data, storer):
@@ -301,18 +291,20 @@ class Trainer():
 
     def _grads_only(self, data, storer=None, **inject):
         """Forward + loss + backward (+ the data-parallel gradient average) of one batch WITHOUT an optimizer step:
-        afterwards every `p.grad` (and, for FactorVAE, the discriminator's) holds exactly what the optimizers would
-        consume.  Used by the parity checks (bench.py `parity` / `ddp_parity`, tests); `inject` forwards
-        eps1/eps2/perms to FactorKLoss.call_optimize."""
+        afterwards every `p.grad` (and, for FactorVAE, the discriminator's) holds the rank mean, which
+        `_optimizer_steps()` consumes as it is.  Used by the parity checks (bench.py `parity` / `ddp_parity`, tests);
+        `inject` forwards eps1/eps2/perms to FactorKLoss.call_optimize."""
         loss = self._forward_backward(self._device_batch(data), storer, **inject)
-        self._average_grads()
+        scale = self._average_grads()
+        if scale != 1.0:
+            self._grad_avg.flat.mul_(scale)
         return loss
 
 
 # One captured training step (Trainer._graphs): the graph, its input buffer and loss, the native kernels one replay runs,
-# under data parallelism the flat all-reduce buffers (flat, static grads, params, views of flat), and the FusedAdams
-# whose steps the graph holds.
-_Graph = namedtuple("_Graph", "graph static_x static_loss n_kernels reduce adams")
+# under data parallelism the static gradient tensors the replay writes (in GradAverage order; None otherwise), and the
+# FusedAdams whose steps the graph holds.
+_Graph = namedtuple("_Graph", "graph static_x static_loss n_kernels grads adams")
 
 
 class _EpochTally:

@@ -6,9 +6,9 @@ scripts/gpu_multi.sh as
         --loss btcvae|factor|betaH [--per 32] [--z 10]
 
 With N visible GPUs every rank takes its own device over NCCL; with fewer GPUs than ranks (the single-GPU test box) all
-ranks share cuda:0 and the collectives run over gloo on CUDA tensors -- the host-side logic under test
-(FlatGradSync, the FactorVAE discriminator broadcast and gradient average of Trainer._forward_backward /
-_average_grads, the graph path's flat gather + all-reduce + fused Adam) is the same.
+ranks share cuda:0 and the collectives run over gloo on CUDA tensors -- the host-side logic under test (the FactorVAE
+discriminator broadcast, and the one gradient average, `GradAverage` via Trainer._average_grads, that eager and replayed
+steps share before the fused Adam takes the 1/world scale) is the same.
 
 Checked on every rank, verdict gathered on rank 0 (exit code 0/1, one "DDP_WORKER {json}" line):
   * rank r's loss == oracle loss on shard r                                   (1e-4)
@@ -17,6 +17,10 @@ Checked on every rank, verdict gathered on rank 0 (exit code 0/1, one "DDP_WORKE
   * after one real optimisation step: Adam's exp_avg == (1-beta1) * that mean gradient, exp_avg_sq == (1-beta2) * its
     square (linear / quadratic in the gradient -- unlike the parameters, which move by +-lr whatever the gradient is)
   * replicas stay bit-identical over further steps (device noise, CUDA-graph path where eligible), loss decreases
+  * every one of those steps, eager or replayed, FactorVAE included, makes exactly one all-reduce of the gradient
+    buffer (other all-reduces, e.g. the global-batch estimator's, are not counted)
+  * after the first (eager) step and after the last one, every `p.grad` (FactorVAE: the discriminator's too) lies in
+    that one buffer
 """
 import argparse
 import json
@@ -179,10 +183,29 @@ def main():
     torch.manual_seed(99)
     first = last = None
     xb = x.to(dev)
+    buf = tr._grad_avg.flat                            # the gradient buffer (built by the first _grads_only)
+    all_reduce, n_grad_reduce = dist.all_reduce, [0]
+
+    def counting_all_reduce(t, *a, **k):
+        if t is buf:
+            n_grad_reduce[0] += 1
+        return all_reduce(t, *a, **k)
+
+    def grads_in_one_buffer():
+        return {p.grad.untyped_storage().data_ptr() for p in named.values()} == {buf.untyped_storage().data_ptr()}
+
+    dist.all_reduce, counts = counting_all_reduce, []
     for it in range(args.steps):
+        n_grad_reduce[0] = 0
         v = tr._step(xb, None).item()
+        counts.append(n_grad_reduce[0])
+        if it == 0:
+            rep["grads_in_one_buffer_eager"] = grads_in_one_buffer()
         first = v if first is None else first
         last = v
+    dist.all_reduce = all_reduce
+    rep["grads_in_one_buffer_last"] = grads_in_one_buffer()
+    rep["grad_allreduces_per_step"] = counts             # steps 1-2 eager, then replays on the graph path
     flat = torch.cat([p.detach().flatten() for p in named.values()])
     if shared:
         flat = flat.cpu()                                            # gloo has no CUDA all_gather
@@ -197,7 +220,8 @@ def main():
     # occasional ReLU unit that two fp32 evaluation orders round to opposite sides of zero (oracle/same_branch.py).
     ok = (rep["loss_rel"] < 1e-4 and rep["step_loss_rel"] < 1e-4 and rep["avg_grad_rel_err"] < 3e-3
           and rep["exp_avg_rel_err"] < 3e-3 and rep["exp_avg_sq_rel_err"] < 6e-3 and rep["in_sync"] and last < first
-          and (glob or rep["graph_path"] or dev.type != "cuda"))
+          and (glob or rep["graph_path"] or dev.type != "cuda") and counts == [1] * args.steps
+          and rep["grads_in_one_buffer_eager"] and rep["grads_in_one_buffer_last"])
     rep["ok"] = bool(ok)
     reps = [None] * world
     dist.all_gather_object(reps, rep)

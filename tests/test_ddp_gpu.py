@@ -1,8 +1,8 @@
 """Data-parallel parity as pytest (SURVEY.md 8e): two ranks (NCCL on two GPUs, or gloo over CUDA tensors when the box has
 one) run tests/ddp_worker.py -- rank-r loss vs the oracle on shard r, rank-averaged gradients vs the mean of the oracle's
-shard gradients, Adam moments after a real step, replicas bit-identical afterwards.  Covers the eager FactorVAE
-gradient average of Trainer._forward_backward / _average_grads (BASELINE configs[3]) and the graph path's flat
-gather/all-reduce (configs[1], [4])."""
+shard gradients, Adam moments after a real step, replicas bit-identical afterwards, and one all-reduce of one gradient
+buffer per step.  Covers the gradient average (Trainer._average_grads) that eager steps (FactorVAE: BASELINE
+configs[3]) and graph replays (configs[1], [4]) share."""
 import json
 import os
 import socket

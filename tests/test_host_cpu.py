@@ -192,39 +192,61 @@ def test_ctypes_signatures_match_the_header_prototypes():
             assert ("*" in decl) == (ctype is ctypes.c_void_p), (name, decl.strip())
 
 
-def _ddp_worker(rank, world, port, out):
+def _grad_average_worker(rank, world, port, out):
     import torch.distributed as dist
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
-    from disvae.parallel import FlatGradSync, broadcast_parameters, shard_batch
+    from disvae.parallel import GradAverage, broadcast_parameters, shard_batch
     torch.manual_seed(rank)                                   # different init per rank on purpose
     m = disvae.init_specific_model("Burgess", (1, 32, 32), 10)
+    disc = torch.nn.Sequential(torch.nn.Linear(10, 16), torch.nn.ReLU(), torch.nn.Linear(16, 2))   # FactorVAE's role
     broadcast_parameters(m)
     ref = torch.cat([p.detach().flatten() for p in m.parameters()])
     gathered = [torch.empty_like(ref) for _ in range(world)]
     dist.all_gather(gathered, ref)
     same = all(torch.equal(gathered[0], g) for g in gathered)
-    for i, p in enumerate(m.parameters()):
-        p.grad = torch.full_like(p, float(rank + 1) * (i + 1))
-    sync = FlatGradSync(list(m.parameters()))
-    sync.sync()
-    expect = sum(range(1, world + 1)) / world
-    ok = all(torch.allclose(p.grad, torch.full_like(p, expect * (i + 1))) for i, p in enumerate(m.parameters()))
-    views = all(p.grad.data_ptr() == v.data_ptr() for p, v in zip(sync.params, sync.views))
+    params = list(m.parameters()) + list(disc.parameters())
+    avg = GradAverage(params)
+    n_reduce = [0]
+    all_reduce = dist.all_reduce
+
+    def counting_all_reduce(*a, **k):
+        n_reduce[0] += 1
+        return all_reduce(*a, **k)
+
+    dist.all_reduce = counting_all_reduce
+    mean = sum(range(1, world + 1)) / world
+    ok, views, scales = [], [], []
+    for call in (1, 2, 3):
+        for p in params:
+            p.grad = None                                     # as zero_grad() leaves them between steps
+        # calls 1, 2: every gradient present (one gather into the buffer); call 3: the last one missing (zeros)
+        present = params[:-1] if call == 3 else params
+        for i, p in enumerate(present):
+            p.grad = torch.full_like(p, float(rank + 1) * (i + 1) * call)
+        want = [mean * (i + 1) * call if i < len(present) else 0.0 for i in range(len(params))]
+        scales.append(avg())
+        ok.append(all(torch.allclose(p.grad * scales[-1], torch.full_like(p, w)) for p, w in zip(params, want)))
+        views.append(all(p.grad.data_ptr() == v.data_ptr() for p, v in zip(params, avg.views)))
+    dist.all_reduce = all_reduce
     x = torch.arange(8).view(8, 1)
     shard = shard_batch(x)
     ok_shard = shard.flatten().tolist() == list(range(rank * 4, rank * 4 + 4))
     if rank == 0:
-        torch.save(dict(same=same, ok=ok, views=views, ok_shard=ok_shard), out)
+        torch.save(dict(same=same, ok=ok, views=views, scales=scales, n_reduce=n_reduce[0], ok_shard=ok_shard), out)
     dist.destroy_process_group()
 
 
-def test_flat_grad_allreduce_world2_gloo(tmp_path):
+def test_grad_average_world2_gloo(tmp_path):
+    """GradAverage over two ranks: the model and a second network (FactorVAE's discriminator) share ONE all-reduce per
+    average; `.grad` becomes the rank sum in views of the buffer, and the returned 1/world scales it to the mean;
+    averages after `.grad = None` gather the new gradients, a missing one as zeros.  Also the parameter broadcast and
+    `shard_batch`."""
     import torch.multiprocessing as mp
     out = str(tmp_path / "r.pt")
-    mp.spawn(_ddp_worker, args=(2, 29561, out), nprocs=2, join=True)
+    mp.spawn(_grad_average_worker, args=(2, 29561, out), nprocs=2, join=True)
     r = torch.load(out)
-    assert r == dict(same=True, ok=True, views=True, ok_shard=True)
+    assert r == dict(same=True, ok=[True] * 3, views=[True] * 3, scales=[0.5] * 3, n_reduce=3, ok_shard=True)
 
 
 def test_bench_reference_arm_contract():

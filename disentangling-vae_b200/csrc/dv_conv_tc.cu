@@ -8,9 +8,11 @@
 //     MMAs below are free of bank conflicts.
 //   * fp32 parity on tf32 tensor cores: error-compensated 3xTF32 (dv_ptx.cuh).  The operands are split into hi/lo planes
 //     in registers right after their fragment loads; the packed weights already hold both planes.
-//   * warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 load fragments, issue mma.sync m16n8k8 and run
-//     the epilogue; warp 8 is the TMA producer.  mbarrier rings between them: raw-full (TMA transaction count) and
-//     raw-empty (one arrival per consumer warp).
+//   * warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 load fragments, run the MMAs and the
+//     epilogue; warp 8 is the TMA producer.  mbarrier rings between them: raw-full (TMA transaction count) and
+//     raw-empty (one arrival per consumer warp).  down and up: warps 0-3 and 4-7 are two warpgroups of 64 MMA rows
+//     issuing wgmma with A from registers and B (the resident packed weights) from shared memory; wgrad: each warp
+//     issues mma.sync m16n8k8.
 #include "dv_common.cuh"
 #include "dv_ptx.cuh"
 
@@ -28,16 +30,46 @@ constexpr int kSmemMax = 232448;             // 227 KB per block on sm_90
 
 __device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers * 32) : "memory"); }
 
-// The B fragments (hi and lo planes) of k slice ks for output columns nt*8 + g, from a packed-weight tap:
-// 64 rows x 128 B, rows [0,32) hi and [32,64) lo of the N-by-K (K contiguous) weight.  ONE ldmatrix .x4 instead of four
-// 32-bit loads: matrices {hi, k 0-3}, {hi, k 4-7}, {lo, k 0-3}, {lo, k 4-7} of the 8 columns; lane l gives the address
-// of row b_row = (l >> 4) * 32 + (l & 7) (+ 8 nt), column b_col = ((l >> 3) & 1) * 4 (b_lane_row / b_lane_col).
-__device__ __forceinline__ int b_lane_row(int lane) { return (lane >> 4) * 32 + (lane & 7); }
-__device__ __forceinline__ int b_lane_col(int lane) { return (lane & 8) >> 1; }
-__device__ __forceinline__ void load_b_tap(uint32_t tap_base, int nt, int ks, int b_row, int b_col, uint32_t (&bh)[2], uint32_t (&bl)[2]) {
-  uint32_t r[4];
-  ldsm_x4(tap_base + swz128(b_row + 8 * nt, 8 * ks + b_col), r);
-  bh[0] = r[0]; bh[1] = r[1]; bl[0] = r[2]; bl[1] = r[3];
+// Once a product's commit groups are complete: its hi*hi is added to the fp32 total.  tot[4 nt + e] (like every
+// accumulator here) is element e of n-tile nt in the m16n8 accumulator layout.
+__device__ __forceinline__ void fold_tap(float (&tot)[16], float (&acc)[16]) {
+  fence_regs(acc);
+#pragma unroll
+  for (int i = 0; i < 16; ++i) tot[i] += acc[i];
+}
+
+// 3xTF32 of one (activation tile, weight tap) product, K = 32 channels, on the warpgroup's tensor cores.
+// A: rows p0 and p1 (this thread's MMA rows g and g + 8) of a swizzled [pixel][32 ch] tile at a_base, AND-ed with
+// keep0 / keep1 (0 zeroes a row), split into hi and lo planes in registers.  B: the packed tap at tap_base,
+// [32 hi | 32 lo rows][32 K].  Per k8: acc = A_hi.W_hi (overwritten by the first slice), corr += A_hi.W_lo + A_lo.W_hi
+// (overwritten first when corr_accumulate == 0): the summation of the mma.sync kernels, where the correction products
+// run across taps and hi*hi is folded into an fp32 total per tap.  (One m64n64k8 against [W_hi | W_lo] would issue the
+// same work, but its 32 accumulators per thread, double-buffered, do not fit the 168 registers a 288-thread wgmma kernel
+// gets: ptxas allocates whole warpgroups.)
+// Every k8 slice is its own commit group, and the previous product (accumulating into acc_prev) is still in flight:
+// before slice ks is loaded into ah/al[4 ks, 4 ks + 4), wait_group 3 completes slice ks of the previous product (the
+// last reader of those registers), and before the last slice it completes the whole previous product, which is then
+// folded.  So one register set of A fragments serves both products, and the fold runs beside this product's MMAs.
+__device__ __forceinline__ void product(float (&acc)[16], float (&acc_prev)[16], float (&corr)[16], float (&tot)[16],
+                                        uint32_t (&ah)[16], uint32_t (&al)[16], uint32_t a_base, int p0, int p1,
+                                        uint32_t keep0, uint32_t keep1, int t, uint32_t tap_base, int corr_accumulate) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    wgmma_wait<3>();
+    if (ks == 3) fold_tap(tot, acc_prev);
+    split_tf32(lds32(a_base + swz128(p0, 8 * ks + t)) & keep0, ah[4 * ks + 0], al[4 * ks + 0]);
+    split_tf32(lds32(a_base + swz128(p1, 8 * ks + t)) & keep1, ah[4 * ks + 1], al[4 * ks + 1]);
+    split_tf32(lds32(a_base + swz128(p0, 8 * ks + t + 4)) & keep0, ah[4 * ks + 2], al[4 * ks + 2]);
+    split_tf32(lds32(a_base + swz128(p1, 8 * ks + t + 4)) & keep1, ah[4 * ks + 3], al[4 * ks + 3]);
+    fence_regs(acc);
+    fence_regs(corr);
+    wgmma_fence();
+    const uint64_t w_hi = wgmma_desc_k128(tap_base + 32 * ks), w_lo = wgmma_desc_k128(tap_base + 32 * 128 + 32 * ks);
+    wgmma_m64n32k8_rs(acc, ah + 4 * ks, w_hi, ks);
+    wgmma_m64n32k8_rs(corr, ah + 4 * ks, w_lo, ks | corr_accumulate);
+    wgmma_m64n32k8_rs(corr, al + 4 * ks, w_hi, 1);
+    wgmma_commit();
+  }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -108,42 +140,33 @@ conv_down32_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   }
 
   const int gq = lane >> 2, t = lane & 3;
-  const int b_row = b_lane_row(lane), b_col = b_lane_col(lane);
   const int r0 = warp * 16 + gq;                             // this thread's tile rows: r0 and r0 + 8
   const uint32_t bs = smem_u32(Bs), raw0 = smem_u32(Raw);
   float csum[4][2] = {};                                     // channel sums of the stored output (colsum_part)
   mbar_wait(&bars->b_full, 0);
   int stage = 0; uint32_t phase = 0;
+  uint32_t ah[16], al[16];
+  // tap `tap` of the ring's current tile into acc while the previous tap (acc_prev) completes; the stage is free again
+  // once its fragments are in registers
+  auto tap_product = [&](float (&acc)[16], float (&acc_prev)[16], float (&corr)[16], float (&tot)[16], int tap) {
+    mbar_wait(&bars->raw_full[stage], phase);
+    product(acc, acc_prev, corr, tot, ah, al, raw0 + stage * kATile, r0, r0 + 8, ~0u, ~0u, t, bs + tap * kBTap, tap);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars->raw_empty[stage]);
+    if (++stage == kDownStages) { stage = 0; phase ^= 1; }
+  };
   for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-    float tot[4][4] = {}, corr[4][4] = {};
-    for (int tap = 0; tap < kTaps; ++tap) {
-      mbar_wait(&bars->raw_full[stage], phase);
-      const uint32_t a_base = raw0 + stage * kATile, b_base = bs + tap * kBTap;
-      float mn[4][4] = {};                                   // hi*hi of this tap, added to tot in fp32 below
+    float tot[16] = {}, corr[16], acc[2][16];
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        uint32_t a[4], ah[4], al[4];
-        a[0] = lds32(a_base + swz128(r0, 8 * ks + t));
-        a[1] = lds32(a_base + swz128(r0 + 8, 8 * ks + t));
-        a[2] = lds32(a_base + swz128(r0, 8 * ks + t + 4));
-        a[3] = lds32(a_base + swz128(r0 + 8, 8 * ks + t + 4));
-#pragma unroll
-        for (int e = 0; e < 4; ++e) split_tf32(a[e], ah[e], al[e]);
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-          uint32_t bh[2], bl[2];
-          load_b_tap(b_base, nt, ks, b_row, b_col, bh, bl);
-          mma_3xtf32(mn[nt], corr[nt], ah, al, bh, bl);
-        }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->raw_empty[stage]);
-      if (++stage == kDownStages) { stage = 0; phase ^= 1; }
-#pragma unroll
-      for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) tot[nt][e] += mn[nt][e];
+    for (int i = 0; i < 16; ++i) acc[1][i] = 0.f;           // folded while tap 0 runs
+#pragma unroll 1
+    for (int tap = 0; tap < kTaps; tap += 2) {
+      tap_product(acc[0], acc[1], corr, tot, tap);
+      tap_product(acc[1], acc[0], corr, tot, tap + 1);
     }
+    wgmma_wait<0>();
+    fold_tap(tot, acc[1]);
+    fence_regs(corr);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const long long p = (long long)tile * 128 + r0 + 8 * h;
@@ -158,7 +181,7 @@ conv_down32_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         float v[2];
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          float x = (tot[nt][2 * h + e] + corr[nt][2 * h + e]) + bars->bias[c + e];
+          float x = (tot[4 * nt + 2 * h + e] + corr[4 * nt + 2 * h + e]) + bars->bias[c + e];
           if (act == DV_ACT_RELU) x = fmaxf(x, 0.f);
           v[e] = ((mb >> (c + e)) & 1u) ? x : 0.f;
         }
@@ -409,7 +432,6 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
   }
 
   const int gq = lane >> 2, t = lane & 3;
-  const int b_row = b_lane_row(lane), b_col = b_lane_col(lane);
   const int HH = 2 * g.H, WW = 2 * g.W;
   const uint32_t bs = smem_u32(Bs), raw0 = smem_u32(Raw);
   // the two MMA rows of this thread (r = 16*warp + gq + 8h): centre pixel inside the resident box [TB][TR+2][W]
@@ -423,6 +445,7 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
     src0[h] = min((rtb * (g.TR + 2) + (rt - rtb * g.TR) + 1) * g.W + rj[h], g.box_px - 1);
     row_ok[h] = row < g.valid_rows;
   }
+  uint32_t ah[16], al[16];
   mbar_wait(&bars->b_full, 0);
   uint32_t t_seq = 0;
   for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x, ++t_seq) {
@@ -431,18 +454,19 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
     mbar_wait(&bars->raw_full[stage], (t_seq / kHaloStages) & 1u);
     int b0, i0;
     if (g.TB > 1) { b0 = tile * g.TB; i0 = 0; } else { b0 = tile / g.tiles_per_img; i0 = (tile % g.tiles_per_img) * g.TR; }
-    // one output phase (ph, pw) at a time: its four (shift, tap) products, hi*hi added to the fp32 total after every
-    // shift, the correction products in their own accumulator
+    // one output phase (ph, pw) at a time: its four (shift, tap) products, shift (di, dj) = (ph - 1 + (q >> 1),
+    // pw - 1 + (q & 1)) through tap (3 - ph - 2 (q >> 1), 3 - pw - 2 (q & 1)); hi*hi added to the fp32 total after
+    // every product, the correction products in their own total.
 #pragma unroll 1
     for (int pidx = 0; pidx < 4; ++pidx) {
       const int ph = pidx >> 1, pw = pidx & 1;
-      float tot[4][4] = {}, corr[4][4] = {};
+      float tot[16] = {}, corr[16], acc[2][16];
 #pragma unroll
-      for (int s = 0; s < 9; ++s) {
-        const int di = s / 3 - 1, dj = s % 3 - 1;
-        const int kh = ph + 1 - 2 * di, kw = pw + 1 - 2 * dj;
-        if (kh < 0 || kh > 3 || kw < 0 || kw > 3) continue;
-        const uint32_t b_base = bs + (kh * 4 + kw) * kBTap;
+      for (int i = 0; i < 16; ++i) acc[1][i] = 0.f;         // folded while product 0 runs
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int di = ph - 1 + (q >> 1), dj = pw - 1 + (q & 1);
+        const uint32_t b_base = bs + ((3 - ph - 2 * (q >> 1)) * 4 + 3 - pw - 2 * (q & 1)) * kBTap;
         int p[2];
         uint32_t keep[2];
 #pragma unroll
@@ -451,26 +475,11 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
           p[h] = ok ? src0[h] + di * g.W + dj : src0[h];
           keep[h] = ok ? 0xffffffffu : 0u;
         }
-        float mn[4][4] = {};
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          uint32_t ah[4], al[4];
-          split_tf32(lds32(a_base + swz128(p[0], 8 * ks + t)) & keep[0], ah[0], al[0]);
-          split_tf32(lds32(a_base + swz128(p[1], 8 * ks + t)) & keep[1], ah[1], al[1]);
-          split_tf32(lds32(a_base + swz128(p[0], 8 * ks + t + 4)) & keep[0], ah[2], al[2]);
-          split_tf32(lds32(a_base + swz128(p[1], 8 * ks + t + 4)) & keep[1], ah[3], al[3]);
-#pragma unroll
-          for (int nt = 0; nt < 4; ++nt) {
-            uint32_t bh[2], bl[2];
-            load_b_tap(b_base, nt, ks, b_row, b_col, bh, bl);
-            mma_3xtf32(mn[nt], corr[nt], ah, al, bh, bl);
-          }
-        }
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) tot[nt][e] += mn[nt][e];
+        product(acc[q & 1], acc[(q + 1) & 1], corr, tot, ah, al, a_base, p[0], p[1], keep[0], keep[1], t, b_base, q);
       }
+      wgmma_wait<0>();
+      fold_tap(tot, acc[1]);
+      fence_regs(corr);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = warp * 16 + gq + 8 * h, tr = r / g.W;
@@ -488,7 +497,7 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
           float v[2];
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            float x = (tot[nt][2 * h + e] + corr[nt][2 * h + e]) + bars->bias[c + e];
+            float x = (tot[4 * nt + 2 * h + e] + corr[4 * nt + 2 * h + e]) + bars->bias[c + e];
             if (act == DV_ACT_RELU) x = fmaxf(x, 0.f);
             v[e] = ((mb >> (c + e)) & 1u) ? x : 0.f;
           }

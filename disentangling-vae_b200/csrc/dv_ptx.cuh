@@ -1,6 +1,6 @@
 // Inline-PTX wrappers for the Hopper (sm_90a) async machinery the tensor-core kernels use: mbarrier, TMA
-// (cp.async.bulk.tensor) and the warp-level tf32 tensor-core MMA (mma.sync m16n8k8), and the host-side lookup of the
-// driver's tensor-map encoder.
+// (cp.async.bulk.tensor), the warp-level tf32 tensor-core MMA (mma.sync m16n8k8) and the warpgroup one (wgmma), and the
+// host-side lookup of the driver's tensor-map encoder.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -47,16 +47,6 @@ __device__ __forceinline__ uint32_t lds32(uint32_t smem_addr) {
   uint32_t v;
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(smem_addr) : "memory");
   return v;
-}
-
-// Four 8x8 b16 matrices (ldmatrix .x4): lane l gives the 16-byte row address of row l & 7 of matrix l >> 3, and
-// register j of lane l receives 32-bit word l & 3 of row l >> 2 of matrix j.  Read as 32-bit data, that is exactly the
-// tf32 m16n8k8 fragment layout: one instruction for a whole A fragment, or for the hi and lo B fragments of 8 columns.
-__device__ __forceinline__ void ldsm_x4(uint32_t smem_addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(smem_addr)
-               : "memory");
 }
 
 // Byte offset of fp32 element (row r, column c < 32) in a tile of 128-byte rows written by TMA with
@@ -138,6 +128,39 @@ __device__ __forceinline__ void mma_3xtf32(float (&main)[4], float (&corr)[4], c
   mma_tf32(main, a_hi, b_hi);
   mma_tf32(corr, a_hi, b_lo);
   mma_tf32(corr, a_lo, b_hi);
+}
+
+// ---- warpgroup tf32 MMA (wgmma), A from registers -------------------------------------------
+// Shared-memory descriptor of a K-major operand tile written by TMA with the 128-byte swizzle: rows of 128 B (32 fp32
+// of K), 8-row swizzle atoms 1024 B apart (stride byte offset), leading byte offset unused for a swizzled K-major tile.
+// The k8 slice ks of a tile starts 32*ks bytes into the tile (the hardware applies the swizzle to the full address).
+__device__ __forceinline__ uint64_t wgmma_desc_k128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Pins the order of register accesses around the asynchronous MMAs (the compiler does not know that the registers of
+// an issued wgmma change until its wait_group).
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+
+// D[64 x 32] (+)= A[64 x 8] * B[8 x 32], tf32 operands, fp32 accumulate, issued by a whole warpgroup.  A per warp
+// (rows 16*(warp%4) + ...) in the m16n8k8 layout of mma_tf32; D per warp in the m16n8 layout repeated along N:
+// d[4j + e] = D[g + 8(e>>1)][8j + 2t + (e&1)].  B: descriptor of the 32 x 8 K-major slice.  accumulate == 0 overwrites D.
+__device__ __forceinline__ void wgmma_m64n32k8_rs(float (&d)[16], const uint32_t* a, uint64_t b_desc, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
 }
 
 }  // namespace ptx

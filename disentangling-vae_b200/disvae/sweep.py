@@ -14,7 +14,8 @@ Member k's result is bit-identical to a lone `Trainer` run with the same setting
 Philox keys come from `seeds` (`philox_keys`) rather than from `torch.initial_seed()` at first use.
 
 Limits: one process, one GPU, the CUDA-graph path.  Members must not have taken a training step yet (call the same
-Sweep again to continue).  They must share the device and the input image shape, and
+Sweep again to continue, or, in a new process, give every member the training state it saved with `save_state=True`
+through `load_training_state`).  They must share the device and the input image shape, and
 their optimizers (and FactorVAE's discriminator optimizer) must be ones `FusedAdam` takes over.  Anything else raises
 `ValueError` before any GPU work.
 """
@@ -33,7 +34,7 @@ from disvae.fused import FusedAdam
 from disvae.models.losses import permutation_key
 from disvae.models.vae import noise_key
 from disvae.parallel import is_distributed
-from disvae.training import Trainer, _EpochTally
+from disvae.training import Trainer, _EpochTally, apply_loader_state, check_loader_state
 
 _tokens = itertools.count()          # ops.owner tokens: one per Trainer that ever joined a sweep
 
@@ -66,8 +67,9 @@ class Sweep:
             if not m.use_cuda_graph:
                 raise ValueError("Sweep: member %d has use_cuda_graph=False (DISVAE_CUDA_GRAPH=0); a sweep replays "
                                  "each member's captured CUDA graph and has no eager path" % k)
-            if m._graphs or m._eligible_steps or m.loss_f.n_train_steps:
+            if m._graphs or m._eligible_steps or m.loss_f.n_train_steps != m._steps_at_load:
                 # its graph would read scratch shared with every other Trainer, and its Philox keys are already fixed
+                # (a member that loaded a training state has taken no step in this process: it is accepted)
                 raise ValueError("Sweep: member %d has already taken training steps; a sweep starts from members that "
                                  "have not (call the same Sweep again to continue training)" % k)
         for what in ("model", "optimizer", "loss_f"):
@@ -126,14 +128,41 @@ class Sweep:
             entry = self._device_loaders[id(data_loader)] = (data_loader, device_loader_for(data_loader, self.device))
         return entry[1]
 
-    def __call__(self, data_loader, epochs=10, checkpoint_every=10):
+    def __call__(self, data_loader, epochs=10, checkpoint_every=10, save_state=False):
         """Train every member for `epochs` epochs over `data_loader` (a DeviceLoader, or a DataLoader converted to one
         once per Sweep), like `Trainer.__call__` for each.  Calling again continues as a lone Trainer called again
-        does: step counters, Adam state, Philox counters and the loader's epochs carry on."""
+        does: step counters, Adam state, Philox counters and the loader's epochs carry on.  `save_state=True` writes
+        each member's training state into its own save_dir; members that loaded one continue from it."""
+        first, loader_state = self._resume()
+        if loader_state is not None:
+            check_loader_state(loader_state, data_loader, device_data=True)
         loader = self._loader(data_loader)
+        for m in self.members:
+            m._resume = None
+        if loader_state is not None:
+            apply_loader_state(loader_state, loader)
         start = default_timer()
         with torch.cuda.device(self.device):
-            self._run(loader, epochs, checkpoint_every, start)
+            self._run(loader, first, epochs, checkpoint_every, save_state, start)
+
+    def _resume(self):
+        """(first epoch, saved loader state) of the members' loaded training states, (0, None) if none has one.
+        Members that loaded states must all have stopped at the same epoch of the same data order."""
+        pending = [m._resume for m in self.members]
+        if all(r is None for r in pending):
+            return 0, None
+        for k, r in enumerate(pending):
+            if r is None:
+                raise ValueError("Sweep: member %d has not loaded a training state but others have; resume every "
+                                 "member or none" % k)
+            epoch, loader = r
+            if loader is None or loader["kind"] != "device":
+                raise ValueError("Sweep: member %d's training state was not saved over a DeviceLoader; a sweep "
+                                 "continues only the data order of one" % k)
+            if epoch != pending[0][0] or loader != pending[0][1]:
+                raise ValueError("Sweep: member %d's training state (epoch %d, loader %r) is not where member 0's "
+                                 "(epoch %d, loader %r) stopped" % (k, epoch, loader, pending[0][0], pending[0][1]))
+        return pending[0]
 
     @contextlib.contextmanager
     def _member(self, k):
@@ -141,7 +170,7 @@ class Sweep:
         with torch.cuda.stream(self.streams[k]), ops.owner(self.members[k]._sweep_token):
             yield
 
-    def _run(self, loader, epochs, checkpoint_every, start):
+    def _run(self, loader, first, epochs, checkpoint_every, save_state, start):
         members = self.members
         main = torch.cuda.current_stream(self.device)
         if self.streams is None:
@@ -157,11 +186,13 @@ class Sweep:
                 m.model.seed_noise(noise, self.device)
             if hasattr(m.loss_f, "seed_permutations") and m.loss_f._perm_offset is None:
                 m.loss_f.seed_permutations(perm, self.device)
+            m._data_loader = loader
             m.model.train()
         done = [None] * len(members)      # each member's stream after its latest step
         inputs = self._inputs             # batch size -> the buffer the gather writes and every member's graph reads
+        last = first + epochs - 1
         try:
-            for epoch in range(epochs):
+            for epoch in range(first, first + epochs):
                 storers = [defaultdict(list) for _ in members]
                 tallies = []
                 for k, m in enumerate(members):
@@ -187,7 +218,8 @@ class Sweep:
                             done[k].record()
                 for k, m in enumerate(members):
                     with self._member(k):
-                        m._end_epoch(epoch, storers[k], tallies[k].close(), checkpoint_every)
+                        m._end_epoch(epoch, storers[k], tallies[k].close(), checkpoint_every,
+                                     save_state=save_state and (epoch % checkpoint_every == 0 or epoch == last))
                         done[k] = torch.cuda.Event()
                         done[k].record()
         finally:

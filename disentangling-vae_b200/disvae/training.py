@@ -6,6 +6,10 @@ per-step copy of the loss into pinned host memory (the progress bar shows the la
 already landed), host batches are uploaded one step ahead on a copy stream (`_Prefetcher`), and under
 torch.distributed (one process per GPU) gradients are averaged with one flat all-reduce per step
 (disvae.parallel).
+
+A run can be stopped and continued at an epoch boundary: `training_state()` / `load_training_state()` (and
+`trainer(..., save_state=True)`, which writes one at every checkpoint) carry everything a later step reads, so the
+continued run is bit-identical to one that was never stopped.
 """
 import logging
 import os
@@ -13,15 +17,24 @@ from collections import defaultdict, namedtuple
 from timeit import default_timer
 
 import torch
+import torch.distributed as dist
 from tqdm import trange
 
 from disvae import _native
 from disvae.fused import FusedAdam
 from disvae.models.losses import DeviceLossLog
 from disvae.parallel import GradAverage, broadcast_parameters, is_distributed
-from disvae.utils.modelIO import save_model
+from disvae.utils.modelIO import TRAINING_STATE_PREFIX, save_model, save_training_state
 
 TRAIN_LOSSES_LOGFILE = "train_losses.log"
+TRAINING_STATE_FORMAT = 1                 # version of the dict `Trainer.training_state` returns
+
+
+def training_state_filename(epoch):
+    """`training-state-{epoch}.pt`; under data parallelism one file per rank, `training-state-{epoch}-rank{r}.pt`."""
+    if is_distributed():
+        return "{}{}-rank{}.pt".format(TRAINING_STATE_PREFIX, epoch, dist.get_rank())
+    return "{}{}.pt".format(TRAINING_STATE_PREFIX, epoch)
 
 
 class Trainer():
@@ -52,28 +65,135 @@ class Trainer():
         self._loss_log = None                     # DeviceLossLog of the training steps (built on the first GPU step)
         self._resident_input = None               # fp32 device batch a caller refills in place (disvae.sweep): a graph
                                                   # captured on it reads it directly instead of a copy
+        self._next_epoch = 0                      # number of the epoch after the last one completed (training state)
+        self._data_loader = None                  # the loader of the current / latest call (its data-order state)
+        self._resume = None                       # (first epoch, loader state) of a loaded state, for the next call
+        self._steps_at_load = 0                   # n_train_steps a loaded state restored
         self.logger.info("Training Device: {}".format(self.device))
 
-    def __call__(self, data_loader, epochs=10, checkpoint_every=10):
-        """training.py:64-102"""
+    def __call__(self, data_loader, epochs=10, checkpoint_every=10, save_state=False):
+        """training.py:64-102.  `save_state=True` also writes the training state (`training_state_filename`) next to
+        every checkpoint and after the last epoch.  After `load_training_state` the epochs are numbered on from the
+        saved one and the loader continues the saved data order."""
         start = default_timer()
+        first, loader_state = (0, None) if self._resume is None else self._resume
+        if loader_state is not None:
+            check_loader_state(loader_state, data_loader, self.device_data)
+        self._resume = None
         if self.device_data and isinstance(data_loader, torch.utils.data.DataLoader):
             data_loader = self._device_loader(data_loader)
+        if loader_state is not None:
+            apply_loader_state(loader_state, data_loader)
+        self._data_loader = data_loader
         self.model.train()
-        for epoch in range(epochs):
+        for epoch in range(first, first + epochs):
             storer = defaultdict(list)
             mean_epoch_loss = self._train_epoch(data_loader, storer, epoch)
-            self._end_epoch(epoch, storer, mean_epoch_loss, checkpoint_every)
+            self._end_epoch(epoch, storer, mean_epoch_loss, checkpoint_every,
+                            save_state=save_state and (epoch % checkpoint_every == 0 or epoch == first + epochs - 1))
         self._end_training(start)
 
-    def _end_epoch(self, epoch, storer, mean_epoch_loss, checkpoint_every):
-        """training.py:84-90: epoch log line, train_losses.log rows, GIF frame, checkpoint."""
+    def _end_epoch(self, epoch, storer, mean_epoch_loss, checkpoint_every, save_state=False):
+        """training.py:84-90: epoch log line, train_losses.log rows, GIF frame, checkpoint; the training state when
+        `save_state`."""
         self.logger.info('Epoch: {} Average loss per image: {:.2f}'.format(epoch + 1, mean_epoch_loss))
         self.losses_logger.log(epoch, storer)
+        self._next_epoch = epoch + 1
         if self.gif_visualizer is not None:
             self.gif_visualizer()
         if epoch % checkpoint_every == 0:
             save_model(self.model, self.save_dir, filename="model-{}.pt".format(epoch))
+        if save_state:
+            save_training_state(self, self.save_dir, training_state_filename(epoch))
+
+    # -- training state -------------------------------------------------------------------------
+    def training_state(self):
+        """The state a continued run needs, as CPU tensors and Python values (see INTEGRATION.md, "Resuming
+        training").  Taken at an epoch end, where the optimizers' step counts have been written back (flush_state)."""
+        model, lf = self.model, self.loss_f
+        loader = self._resume[1] if self._resume is not None else loader_state(self._data_loader)
+        state = dict(
+            format=TRAINING_STATE_FORMAT, epoch=self._next_epoch,
+            model=dict(model_type=getattr(model, "model_type", None), img_size=list(model.img_size),
+                       latent_dim=int(model.latent_dim), state_dict=_cpu(model.state_dict())),
+            optimizer=_cpu(self.optimizer.state_dict()),
+            loss=dict(cls=type(lf).__name__, hparams=loss_hparams(lf), n_train_steps=int(lf.n_train_steps)),
+            noise=_philox(getattr(model, "_rng_seed", None), getattr(model, "_rng_offset", None)),
+            factor=None, loader=loader, log_rows=list(self.losses_logger.rows),
+            world_size=dist.get_world_size() if is_distributed() else 1,
+            rank=dist.get_rank() if is_distributed() else 0)
+        if hasattr(lf, "call_optimize"):
+            state["factor"] = dict(discriminator=_cpu(lf.discriminator.state_dict()),
+                                   optimizer_d=_cpu(lf.optimizer_d.state_dict()),
+                                   perm=_philox(getattr(lf, "_perm_seed", None), lf._perm_offset),
+                                   global_perm=_philox(getattr(lf, "_gperm_seed", None), lf._gperm_offset))
+        return state
+
+    def load_training_state(self, state):
+        """Continue from `state` (a `training_state()`): into a Trainer that has taken no step in this process, with
+        the same model geometry, loss class and hyper-parameters and world size; raises ValueError naming the first
+        field that differs, before anything is changed.  The loader is checked and set at the next call."""
+        self._check_training_state(state)
+        model, lf = self.model, self.loss_f
+        dev = next(model.parameters()).device
+        model.load_state_dict(state["model"]["state_dict"])
+        self.optimizer.load_state_dict(state["optimizer"])   # FusedAdam, built at the first step, starts from its counts
+        lf.n_train_steps = self._steps_at_load = state["loss"]["n_train_steps"]   # (_step_counter follows it)
+        # the Philox keys and counters: the first steps (eager and captured alike) continue the saved streams
+        if state["noise"]["key"] is not None:
+            model.seed_noise(state["noise"]["key"], dev)
+            model._rng_offset.fill_(state["noise"]["offset"])
+        if state["factor"] is not None:
+            f = state["factor"]
+            lf.discriminator.load_state_dict(f["discriminator"])
+            lf.optimizer_d.load_state_dict(f["optimizer_d"])
+            if f["perm"]["key"] is not None:
+                lf.seed_permutations(f["perm"]["key"], dev)
+                lf._perm_offset.fill_(f["perm"]["offset"])
+            if f["global_perm"]["key"] is not None:
+                lf._gperm_seed = f["global_perm"]["key"]
+                lf._gperm_offset = torch.full((1,), f["global_perm"]["offset"], dtype=torch.int64, device=dev)
+        loader = state["loader"]
+        if loader is not None and loader["kind"] == "host":
+            torch.set_rng_state(loader["rng_state"])         # a RandomSampler draws its next orders from it
+        self.losses_logger.restore(state["log_rows"])
+        self._next_epoch = state["epoch"]
+        self._resume = (state["epoch"], loader)
+
+    def _check_training_state(self, state):
+        def refuse(field, saved, here):
+            raise ValueError("load_training_state: {} is {!r} in the saved state but {!r} here".format(field, saved, here))
+        if not isinstance(state, dict) or state.get("format") != TRAINING_STATE_FORMAT:
+            raise ValueError("load_training_state: unknown training-state format {!r} (this version reads {})".format(
+                state.get("format") if isinstance(state, dict) else type(state).__name__, TRAINING_STATE_FORMAT))
+        lf = self.loss_f
+        if (self._graphs or self._eligible_steps or self._fused is not None or getattr(lf, "_fused_d", None) is not None
+                or lf.n_train_steps != self._steps_at_load):
+            raise ValueError("load_training_state: this Trainer has already taken training steps; load the state into "
+                             "a new Trainer")
+        m = state["model"]
+        here = dict(model_type=getattr(self.model, "model_type", None), img_size=list(self.model.img_size),
+                    latent_dim=int(self.model.latent_dim))
+        for field in ("model_type", "img_size", "latent_dim"):
+            if m[field] != here[field]:
+                refuse(field, m[field], here[field])
+        if state["loss"]["cls"] != type(lf).__name__:
+            refuse("the loss class", state["loss"]["cls"], type(lf).__name__)
+        saved, hp = state["loss"]["hparams"], loss_hparams(lf)
+        for k in sorted(set(saved) | set(hp)):
+            if saved.get(k) != hp.get(k):
+                refuse("loss hyper-parameter " + k, saved.get(k), hp.get(k))
+        world = dist.get_world_size() if is_distributed() else 1
+        if state["world_size"] != world:
+            refuse("the world size", state["world_size"], world)
+        rank = dist.get_rank() if is_distributed() else 0
+        if state["rank"] != rank:
+            refuse("the rank", state["rank"], rank)
+        if (state["factor"] is not None) != hasattr(lf, "call_optimize"):
+            refuse("the discriminator state", state["factor"] is not None, hasattr(lf, "call_optimize"))
+        if state["factor"] is not None:
+            _check_shapes("discriminator", state["factor"]["discriminator"], lf.discriminator.state_dict())
+        _check_shapes("model", m["state_dict"], self.model.state_dict())
 
     def _end_training(self, start):
         if self.gif_visualizer is not None:
@@ -301,6 +421,91 @@ class Trainer():
         return loss
 
 
+# -- training-state helpers -------------------------------------------------------------------------------------------
+def _cpu(obj):
+    """`obj` (a state_dict: nested dicts / lists of tensors and Python values) with every tensor copied to the host."""
+    if torch.is_tensor(obj):
+        return obj.detach().to("cpu", copy=True)
+    if isinstance(obj, dict):
+        return {k: _cpu(v) for k, v in obj.items()}
+    if isinstance(obj, (list, tuple)):
+        return type(obj)(_cpu(v) for v in obj)
+    return obj
+
+
+def _philox(key, counter):
+    """A Philox stream's key and counter value (None, None before its first draw)."""
+    return dict(key=key, offset=None if counter is None else int(counter))
+
+
+def loss_hparams(loss_f):
+    """The loss's settings that a continued run must share: its public int / float / str / bool attributes
+    (record_loss_every, rec_dist, steps_anneal, beta, gamma, ...), the step counter excepted."""
+    return {k: v for k, v in sorted(vars(loss_f).items())
+            if not k.startswith("_") and k != "n_train_steps" and isinstance(v, (bool, int, float, str))}
+
+
+def _check_shapes(what, saved, here):
+    if list(saved) != list(here):
+        raise ValueError("load_training_state: the {} has parameters {} in the saved state but {} here".format(
+            what, list(saved), list(here)))
+    for k, v in saved.items():
+        if tuple(v.shape) != tuple(here[k].shape):
+            raise ValueError("load_training_state: {} parameter {} is {} in the saved state but {} here".format(
+                what, k, tuple(v.shape), tuple(here[k].shape)))
+
+
+def _loader_shape(loader):
+    """(n, batch_size, shuffle, drop_last) of a DeviceLoader or a torch DataLoader."""
+    from disvae.data import DeviceLoader
+    if isinstance(loader, DeviceLoader):
+        return loader.n, loader.batch_size, loader.shuffle, loader.drop_last
+    return (len(loader.dataset), loader.batch_size, isinstance(loader.sampler, torch.utils.data.RandomSampler),
+            loader.drop_last)
+
+
+def loader_state(loader):
+    """The data-order state of `loader` after the epochs it has run: a DeviceLoader's seed and epoch, or for a host
+    loader the CPU RNG state its RandomSampler draws from.  None for no loader."""
+    from disvae.data import DeviceLoader
+    if loader is None:
+        return None
+    if isinstance(loader, DeviceLoader):
+        n, b, shuffle, drop_last = _loader_shape(loader)
+        return dict(kind="device", seed=loader.seed, epoch=loader.epoch, n=n, batch_size=b, shuffle=shuffle,
+                    drop_last=drop_last)
+    state = dict(kind="host", rng_state=torch.get_rng_state(), n=None, batch_size=None, shuffle=None, drop_last=None)
+    if isinstance(loader, torch.utils.data.DataLoader):
+        state.update(zip(("n", "batch_size", "shuffle", "drop_last"), _loader_shape(loader)))
+    return state
+
+
+def check_loader_state(saved, loader, device_data=False):
+    """ValueError unless `loader` continues the data order `saved` describes: the same kind (a DeviceLoader, also one
+    that DISVAE_DEVICE_DATA=1 builds from a DataLoader, or a host loader) over the same number of items, batch size,
+    shuffling and drop_last.  No GPU work."""
+    from disvae.data import DeviceLoader
+    is_dl = isinstance(loader, torch.utils.data.DataLoader)
+    kind = "device" if isinstance(loader, DeviceLoader) or (device_data and is_dl) else "host"
+    if kind != saved["kind"]:
+        raise ValueError("training state: the saved run read a {} loader but this call passes a {} one; the data order "
+                         "would differ".format(saved["kind"], kind))
+    if saved["n"] is None or not (is_dl or kind == "device"):
+        return
+    for field, want, got in zip(("n", "batch_size", "shuffle", "drop_last"),
+                                (saved["n"], saved["batch_size"], saved["shuffle"], saved["drop_last"]),
+                                _loader_shape(loader)):
+        if want != got:
+            raise ValueError("training state: the loader's {} is {!r} in the saved state but {!r} here".format(
+                field, want, got))
+
+
+def apply_loader_state(saved, loader):
+    """A DeviceLoader continues the saved order (its seed and epoch); a host loader's RNG was restored at the load."""
+    if saved["kind"] == "device":
+        loader.seed, loader.epoch = saved["seed"], saved["epoch"]
+
+
 # One captured training step (Trainer._graphs): the graph, its input buffer and loss, the native kernels one replay runs,
 # under data parallelism the static gradient tensors the replay writes (in GradAverage order; None otherwise), and the
 # FusedAdams whose steps the graph holds.
@@ -419,24 +624,44 @@ class _HostLossRing:
 
 
 class LossesLogger(object):
-    """CSV "Epoch,Loss,Value" writer (training.py:167-190)."""
+    """CSV "Epoch,Loss,Value" writer (training.py:167-190).  `rows` keeps the rows written after the header, which a
+    training state carries and `restore` writes back."""
+
+    HEADER = ",".join(["Epoch", "Loss", "Value"])
 
     def __init__(self, file_path_name):
         if os.path.isfile(file_path_name):
             os.remove(file_path_name)
+        self.file_path_name = file_path_name
+        self.rows = []
         # a logger of its own, not the shared named one: several Trainers in one process (disvae.sweep) each write
         # only their own file
         self.logger = logging.Logger("losses_logger")
         self.logger.parent = logging.getLogger("losses_logger")
         self.logger.setLevel(1)
-        file_handler = logging.FileHandler(file_path_name)
+        self._open()
+        self.logger.debug(self.HEADER)
+
+    def _open(self):
+        file_handler = logging.FileHandler(self.file_path_name)
         file_handler.setLevel(1)
         self.logger.addHandler(file_handler)
-        self.logger.debug(",".join(["Epoch", "Loss", "Value"]))
 
     def log(self, epoch, losses_storer):
         for k, v in losses_storer.items():
-            self.logger.debug(",".join(str(item) for item in [epoch, k, mean(v)]))
+            row = ",".join(str(item) for item in [epoch, k, mean(v)])
+            self.rows.append(row)
+            self.logger.debug(row)
+
+    def restore(self, rows):
+        """Rewrite the file as the header and `rows` (a saved run's); later rows are appended to it."""
+        for h in list(self.logger.handlers):
+            self.logger.removeHandler(h)
+            h.close()
+        self.rows = list(rows)
+        with open(self.file_path_name, "w") as f:
+            f.write("".join(line + "\n" for line in [self.HEADER] + self.rows))
+        self._open()
 
 
 def mean(l):

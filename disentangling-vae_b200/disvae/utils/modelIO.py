@@ -1,6 +1,7 @@
 """Checkpoint IO with the reference's on-disk format (disvae/utils/modelIO.py:14-173):
 `model.pt` is a plain state_dict with the reference's keys, `specs.json` the metadata, so
-checkpoints shipped with the reference (results/*/model.pt) load into this implementation."""
+checkpoints shipped with the reference (results/*/model.pt) load into this implementation.  `training-state-*.pt`
+files (save_training_state) hold what continuing a run needs besides the weights."""
 import json
 import os
 import re
@@ -10,6 +11,7 @@ import torch
 
 MODEL_FILENAME = "model.pt"
 META_FILENAME = "specs.json"
+TRAINING_STATE_PREFIX = "training-state-"
 
 
 def save_metadata(metadata, directory, filename=META_FILENAME, **kwargs):
@@ -47,10 +49,26 @@ def load_checkpoints(directory, is_gpu=True):
     checkpoints = []
     for root, _, filenames in os.walk(directory):
         for filename in filenames:
+            if filename.startswith(TRAINING_STATE_PREFIX):          # not a model checkpoint
+                continue
             results = re.search(r'.*?-([0-9].*?).pt', filename)
             if results is not None:
                 checkpoints.append((int(results.group(1)), load_model(root, is_gpu=is_gpu, filename=filename)))
     return checkpoints
+
+
+def save_training_state(trainer, directory, filename):
+    """`trainer.training_state()` (disvae.training.Trainer) saved to directory/filename; returns the path."""
+    path = os.path.join(directory, filename)
+    torch.save(trainer.training_state(), path)
+    return path
+
+
+def load_training_state(trainer, path):
+    """Apply the training state saved at `path` to `trainer` (Trainer.load_training_state); returns the state."""
+    state = torch.load(path, map_location="cpu", weights_only=True)
+    trainer.load_training_state(state)
+    return state
 
 
 def numpy_serialize(obj):

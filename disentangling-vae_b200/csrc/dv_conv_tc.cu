@@ -10,9 +10,9 @@
 //     in registers right after their fragment loads; the packed weights already hold both planes.
 //   * warp roles (288 threads, 1 CTA/SM, persistent over tiles): warps 0-7 load fragments, run the MMAs and the
 //     epilogue; warp 8 is the TMA producer.  mbarrier rings between them: raw-full (TMA transaction count) and
-//     raw-empty (one arrival per consumer warp).  down and up: warps 0-3 and 4-7 are two warpgroups of 64 MMA rows
-//     issuing wgmma with A from registers and B (the resident packed weights) from shared memory; wgrad: each warp
-//     issues mma.sync m16n8k8.
+//     raw-empty (one arrival per consumer warp that reads the slot).  Warps 0-3 and 4-7 are two warpgroups of 64 MMA
+//     rows issuing wgmma with A from registers and B from shared memory: the resident packed weights (down, up), or the
+//     lo tile transposed and split once per tile by the consumer warps (wgrad).
 #include "dv_common.cuh"
 #include "dv_ptx.cuh"
 
@@ -221,21 +221,33 @@ conv_down32_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 
 // ------------------------------------------------------------------------------------------
 // wgrad: dw[cl][c][tap] = sum_p lo[p][cl] * hi(2i-1+kh, 2j-1+kw)[c]   (reduction over PIXELS)
-//   Per 128-pixel tile: the lo tile (B operand, N = 32 lo channels) and the 16 tap tiles of the hi patch (A operand,
-//   M = 32 hi channels, read transposed out of the [pixel][channel] tile).  Warp w owns taps w and w + 8 and always
-//   consumes ring slot w.  K slot t of an MMA holds pixel 8ks + 2t and slot t + 4 pixel 8ks + 2t + 1: with the 128-byte
-//   swizzle the transposed fragment loads then hit 32 distinct banks.  The fp32 running totals (2 taps x 32 x 32 per
-//   warp) live in shared memory, lane-interleaved (conflict-free), which keeps the MMA loop free of register spills.
+//   Per 128-pixel tile one GEMM per pair of taps: M = 64 (2 taps x 32 hi channels), N = 32 lo channels, K = 128 pixels
+//   in 16 k8 slices.  Each warpgroup owns 8 taps: warpgroup wg runs the tap pairs (4j + 2wg, 4j + 2wg + 1), j = 0..3,
+//   and inside a pair warps 0-1 hold the first tap (channels 0-15 / 16-31), warps 2-3 the second.
+//   A (registers): the tap tiles, read transposed out of the swizzled [pixel][channel] TMA tile and split hi/lo.  K slot
+//   t of a slice holds pixel 8ks + 2t and slot t + 4 pixel 8ks + 2t + 1: with the 128-byte swizzle the transposed loads
+//   then hit 32 distinct banks.
+//   B (shared memory): tf32 wgmma reads shared operands K-major only and the lo tile lands [pixel][channel], so once per
+//   tile the consumer warps transpose it: warp w reads pixels [16w, 16w + 16) of channel `lane`, splits them and writes
+//   the hi and the lo plane, each [32 channels][128 pixels] as four K-blocks of 32 pixels (4 KB, 128-byte rows, 128-byte
+//   swizzle: what wgmma_desc_k128 describes), in the K-slot order of A.  The channel sums of lo (bias gradient) come
+//   from the same registers.
+//   Per (tile, tap pair): acc = A_hi.B_hi and corr = A_hi.B_lo + A_lo.B_hi accumulate over the 16 slices in the tensor
+//   core, one commit group per slice, four slices of A fragments in flight; acc + corr is then added to the fp32
+//   running totals, which live in shared memory, lane-interleaved (conflict-free).
 //   Split-K over CTAs; the partials are reduced in a fixed order by conv_wgrad_reduce_kernel.
+//   smem: 7-slot ring of 16 KB tap tiles (112 KB) + raw lo tile (16 KB) + hi/lo planes (32 KB) + barriers (2 KB) +
+//   totals (64 KB) + 1 KB alignment slack = 227 KB.
 // ------------------------------------------------------------------------------------------
-constexpr int kWtSlots = kConsumers;
+constexpr int kWtSlots = 7;
+constexpr int kWtPlane = 32 * 128 * 4;                 // bytes: one plane, [32 channels][128 pixels]
 struct WtBarriers {
   uint64_t raw_full[kWtSlots], raw_empty[kWtSlots];
-  uint64_t l_full[2], l_empty[2];
+  uint64_t l_full, l_empty;
   float lsum[kConsumers][32];
 };
-constexpr int kWtTotFloats = 2 * 32 * 32;              // per consumer warp: [tap w / w+8][32 fragment values][lane]
-constexpr int kWtSmem = kWtSlots * kATile + 2 * kATile + 2048 + kConsumers * kWtTotFloats * 4 + 1024;
+constexpr int kWtTotFloats = 4 * 16 * 32;              // per consumer warp: [tap pair][16 accumulator values][lane]
+constexpr int kWtSmem = kWtSlots * kATile + kATile + 2 * kWtPlane + 2048 + kConsumers * kWtTotFloats * 4 + 1024;
 static_assert(sizeof(WtBarriers) <= 2048, "barrier block too large");
 static_assert(kWtSmem <= kSmemMax, "smem");
 
@@ -244,21 +256,22 @@ struct WtGeom {
 };
 
 __global__ void __launch_bounds__(kThreads, 1)
-conv_wgrad32_mma_kernel(const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo,
-                        float* __restrict__ ws, WtGeom g) {
+conv_wgrad32_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo,
+                          float* __restrict__ ws, WtGeom g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint8_t* Raw = smem;                                       // [slot][128 px][32 ch]
-  uint8_t* Ls = smem + kWtSlots * kATile;                    // [buf][128 px][32 ch]
-  WtBarriers* bars = reinterpret_cast<WtBarriers*>(Ls + 2 * kATile);
+  uint8_t* Ls = smem + kWtSlots * kATile;                    // [128 px][32 ch]
+  uint8_t* Planes = Ls + kATile;                             // [hi / lo][K-block][32 ch][32 px]
+  WtBarriers* bars = reinterpret_cast<WtBarriers*>(Planes + 2 * kWtPlane);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float* tot = reinterpret_cast<float*>(Ls + 2 * kATile + 2048) + warp * kWtTotFloats + lane;   // tot[k * 32]
+  float* tot = reinterpret_cast<float*>(Planes + 2 * kWtPlane + 2048) + warp * kWtTotFloats + lane;   // tot[k * 32]
   const int t_begin = blockIdx.x * g.tiles_per_cta;
   const int t_end = min(g.num_tiles, t_begin + g.tiles_per_cta);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kWtSlots; ++s) { mbar_init(&bars->raw_full[s], 1); mbar_init(&bars->raw_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&bars->l_full[s], 1); mbar_init(&bars->l_empty[s], kConsumers); }
+    for (int s = 0; s < kWtSlots; ++s) { mbar_init(&bars->raw_full[s], 1); mbar_init(&bars->raw_empty[s], 2); }
+    mbar_init(&bars->l_full, 1); mbar_init(&bars->l_empty, kConsumers);
     fence_mbar_init();
   }
   __syncthreads();
@@ -266,7 +279,7 @@ conv_wgrad32_mma_kernel(const __grid_constant__ CUtensorMap tmap_hi, const __gri
   if (warp == kConsumers) {
     if (lane != 0) return;
     prefetch_tmap(&tmap_hi); prefetch_tmap(&tmap_lo);
-    uint32_t tseq = 0;
+    int slot = 0; uint32_t phase = 0, tseq = 0;
     for (int tile = t_begin; tile < t_end; ++tile, ++tseq) {
       const int r0 = tile * g.rows_per_tile;
       const int b0 = r0 / g.H, i0 = r0 % g.H;
@@ -276,90 +289,104 @@ conv_wgrad32_mma_kernel(const __grid_constant__ CUtensorMap tmap_hi, const __gri
         for (int t4 = 0; t4 < 4; ++t4) tma_prefetch_4d(&tmap_hi, 0, (t4 & 1), 2 * in_ + (t4 >> 1), bn);
         tma_prefetch_4d(&tmap_lo, 0, 0, in_, bn);
       }
-      const int lb = tseq & 1;
-      mbar_wait(&bars->l_empty[lb], ((tseq >> 1) & 1u) ^ 1u);
-      mbar_arrive_expect_tx(&bars->l_full[lb], kATile);
-      tma_load_4d(Ls + lb * kATile, &tmap_lo, &bars->l_full[lb], 0, 0, i0, b0);
-      for (int tap = 0; tap < kTaps; ++tap) {
-        const int kh = tap >> 2, kw = tap & 3, slot = tap & 7;
-        const uint32_t use = tseq * 2 + (tap >> 3);          // uses of this slot so far
-        mbar_wait(&bars->raw_empty[slot], (use & 1u) ^ 1u);
+      mbar_wait(&bars->l_empty, (tseq & 1u) ^ 1u);
+      mbar_arrive_expect_tx(&bars->l_full, kATile);
+      tma_load_4d(Ls, &tmap_lo, &bars->l_full, 0, 0, i0, b0);
+      for (int tap = 0; tap < kTaps; ++tap) {                // the order the two warpgroups consume them in
+        const int kh = tap >> 2, kw = tap & 3;
+        mbar_wait(&bars->raw_empty[slot], phase ^ 1);
         mbar_arrive_expect_tx(&bars->raw_full[slot], kATile);
         tma_load_4d(Raw + slot * kATile, &tmap_hi, &bars->raw_full[slot], 0, kw - 1, 2 * i0 - 1 + kh, b0);
+        if (++slot == kWtSlots) { slot = 0; phase ^= 1; }
       }
     }
     return;
   }
 
-  const int gq = lane >> 2, t = lane & 3;
-  const uint32_t slot_base = smem_u32(Raw) + warp * kATile, l0 = smem_u32(Ls);
-  for (int k = 0; k < 64; ++k) tot[k * 32] = 0.f;          // k = (tap w / w+8) * 32 + (c block * 4 + cl block) * 4 + fragment
+  const int gq = lane >> 2, t = lane & 3, wg = warp >> 2, wq = warp & 3;
+  const uint32_t raw0 = smem_u32(Raw), l_base = smem_u32(Ls), planes = smem_u32(Planes);
+  // A fragment {A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4]} of slice ks = the tap tile at (pixel 8ks + 2t, c),
+  // (8ks + 2t, c + 8), (8ks + 2t + 1, c), (8ks + 2t + 1, c + 8): 1024 ks bytes past these offsets
+  const int c0 = (wq & 1) * 16 + gq;
+  const uint32_t a_off[4] = {swz128(2 * t, c0), swz128(2 * t, c0 + 8), swz128(2 * t + 1, c0), swz128(2 * t + 1, c0 + 8)};
+  for (int k = 0; k < 64; ++k) tot[k * 32] = 0.f;          // k = tap pair * 16 + accumulator index
   float lsum = 0.f;                                          // lo channel `lane` over this warp's 16 rows of every tile
   uint32_t tseq = 0;
   for (int tile = t_begin; tile < t_end; ++tile, ++tseq) {
-    const int lb = tseq & 1;
-    mbar_wait(&bars->l_full[lb], (tseq >> 1) & 1u);
-    const uint32_t l_base = l0 + lb * kATile;
-#pragma unroll 4
-    for (int r = 0; r < 16; ++r) lsum += __uint_as_float(lds32(l_base + swz128(warp * 16 + r, lane)));
-#pragma unroll 1
-    for (int j = 0; j < 2; ++j) {
-      const uint32_t use = tseq * 2 + j;
-      mbar_wait(&bars->raw_full[warp], use & 1u);
-      float mn[2][4][4] = {}, cr[2][4][4] = {};
-#pragma unroll 1
-      for (int ks = 0; ks < 16; ++ks) {
-        const int px0 = 8 * ks + 2 * t, px1 = px0 + 1;
-        uint32_t ah[2][4], al[2][4], bh[4][2], bl[4][2];
+    mbar_wait(&bars->l_full, tseq & 1u);
+    consumers_sync();                                        // every warp's MMAs of the previous tile have read the planes
+    {
+      uint32_t v[16];
 #pragma unroll
-        for (int mt = 0; mt < 2; ++mt) {
-          const int c = mt * 16 + gq;
-          uint32_t a[4];
-          a[0] = lds32(slot_base + swz128(px0, c));
-          a[1] = lds32(slot_base + swz128(px0, c + 8));
-          a[2] = lds32(slot_base + swz128(px1, c));
-          a[3] = lds32(slot_base + swz128(px1, c + 8));
+      for (int r = 0; r < 16; ++r) v[r] = lds32(l_base + swz128(warp * 16 + r, lane));
 #pragma unroll
-          for (int e = 0; e < 4; ++e) split_tf32(a[e], ah[mt][e], al[mt][e]);
+      for (int r = 0; r < 16; ++r) lsum += __uint_as_float(v[r]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->l_empty);            // the raw tile is in registers
+      // slice ks = 2 warp + h, pixels 8ks + 2q + par -> K columns 8 (ks & 3) + 4 par + q of K-block ks >> 2: one 16-byte
+      // chunk of row `lane` per (h, par)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int par = 0; par < 2; ++par) {
+          const int ks = 2 * warp + h;
+          uint32_t ph[4], pl[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) split_tf32(v[8 * h + 2 * q + par], ph[q], pl[q]);
+          const uint32_t dst = planes + (ks >> 2) * 4096 + swz128(lane, 8 * (ks & 3) + 4 * par);
+          sts128(dst, ph);
+          sts128(dst + kWtPlane, pl);
         }
+    }
+    fence_proxy_async();
+    consumers_sync();
+#pragma unroll 1
+    for (int j = 0; j < 4; ++j) {
+      const uint32_t n = tseq * kTaps + 4 * j + 2 * wg + (wq >> 1);      // this warp's tap tile in the producer's sequence
+      const uint32_t slot = n % kWtSlots;
+      mbar_wait(&bars->raw_full[slot], (n / kWtSlots) & 1u);
+      const uint32_t a_base = raw0 + slot * kATile;
+      float acc[16], corr[16];
+      uint32_t ah[16], al[16];
+#pragma unroll 1
+      for (int kb = 0; kb < 4; ++kb) {
 #pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-          const int cl = nt * 8 + gq;
-          split_tf32(lds32(l_base + swz128(px0, cl)), bh[nt][0], bl[nt][0]);
-          split_tf32(lds32(l_base + swz128(px1, cl)), bh[nt][1], bl[nt][1]);
+        for (int k4 = 0; k4 < 4; ++k4) {
+          const int ks = 4 * kb + k4;
+          wgmma_wait<3>();                                   // slice ks - 4, the last reader of these A registers
+#pragma unroll
+          for (int e = 0; e < 4; ++e) split_tf32(lds32(a_base + 1024 * ks + a_off[e]), ah[4 * k4 + e], al[4 * k4 + e]);
+          fence_regs(acc);
+          fence_regs(corr);
+          wgmma_fence();
+          const uint64_t b_hi = wgmma_desc_k128(planes + kb * 4096 + 32 * k4), b_lo = wgmma_desc_k128(planes + kWtPlane + kb * 4096 + 32 * k4);
+          wgmma_m64n32k8_rs(acc, ah + 4 * k4, b_hi, ks);
+          wgmma_m64n32k8_rs(corr, ah + 4 * k4, b_lo, ks);
+          wgmma_m64n32k8_rs(corr, al + 4 * k4, b_hi, 1);
+          wgmma_commit();
         }
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-          for (int nt = 0; nt < 4; ++nt) mma_3xtf32(mn[mt][nt], cr[mt][nt], ah[mt], al[mt], bh[nt], bl[nt]);
       }
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->raw_empty[warp]);
+      if (lane == 0) mbar_arrive(&bars->raw_empty[slot]);    // the tap tile is in registers
+      wgmma_wait<0>();
+      fence_regs(acc);
+      fence_regs(corr);
 #pragma unroll
-      for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) tot[(j * 32 + (mt * 4 + nt) * 4 + e) * 32] += mn[mt][nt][e] + cr[mt][nt][e];
+      for (int i = 0; i < 16; ++i) tot[(j * 16 + i) * 32] += acc[i] + corr[i];
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars->l_empty[lb]);
   }
 
+  // accumulator i = 4 nt + 2 h + e of tap pair j: tap 4j + 2wg + (wq >> 1), c = c0 + 8 h, cl = 8 nt + 2 t + e
   float* out = ws + (long long)blockIdx.x * (kTaps * 32 + 1) * kLoCh;
 #pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const int tap = warp + 8 * j;
+  for (int j = 0; j < 4; ++j) {
+    const int tap = 4 * j + 2 * wg + (wq >> 1);
 #pragma unroll
-    for (int mt = 0; mt < 2; ++mt)
+    for (int nt = 0; nt < 4; ++nt)
 #pragma unroll
-      for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int c = mt * 16 + gq + 8 * h, cl = nt * 8 + 2 * t;
-          *reinterpret_cast<float2*>(out + (tap * 32 + c) * kLoCh + cl) =
-              make_float2(tot[(j * 32 + (mt * 4 + nt) * 4 + 2 * h) * 32], tot[(j * 32 + (mt * 4 + nt) * 4 + 2 * h + 1) * 32]);
-        }
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<float2*>(out + (tap * 32 + c0 + 8 * h) * kLoCh + nt * 8 + 2 * t) =
+            make_float2(tot[(j * 16 + 4 * nt + 2 * h) * 32], tot[(j * 16 + 4 * nt + 2 * h + 1) * 32]);
   }
   bars->lsum[warp][lane] = lsum;                             // bias gradient: channel sums of lo, fixed order
   consumers_sync();
@@ -619,7 +646,7 @@ int conv_down32_tc(const float* hi, const float* wd_packed, const float* bias, c
   return check_launch();
 }
 
-// CTAs of conv_wgrad32_mma_kernel, one split-K partial each: at most one per SM, no empty CTA
+// CTAs of conv_wgrad32_wgmma_kernel, one split-K partial each: at most one per SM, no empty CTA
 int wgrad_splits(int B, int H, int W) {
   const int num_tiles = (int)(((long long)B * H * W + 127) / 128);
   const int grid = num_tiles < kNumSMs ? num_tiles : kNumSMs;
@@ -643,9 +670,9 @@ int conv_wgrad32_tc(const float* lo, const float* hi, float* ws, int B, int H, i
   if (!make_act_tmap(&thi, hi, B, 2 * H, 2 * W, 2 * W, 2 * TR, TB, 2)) return DV_ERR_CUDA;
   if (!make_act_tmap(&tlo, lo, B, H, W, W, TR, TB, 1)) return DV_ERR_CUDA;
   static bool attr = false;
-  const int rc = set_max_dynamic_smem(conv_wgrad32_mma_kernel, kWtSmem, &attr);
+  const int rc = set_max_dynamic_smem(conv_wgrad32_wgmma_kernel, kWtSmem, &attr);
   if (rc != DV_OK) return rc;
-  conv_wgrad32_mma_kernel<<<grid, kThreads, kWtSmem, st>>>(thi, tlo, ws, g);
+  conv_wgrad32_wgmma_kernel<<<grid, kThreads, kWtSmem, st>>>(thi, tlo, ws, g);
   return check_launch();
 }
 

@@ -49,6 +49,14 @@ __device__ __forceinline__ uint32_t lds32(uint32_t smem_addr) {
   return v;
 }
 
+// four consecutive 32-bit words of shared memory (16-byte aligned address)
+__device__ __forceinline__ void sts128(uint32_t smem_addr, const uint32_t (&v)[4]) {
+  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(smem_addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]) : "memory");
+}
+// Orders this thread's earlier shared-memory stores (generic proxy) before later reads of the async proxy: a wgmma
+// whose descriptor points at a tile that threads wrote themselves, not TMA.  Followed by a barrier among the writers.
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
 // Byte offset of fp32 element (row r, column c < 32) in a tile of 128-byte rows written by TMA with
 // CU_TENSOR_MAP_SWIZZLE_128B into a 1024-byte aligned buffer: the 16-byte chunk index is XOR-ed with (r & 7).
 __device__ __forceinline__ uint32_t swz128(int r, int c) {
@@ -131,7 +139,7 @@ __device__ __forceinline__ void mma_3xtf32(float (&main)[4], float (&corr)[4], c
 }
 
 // ---- warpgroup tf32 MMA (wgmma), A from registers -------------------------------------------
-// Shared-memory descriptor of a K-major operand tile written by TMA with the 128-byte swizzle: rows of 128 B (32 fp32
+// Shared-memory descriptor of a K-major operand tile in the 128-byte swizzle layout (as TMA writes it): rows of 128 B (32 fp32
 // of K), 8-row swizzle atoms 1024 B apart (stride byte offset), leading byte offset unused for a swizzled K-major tile.
 // The k8 slice ks of a tile starts 32*ks bytes into the tile (the hardware applies the swizzle to the full address).
 __device__ __forceinline__ uint64_t wgmma_desc_k128(uint32_t smem_addr) {

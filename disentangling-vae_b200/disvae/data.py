@@ -157,6 +157,34 @@ class DeviceLoader:
     def __len__(self):
         return len(self.windows)
 
+    def in_order(self, batch_size):
+        """A view of the same resident data that yields every item once, in index order, in batches of `batch_size`
+        (the last one shorter): what `DataLoader(self.dataset, batch_size, shuffle=False)` yields, for evaluation.
+        It is never sharded, and iterating it leaves this loader's epoch and seed as they are."""
+        return InOrder(self, batch_size)
+
+
+class InOrder:
+    """DeviceLoader.in_order(batch_size): iterating yields (images fp32 [b, C, H, W], dataset indices int64 [b]) on the
+    device for the windows `batch_windows(n, batch_size)`, gathered from the parent's uint8 tensor (no copy of it);
+    `len()` is ceil(n / batch_size) and `.dataset` the parent's dataset."""
+
+    def __init__(self, parent, batch_size):
+        self.batch_size = int(batch_size)
+        if self.batch_size < 1:
+            raise ValueError("DeviceLoader.in_order: batch_size must be positive, got %d" % self.batch_size)
+        self.parent, self.dataset = parent, parent.dataset
+        self.windows = batch_windows(parent.n, self.batch_size)
+
+    def __iter__(self):
+        order = torch.arange(self.parent.n, dtype=torch.int64, device=self.parent.device)
+        for start, size in self.windows:
+            idx = order[start:start + size]
+            yield ops.gather_u8_to_f32(self.parent.data, idx), idx
+
+    def __len__(self):
+        return len(self.windows)
+
 
 def device_loader_for(loader, device=None):
     """The DeviceLoader that stands in for a torch DataLoader: same dataset, batch size, shuffling and drop_last."""

@@ -4,8 +4,11 @@ same pairwise Gaussian log-density pattern as the beta-TCVAE kernel -- in `dv_la
 materialised [N, D, 10] tensors per call (SURVEY.md 8f-4).  Everything else (index bookkeeping, the two metric
 formulas on a [n_factors, latent_dim] table) is host code that mirrors the reference line for line, quirks included.
 """
+import contextlib
+import inspect
 import logging
 import os
+import tempfile
 from collections import defaultdict
 from functools import reduce
 from timeit import default_timer
@@ -14,11 +17,78 @@ import torch
 from tqdm import tqdm
 
 from disvae import _native as N
+from disvae.parallel import is_distributed
 from disvae.utils.modelIO import save_metadata
 
 TEST_LOSSES_FILE = "test_losses.log"
 METRICS_FILENAME = "metrics.log"
 METRIC_HELPERS_FILE = "metric_helpers.pth"
+EVAL_SEED_STRIDE = 0x9E3779B97F4A7C15      # odd 64-bit constant: consecutive epochs get unrelated seeds
+
+
+def epoch_metrics_filenames(epoch):
+    """(`metrics-{epoch}.log`, `metric_helpers-{epoch}.pth`): the metrics written after training epoch `epoch`."""
+    return "metrics-{}.log".format(epoch), "metric_helpers-{}.pth".format(epoch)
+
+
+def evaluation_seed(noise_key, epoch):
+    """Seed of the device generator for the evaluation of a run's model after epoch `epoch` (numbered from 0, as in
+    `model-{epoch}.pt`): (noise_key + EVAL_SEED_STRIDE * (epoch + 1)) mod 2**64, where `noise_key` is the Philox key of
+    the run's reparameterisation noise (`training_state()["noise"]["key"]`).  Nothing else enters it."""
+    return (int(noise_key) + EVAL_SEED_STRIDE * (int(epoch) + 1)) & 0xFFFFFFFFFFFFFFFF
+
+
+@contextlib.contextmanager
+def evaluation_rng(device, noise_key, epoch):
+    """Inside: `device`'s default CUDA generator is seeded with `evaluation_seed(noise_key, epoch)`, which the
+    estimator's index draws (`torch.randperm`) read.  On exit the CPU generator and that CUDA generator are back in the
+    state they had before."""
+    device = torch.device(device)
+    index = torch.cuda.current_device() if device.index is None else device.index
+    with torch.random.fork_rng(devices=[index]):
+        torch.cuda.default_generators[index].manual_seed(evaluation_seed(noise_key, epoch))
+        yield
+
+
+def check_resident_metrics(loader, metrics_batch_size, device_data):
+    """ValueError unless MIG / AAM can be computed from `loader`'s resident data: a DeviceLoader (or a torch DataLoader
+    that `device_data` converts to one) over a dataset with `lat_sizes` and `lat_names` and at least the estimator's
+    n_samples items, in one process.  No GPU work."""
+    from disvae.data import DeviceLoader
+    if is_distributed():
+        raise ValueError("metrics_every is not supported under torch.distributed; evaluate the saved checkpoints "
+                         "with an Evaluator in one process instead")
+    if isinstance(loader, torch.utils.data.DataLoader):
+        if not device_data:
+            raise ValueError("metrics_every needs the dataset resident on the GPU: pass a disvae.data.DeviceLoader or "
+                             "set DISVAE_DEVICE_DATA=1 (evaluating through the host DataLoader every few epochs costs "
+                             "more than the epochs themselves)")
+    elif not isinstance(loader, DeviceLoader):
+        raise ValueError("metrics_every needs a disvae.data.DeviceLoader, got %s" % type(loader).__name__)
+    ds = loader.dataset
+    if not (hasattr(ds, "lat_sizes") and hasattr(ds, "lat_names")):
+        raise ValueError("metrics_every: the dataset %s has no lat_sizes / lat_names (known factors of variation), "
+                         "which MIG and AAM need" % type(ds).__name__)
+    n_samples = inspect.signature(Evaluator._estimate_latent_entropies).parameters["n_samples"].default
+    if len(ds) < n_samples:
+        raise ValueError("metrics_every: the dataset has %d items, fewer than the %d samples the entropy estimator "
+                         "draws" % (len(ds), n_samples))
+    if int(metrics_batch_size) < 1:
+        raise ValueError("metrics_batch_size must be positive, got %d" % int(metrics_batch_size))
+
+
+def write_epoch_metrics(model, loader, epoch, batch_size, save_dir, logger):
+    """MIG / AAM of `model` over `loader.in_order(batch_size)` (a DeviceLoader) into `save_dir` as
+    `epoch_metrics_filenames(epoch)`, with the index draws seeded by `evaluation_rng(.., model's noise key, epoch)`.
+    The model's train / eval mode is kept."""
+    device = loader.device
+    key = model._noise_state(device)[0]           # fixed at the first training step; this fixes it the same way
+    metrics_file, helpers_file = epoch_metrics_filenames(epoch)
+    with tempfile.TemporaryDirectory(dir=save_dir) as tmp, evaluation_rng(device, key, epoch):
+        Evaluator(model, None, device=device, logger=logger, save_dir=tmp, is_progress_bar=False)(
+            loader.in_order(batch_size), is_metrics=True, is_losses=False)
+        os.replace(os.path.join(tmp, METRICS_FILENAME), os.path.join(save_dir, metrics_file))
+        os.replace(os.path.join(tmp, METRIC_HELPERS_FILE), os.path.join(save_dir, helpers_file))
 
 
 class Evaluator:

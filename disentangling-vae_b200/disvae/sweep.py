@@ -30,11 +30,12 @@ import torch
 
 from disvae import ops
 from disvae.data import DeviceLoader, device_loader_for
+from disvae.evaluate import Evaluator, check_resident_metrics, evaluation_rng, write_epoch_metrics
 from disvae.fused import FusedAdam
 from disvae.models.losses import permutation_key
 from disvae.models.vae import noise_key
 from disvae.parallel import is_distributed
-from disvae.training import Trainer, _EpochTally, apply_loader_state, check_loader_state
+from disvae.training import Trainer, _EpochTally, apply_loader_state, check_loader_state, check_metrics_every
 
 _tokens = itertools.count()          # ops.owner tokens: one per Trainer that ever joined a sweep
 
@@ -83,6 +84,7 @@ class Sweep:
         self.img_size = img
         self._inputs = {}                 # kept across calls: the members' captured graphs read these buffers
         self._device_loaders = {}         # id(DataLoader) -> (DataLoader, its DeviceLoader), converted once
+        self.loader = None                # the DeviceLoader of the latest call (what `evaluate` reads)
         self.streams = None               # one per member, made at the first call
         devs = {self._cuda_device(k, m) for k, m in enumerate(self.members)}
         if len(devs) > 1:
@@ -128,22 +130,47 @@ class Sweep:
             entry = self._device_loaders[id(data_loader)] = (data_loader, device_loader_for(data_loader, self.device))
         return entry[1]
 
-    def __call__(self, data_loader, epochs=10, checkpoint_every=10, save_state=False):
+    def __call__(self, data_loader, epochs=10, checkpoint_every=10, save_state=False, metrics_every=0,
+                 metrics_batch_size=1000):
         """Train every member for `epochs` epochs over `data_loader` (a DeviceLoader, or a DataLoader converted to one
         once per Sweep), like `Trainer.__call__` for each.  Calling again continues as a lone Trainer called again
         does: step counters, Adam state, Philox counters and the loader's epochs carry on.  `save_state=True` writes
-        each member's training state into its own save_dir; members that loaded one continue from it."""
+        each member's training state into its own save_dir; members that loaded one continue from it.
+        `metrics_every` writes each member's `metrics-{epoch}.log` as `Trainer.__call__` does, one member after
+        another on the caller's stream, over the one resident copy."""
         first, loader_state = self._resume()
         if loader_state is not None:
             check_loader_state(loader_state, data_loader, device_data=True)
+        check_metrics_every(metrics_every)
+        if metrics_every:
+            check_resident_metrics(data_loader, metrics_batch_size, device_data=True)
         loader = self._loader(data_loader)
         for m in self.members:
             m._resume = None
         if loader_state is not None:
             apply_loader_state(loader_state, loader)
+        self.loader = loader
         start = default_timer()
         with torch.cuda.device(self.device):
-            self._run(loader, first, epochs, checkpoint_every, save_state, start)
+            self._run(loader, first, epochs, checkpoint_every, save_state, start, metrics_every, metrics_batch_size)
+
+    def evaluate(self, is_metrics=True, is_losses=True, batch_size=1000):
+        """Every member's `Evaluator(...)(loader.in_order(batch_size), is_metrics, is_losses)` over the loader of the
+        latest call, into its save_dir (`metrics.log`, `metric_helpers.pth`, `test_losses.log`, as `main.py
+        --is-eval-only` writes them), with the index draws seeded as the metrics after its latest epoch
+        (`disvae.evaluate.evaluation_rng`); its `metrics.log` equals that epoch's `metrics-{epoch}.log`."""
+        if self.loader is None:
+            raise ValueError("Sweep.evaluate: the sweep has no loader yet; train it first (sweep(loader, ...))")
+        if is_metrics:
+            check_resident_metrics(self.loader, batch_size, device_data=True)
+        elif int(batch_size) < 1:
+            raise ValueError("Sweep.evaluate: batch_size must be positive, got %d" % int(batch_size))
+        with torch.cuda.device(self.device):
+            for m in self.members:
+                with evaluation_rng(self.device, m.model._noise_state(self.device)[0], m._next_epoch - 1):
+                    Evaluator(m.model, m.loss_f, device=self.device, logger=m.logger, save_dir=m.save_dir,
+                              is_progress_bar=m.is_progress_bar)(self.loader.in_order(batch_size), is_metrics=is_metrics,
+                                                                 is_losses=is_losses)
 
     def _resume(self):
         """(first epoch, saved loader state) of the members' loaded training states, (0, None) if none has one.
@@ -170,7 +197,7 @@ class Sweep:
         with torch.cuda.stream(self.streams[k]), ops.owner(self.members[k]._sweep_token):
             yield
 
-    def _run(self, loader, first, epochs, checkpoint_every, save_state, start):
+    def _run(self, loader, first, epochs, checkpoint_every, save_state, start, metrics_every, metrics_batch_size):
         members = self.members
         main = torch.cuda.current_stream(self.device)
         if self.streams is None:
@@ -222,6 +249,11 @@ class Sweep:
                                      save_state=save_state and (epoch % checkpoint_every == 0 or epoch == last))
                         done[k] = torch.cuda.Event()
                         done[k].record()
+                if metrics_every and (epoch % metrics_every == 0 or epoch == last):
+                    for ev in done:                                # every member has ended the epoch
+                        main.wait_event(ev)
+                    for m in members:                              # the next gather, on `main`, waits for these
+                        write_epoch_metrics(m.model, loader, epoch, metrics_batch_size, m.save_dir, m.logger)
         finally:
             for ev in done:
                 if ev is not None:

@@ -21,6 +21,7 @@ import torch.distributed as dist
 from tqdm import trange
 
 from disvae import _native
+from disvae.evaluate import check_resident_metrics, write_epoch_metrics
 from disvae.fused import FusedAdam
 from disvae.models.losses import DeviceLossLog
 from disvae.parallel import GradAverage, broadcast_parameters, is_distributed
@@ -71,14 +72,20 @@ class Trainer():
         self._steps_at_load = 0                   # n_train_steps a loaded state restored
         self.logger.info("Training Device: {}".format(self.device))
 
-    def __call__(self, data_loader, epochs=10, checkpoint_every=10, save_state=False):
+    def __call__(self, data_loader, epochs=10, checkpoint_every=10, save_state=False, metrics_every=0,
+                 metrics_batch_size=1000):
         """training.py:64-102.  `save_state=True` also writes the training state (`training_state_filename`) next to
         every checkpoint and after the last epoch.  After `load_training_state` the epochs are numbered on from the
-        saved one and the loader continues the saved data order."""
+        saved one and the loader continues the saved data order.  `metrics_every=k > 0` writes MIG / AAM of the model
+        (`metrics-{epoch}.log`, `metric_helpers-{epoch}.pth`) after every epoch divisible by k and after the last one,
+        computed from the loader's resident data (`disvae.evaluate.write_epoch_metrics`); training itself is unchanged."""
         start = default_timer()
         first, loader_state = (0, None) if self._resume is None else self._resume
         if loader_state is not None:
             check_loader_state(loader_state, data_loader, self.device_data)
+        check_metrics_every(metrics_every)
+        if metrics_every:
+            check_resident_metrics(data_loader, metrics_batch_size, self.device_data)
         self._resume = None
         if self.device_data and isinstance(data_loader, torch.utils.data.DataLoader):
             data_loader = self._device_loader(data_loader)
@@ -86,11 +93,14 @@ class Trainer():
             apply_loader_state(loader_state, data_loader)
         self._data_loader = data_loader
         self.model.train()
+        last = first + epochs - 1
         for epoch in range(first, first + epochs):
             storer = defaultdict(list)
             mean_epoch_loss = self._train_epoch(data_loader, storer, epoch)
             self._end_epoch(epoch, storer, mean_epoch_loss, checkpoint_every,
-                            save_state=save_state and (epoch % checkpoint_every == 0 or epoch == first + epochs - 1))
+                            save_state=save_state and (epoch % checkpoint_every == 0 or epoch == last))
+            if metrics_every and (epoch % metrics_every == 0 or epoch == last):
+                write_epoch_metrics(self.model, data_loader, epoch, metrics_batch_size, self.save_dir, self.logger)
         self._end_training(start)
 
     def _end_epoch(self, epoch, storer, mean_epoch_loss, checkpoint_every, save_state=False):
@@ -498,6 +508,11 @@ def check_loader_state(saved, loader, device_data=False):
         if want != got:
             raise ValueError("training state: the loader's {} is {!r} in the saved state but {!r} here".format(
                 field, want, got))
+
+
+def check_metrics_every(metrics_every):
+    if isinstance(metrics_every, bool) or not isinstance(metrics_every, int) or metrics_every < 0:
+        raise ValueError("metrics_every must be a non-negative integer (0: no metrics), got %r" % (metrics_every,))
 
 
 def apply_loader_state(saved, loader):

@@ -56,6 +56,9 @@ SIGNATURES = {
     "dv_btcvae_bwd": (I, [I, I, LL, I, P, P, P, P, P, P, P]),
     "dv_btcvae_fwd_rows": (I, [P, P, P, I, I, I, I, I, I, LL, I, P, P, P, P]),
     "dv_btcvae_bwd_rows": (I, [I, I, I, I, LL, I, P, P, P, P, P, P, P]),
+    "dv_dip_workspace_bytes": (SZ, [I, I]),
+    "dv_dip_fwd": (I, [P, P, I, I, I, I, I, P, P, P]),
+    "dv_dip_bwd": (I, [P, P, I, I, I, I, I, P, P, P, P, P]),
     "dv_u8_to_f32": (I, [P, P, LL, P]),
     "dv_gather_u8_to_f32": (I, [P, P, I, I, P, P]),
     "dv_loss_combine_fwd": (I, [P, P, I, P, P, I, P, P]),

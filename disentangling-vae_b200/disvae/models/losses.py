@@ -1,6 +1,6 @@
 """Disentanglement losses with the reference's API (disvae/models/losses.py) on the sm_90a
 kernels: one fused reconstruction+KL kernel (ops.VaeLossFn), the beta-TCVAE decomposition kernel
-(ops.BtcvaeFn) and the FactorVAE heads.  Logged scalars are fetched with ONE device->host copy
+(ops.BtcvaeFn), the FactorVAE heads and, beyond the reference, the DIP-VAE covariance penalty (ops.DipFn).  Logged scalars are fetched with ONE device->host copy
 per recorded step instead of one `.item()` per value (losses.py:151,384-389,447,476-478).
 """
 import abc
@@ -13,6 +13,7 @@ from disvae._native import DIST
 from .discriminator import Discriminator
 
 LOSSES = ["VAE", "betaH", "betaB", "factor", "btcvae"]
+DIP_LOSSES = ["dipI", "dipII"]      # not in LOSSES (the reference's `main.py -l` choices): reachable from Python
 RECON_DIST = ["bernoulli", "laplace", "gaussian"]
 
 
@@ -33,6 +34,9 @@ def get_loss_f(loss_name, **kwargs_parse):
     elif loss_name == "btcvae":
         return BtcvaeLoss(kwargs_parse["n_data"], alpha=kwargs_parse["btcvae_A"], beta=kwargs_parse["btcvae_B"],
                           gamma=kwargs_parse["btcvae_G"], **kwargs_all)
+    elif loss_name in DIP_LOSSES:
+        return DipVAELoss(loss_name[len("dip"):], lambda_od=kwargs_parse.get("dip_lambda_od", 10.),
+                          lambda_d=kwargs_parse.get("dip_lambda_d"), **kwargs_all)
     else:
         assert loss_name not in LOSSES
         raise ValueError("Uknown loss : {}".format(loss_name))
@@ -208,10 +212,11 @@ class BaseLoss(abc.ABC):
         return self._log.spec(self.record_loss_every, names, values)
 
     def _combine(self, out, b, coef_a, coef_b, annealed, is_train, log):
-        """ops.LossCombineSchedFn: coefficient number `annealed` (coef_a, then coef_b) is multiplied by
-        linear_annealing(0, 1, step, steps_anneal) on the device."""
+        """ops.LossCombineSchedFn: coefficient number `annealed` (coef_a, then coef_b; or each number of a tuple) is
+        multiplied by linear_annealing(0, 1, step, steps_anneal) on the device."""
         step = self._step_counter(out.device, True) if is_train else None
-        loss, _ = ops.LossCombineSchedFn.apply(out, b, coef_a, coef_b, 1 << annealed, (0, 1, self.steps_anneal),
+        mask = sum(1 << k for k in annealed) if isinstance(annealed, tuple) else 1 << annealed
+        loss, _ = ops.LossCombineSchedFn.apply(out, b, coef_a, coef_b, mask, (0, 1, self.steps_anneal),
                                                is_train, step, log)
         return loss
 
@@ -433,6 +438,42 @@ class BtcvaeLoss(BaseLoss):
         # rec + (alpha*mi + beta*tc + anneal*gamma*dw_kl) as one launch (the kl entries of `out` only feed the log)
         loss = self._combine(out, terms, [1.0], [self.alpha, self.beta, self.gamma], 3, is_train, log)
         _record(storer, names, [rec_loss, loss, mi_loss, tc_loss, dw_kl_loss, kl_loss, kl_dims])
+        return loss
+
+
+class DipVAELoss(BaseLoss):
+    """DIP-VAE-I / DIP-VAE-II (Kumar et al. 2018, eq. 6 and section 3; not in the reference):
+    rec + kl + anneal * (lambda_od * od + lambda_d * dd) with od = sum_{i != j} C_ij^2, dd = sum_i (C_ii - 1)^2 and
+    C = Cov_mu (dip_type "I") or Cov_mu + diag(mean exp(logvar)) ("II"), the biased covariance of the batch's encoder
+    means (ops.DipFn).  lambda_d=None takes the ratios of Locatello et al. 2019: 10 * lambda_od for I, lambda_od for II.
+    Under torch.distributed the penalty is that of each rank's shard (the gradient average follows it)."""
+
+    def __init__(self, dip_type="I", lambda_od=10., lambda_d=None, **kwargs):
+        import math
+        import numbers
+        if dip_type not in ops.DIP_TYPES:
+            raise ValueError("Unknown DIP-VAE type {!r}: expected one of {}".format(dip_type, sorted(ops.DIP_TYPES)))
+        if lambda_d is None and isinstance(lambda_od, numbers.Real):
+            lambda_d = 10. * lambda_od if dip_type == "I" else lambda_od
+        for name, v in (("lambda_od", lambda_od), ("lambda_d", lambda_d)):
+            if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v) or v < 0:
+                raise ValueError("DIP-VAE {} must be a finite number >= 0, got {!r}".format(name, v))
+        super().__init__(**kwargs)
+        self.dip_type = dip_type
+        self.lambda_od = float(lambda_od)
+        self.lambda_d = float(lambda_d)
+
+    def __call__(self, data, recon_batch, latent_dist, is_train, storer, **kwargs):
+        storer = self._pre_call(is_train, storer)
+        out = self._rec_kl_vec(data, recon_batch, latent_dist)
+        rec_loss, kl_loss, kl_dims = out[0], out[1], out[2:]
+        terms = ops.dip_terms(latent_dist[0], latent_dist[1], self.dip_type)
+        od, dd = terms[0], terms[1]
+        names = ['recon_loss', 'kl_loss', _kl_names(kl_dims.numel()), 'dip_od_loss', 'dip_d_loss', 'loss']
+        log = self._log_spec(is_train, names, [rec_loss, kl_loss, kl_dims, od, dd, None])
+        # rec + kl + anneal * (lambda_od * od + lambda_d * dd) as one launch
+        loss = self._combine(out, terms, [1.0, 1.0], [self.lambda_od, self.lambda_d], (2, 3), is_train, log)
+        _record(storer, names, [rec_loss, kl_loss, kl_dims, od, dd, loss])
         return loss
 
 

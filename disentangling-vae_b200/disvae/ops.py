@@ -770,6 +770,52 @@ def btcvae_terms(z, mu, logvar, n_data, is_mss):
     return terms
 
 
+# ---------------------------------------------------------------------------------------
+# DIP-VAE covariance penalty (Kumar et al. 2018, eq. 6 and section 3; include/disvae_b200.h)
+# ---------------------------------------------------------------------------------------
+DIP_TYPES = {"I": 1, "II": 2}       # DV_DIP_I, DV_DIP_II
+
+
+class DipFn(Function):
+    """-> terms[2] = (od, dd), the unweighted off-diagonal and diagonal penalties on C = Cov_mu (DIP-VAE-I) or
+    Cov_mu + diag(mean exp(logvar)) (DIP-VAE-II).  The workspace, fresh for every call, carries the column means and C
+    from forward to backward.  No logvar gradient for DIP-VAE-I (the term does not depend on it)."""
+
+    @staticmethod
+    def forward(ctx, mu, logvar, dip_type):
+        N.require_cuda_f32(mu, logvar)
+        mu, logvar, ld, rs = _mu_logvar(mu, logvar)
+        B, D = mu.shape
+        t = DIP_TYPES[dip_type]
+        ws = torch.empty((N.lib().dv_dip_workspace_bytes(B, D) + 3) // 4, dtype=torch.float32, device=mu.device)
+        terms = _new((2,), mu)
+        call("dv_dip_fwd", ptr(mu), ptr(logvar), ld, rs, B, D, t, ptr(terms), ptr(ws), stream())
+        ctx.meta = (B, D, ld, rs, t)
+        ctx.save_for_backward(mu, logvar, ws)
+        return terms
+
+    @staticmethod
+    def backward(ctx, g_terms):
+        mu, logvar, ws = ctx.saved_tensors
+        B, D, ld, rs, t = ctx.meta
+        g_terms = _c(g_terms)
+        g_mu = _new((B, D), mu) if ctx.needs_input_grad[0] else None
+        g_lv = _new((B, D), mu) if ctx.needs_input_grad[1] and t == DIP_TYPES["II"] else None
+        call("dv_dip_bwd", ptr(mu), ptr(logvar), ld, rs, B, D, t, ptr(g_terms), ptr(g_mu), ptr(g_lv), ptr(ws), stream())
+        return g_mu, g_lv, None
+
+
+def dip_terms(mu, logvar, dip_type):
+    """DipFn on the MAIN stream.  btcvae_terms moves its node to the weight-gradient side stream because its backward
+    is long and its results are first needed by the encoder's backward.  Neither half of this node gains from that: the
+    forward's terms are needed at once by the loss combination, and the backward is one short launch (~5 us at the c2
+    shape) that the long decoder backward cannot hide much of.  On the side stream the node adds a branch to the
+    captured step graph, and at c2 the replay then started the decoder's first weight-gradient kernel ahead of the
+    input-gradient chain: one replayed step took 2136 us against betaH's 2080 us on an H100.  On the main stream it took
+    2090 us against 2087 us (DESIGN.md section 4)."""
+    return DipFn.apply(mu, logvar, dip_type)
+
+
 class LossCombineFn(Function):
     """loss = sum_i coef_a[i]*a[i] + sum_j coef_b[j]*b[j] with a = the fused loss kernel's output (rec, kl, per-dim kl..:
     only the first len(coef_a) entries are weighted) and b = a short vector or 0-dim tensor (beta-TCVAE terms, the

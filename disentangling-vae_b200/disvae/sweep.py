@@ -4,7 +4,8 @@
     Sweep(members, seeds=[seed_k ...])(loader, epochs=30, checkpoint_every=10)
 
 Every member is an ordinary `Trainer` and keeps its own model, optimizer, loss, save_dir, train_losses.log,
-checkpoints, GIF visualizer and progress output.  All members read the same batches in the same order: one
+checkpoints, GIF visualizer and progress output.  A member's loss may be any of `losses.LOSSES` (VAE, betaH, betaB,
+factor, btcvae) or `losses.DIP_LOSSES` (dipI, dipII), with its own hyper-parameters.  All members read the same batches in the same order: one
 `DeviceLoader` permutation per epoch and one gather per step, into one buffer that every member's captured graph reads.
 Each member runs on its own stream (its two eager warm-up steps, its capture, then one graph replay per step), so the
 replays of different members overlap on the GPU; the next gather waits for all of them.

@@ -215,6 +215,31 @@ int dv_btcvae_bwd_rows(int B, int D, int row0, int nrows, long long n_data, int 
                        const float* rowstats, const void* workspace, const float* g_terms, float* g_z,
                        float* g_mu, float* g_logvar, void* stream);
 
+/* ---- DIP-VAE covariance penalty ----------------------------------------------------------------
+ * The reference has no DIP-VAE: these implement Kumar et al. 2018 ("Variational Inference of Disentangled Latent
+ * Concepts from Unlabeled Observations"), the regulariser of eq. 6 (DIP-VAE-I) and of the second form in section 3
+ * (DIP-VAE-II), on the batch of encoder outputs mu / logvar [B, D] (element (b, d) at b*row_stride + d*ld, as for
+ * dv_vae_loss_fwd: the interleaved encoder output is read in place):
+ *   Cov_mu = (1/B) sum_b (mu_b - m)(mu_b - m)^T   (biased; centred two-pass form, m = mu_0 + mean_b(mu_b - mu_0))
+ *   C = Cov_mu (DV_DIP_I)  or  Cov_mu + diag(mean_b exp(logvar_b)) (DV_DIP_II)
+ *   terms_out[0] = od = sum_{i != j} C_ij^2,   terms_out[1] = dd = sum_i (C_ii - 1)^2   (unweighted)
+ * The weights lambda_od, lambda_d and the annealing are applied by the caller (dv_loss_combine_sched_fwd).
+ * workspace: dv_dip_workspace_bytes(B, D) bytes, 16-byte aligned, contents irrelevant on entry; the forward leaves the
+ * column means and C in it for dv_dip_bwd, so pass the SAME workspace untouched.  Deterministic (fixed-order
+ * reductions, no floating-point atomics).  logvar is read only by DV_DIP_II but must be a valid pointer for both.
+ * DV_ERR_BAD_SHAPE: B < 1, D < 1, D > 1024 or dip_type not DV_DIP_I / DV_DIP_II.
+ * DV_ERR_BAD_ARG: a NULL required pointer, or mu / logvar / terms / gradients not 4-byte or workspace not 16-byte aligned.
+ * Backward: g_terms = device float[2], the upstream gradient of (od, dd) (the lambdas and the annealing included);
+ *   g_mu[b] = (2/B) G (mu_b - m) with G_ij = 2 g_terms[0] C_ij (i != j), G_ii = 2 g_terms[1] (C_ii - 1);
+ *   g_logvar[b][i] = G_ii exp(logvar[b][i]) / B for DV_DIP_II, 0 for DV_DIP_I.
+ *   Outputs contiguous [B, D]; either may be NULL (both NULL: nothing is launched). */
+enum { DV_DIP_I = 1, DV_DIP_II = 2 };
+size_t dv_dip_workspace_bytes(int B, int D);      /* 0 for an unsupported shape */
+int dv_dip_fwd(const float* mu, const float* logvar, int ld, int row_stride, int B, int D, int dip_type,
+               float* terms_out, void* workspace, void* stream);
+int dv_dip_bwd(const float* mu, const float* logvar, int ld, int row_stride, int B, int D, int dip_type,
+               const float* g_terms, float* g_mu, float* g_logvar, const void* workspace, void* stream);
+
 /* ---- input pipeline and step glue (SURVEY.md 8f-3, VERDICT r1 #8) -----------------------------
  * dv_u8_to_f32: dst[i] = src[i] / 255 (true division) -- torchvision ToTensor on the device, so host batches can be
  * uploaded as bytes (training.py:150; utils/datasets.py:182,247,364-367).  Both pointers 16-byte aligned.

@@ -23,12 +23,21 @@ from disvae.utils.modelIO import save_metadata
 TEST_LOSSES_FILE = "test_losses.log"
 METRICS_FILENAME = "metrics.log"
 METRIC_HELPERS_FILE = "metric_helpers.pth"
+FACTOR_SCORE_FILENAME = "factor_vae_score.log"
+FACTOR_SCORE_HELPERS_FILE = "factor_vae_score_helpers.pth"
+FACTOR_SCORE_MIN_VAR = 0.05                # a dim whose global variance is below this is inactive (factor_vae.py)
+FACTOR_SCORE_MAX_DIM = 1024                # dv_group_variance's limit
 EVAL_SEED_STRIDE = 0x9E3779B97F4A7C15      # odd 64-bit constant: consecutive epochs get unrelated seeds
 
 
 def epoch_metrics_filenames(epoch):
     """(`metrics-{epoch}.log`, `metric_helpers-{epoch}.pth`): the metrics written after training epoch `epoch`."""
     return "metrics-{}.log".format(epoch), "metric_helpers-{}.pth".format(epoch)
+
+
+def epoch_factor_score_filenames(epoch):
+    """(`factor_vae_score-{epoch}.log`, `factor_vae_score_helpers-{epoch}.pth`): the score after epoch `epoch`."""
+    return "factor_vae_score-{}.log".format(epoch), "factor_vae_score_helpers-{}.pth".format(epoch)
 
 
 def evaluation_seed(noise_key, epoch):
@@ -77,18 +86,149 @@ def check_resident_metrics(loader, metrics_batch_size, device_data):
         raise ValueError("metrics_batch_size must be positive, got %d" % int(metrics_batch_size))
 
 
-def write_epoch_metrics(model, loader, epoch, batch_size, save_dir, logger):
+def check_epoch_factor_score(factor_score, metrics_every, loader, latent_dim):
+    """ValueError unless the FactorVAE score can be written with the metrics of every `metrics_every` epochs (after
+    `check_resident_metrics` has accepted `loader`).  No GPU work."""
+    if not factor_score:
+        return
+    if not metrics_every:
+        raise ValueError("factor_score=True needs metrics_every > 0: the score is written with the metrics of those "
+                         "epochs")
+    check_factor_score(loader.dataset, latent_dim)
+
+
+def write_epoch_metrics(model, loader, epoch, batch_size, save_dir, logger, factor_score=False):
     """MIG / AAM of `model` over `loader.in_order(batch_size)` (a DeviceLoader) into `save_dir` as
     `epoch_metrics_filenames(epoch)`, with the index draws seeded by `evaluation_rng(.., model's noise key, epoch)`.
-    The model's train / eval mode is kept."""
+    `factor_score=True` also writes the FactorVAE score from the same encodings as `epoch_factor_score_filenames(epoch)`,
+    drawn with seed `evaluation_seed(model's noise key, epoch)`.  The model's train / eval mode is kept."""
     device = loader.device
     key = model._noise_state(device)[0]           # fixed at the first training step; this fixes it the same way
-    metrics_file, helpers_file = epoch_metrics_filenames(epoch)
+    moves = list(zip((METRICS_FILENAME, METRIC_HELPERS_FILE), epoch_metrics_filenames(epoch)))
+    score_args = {}
+    if factor_score:
+        moves += zip((FACTOR_SCORE_FILENAME, FACTOR_SCORE_HELPERS_FILE), epoch_factor_score_filenames(epoch))
+        score_args = {"is_factor_score": True, "factor_score_seed": evaluation_seed(key, epoch)}
     with tempfile.TemporaryDirectory(dir=save_dir) as tmp, evaluation_rng(device, key, epoch):
         Evaluator(model, None, device=device, logger=logger, save_dir=tmp, is_progress_bar=False)(
-            loader.in_order(batch_size), is_metrics=True, is_losses=False)
-        os.replace(os.path.join(tmp, METRICS_FILENAME), os.path.join(save_dir, metrics_file))
-        os.replace(os.path.join(tmp, METRIC_HELPERS_FILE), os.path.join(save_dir, helpers_file))
+            loader.in_order(batch_size), is_metrics=True, is_losses=False, **score_args)
+        for src, dst in moves:
+            os.replace(os.path.join(tmp, src), os.path.join(save_dir, dst))
+
+
+# ---- FactorVAE score (Kim & Mnih 2018, section 4; the conventions of disentanglement_lib's factor_vae.py) ----------
+def check_factor_score(dataset, latent_dim, batch_size=64, num_train=10000, num_eval=5000,
+                       num_variance_estimate=10000):
+    """ValueError unless the FactorVAE score can be computed over `dataset` for a `latent_dim` model with these
+    settings: the dataset has known factors (`lat_sizes`, `lat_names`), is their full grid, and has a factor of more
+    than one value.  No GPU work.  Returns lat_sizes as a list of ints."""
+    if not (hasattr(dataset, "lat_sizes") and hasattr(dataset, "lat_names")):
+        raise ValueError("FactorVAE score: the dataset %s has no lat_sizes / lat_names (known factors of variation)"
+                         % type(dataset).__name__)
+    return _check_factor_grid(dataset.lat_sizes, len(dataset), latent_dim, batch_size, num_train, num_eval,
+                              num_variance_estimate)
+
+
+def _check_factor_grid(lat_sizes, n, latent_dim, batch_size, num_train, num_eval, num_variance_estimate):
+    lat_sizes = [int(s) for s in lat_sizes]
+    if n != reduce(lambda x, y: x * y, lat_sizes, 1):
+        raise ValueError("FactorVAE score: the dataset has %d items, not the %d of the full grid of its factors %s"
+                         % (n, reduce(lambda x, y: x * y, lat_sizes, 1), lat_sizes))
+    if all(s == 1 for s in lat_sizes):
+        raise ValueError("FactorVAE score: every factor of %s has one value; there is nothing to vote on" % lat_sizes)
+    for name, value, least in (("batch_size", batch_size, 2), ("num_train", num_train, 1), ("num_eval", num_eval, 1),
+                               ("num_variance_estimate", num_variance_estimate, 2)):
+        if int(value) < least:
+            raise ValueError("FactorVAE score: %s must be at least %d, got %d" % (name, least, int(value)))
+    if int(latent_dim) > FACTOR_SCORE_MAX_DIM:
+        raise ValueError("FactorVAE score: latent_dim %d is above the kernel's limit of %d"
+                         % (int(latent_dim), FACTOR_SCORE_MAX_DIM))
+    return lat_sizes
+
+
+def factor_vote_rows(lat_sizes, num_votes, batch_size, generator):
+    """(factor [num_votes], rows [num_votes, batch_size]) of `num_votes` votes, drawn from `generator` on its device:
+    one randint for the factor of every vote (among the factors of more than one value), then one randint per factor k,
+    k = 0 .. K-1 in order (size-1 factors included), for the [num_votes, batch_size] values of factor k.  Factor k of
+    a vote on k takes row 0's value in every row.  Rows are the C-order grid indices, the last factor fastest; each
+    value is below its factor's size, so every row is in [0, prod(lat_sizes))."""
+    device = generator.device
+    varying = torch.tensor([k for k, s in enumerate(lat_sizes) if s > 1], dtype=torch.int64, device=device)
+    factor = varying[torch.randint(len(varying), (num_votes,), generator=generator, device=device)]
+    rows = torch.zeros(num_votes, batch_size, dtype=torch.int64, device=device)
+    stride = 1
+    strides = []
+    for s in reversed(lat_sizes):
+        strides.insert(0, stride)
+        stride *= s
+    for k, s in enumerate(lat_sizes):
+        values = torch.randint(s, (num_votes, batch_size), generator=generator, device=device)
+        values = torch.where((factor == k).unsqueeze(1), values[:, :1], values)
+        rows += values * strides[k]
+    return factor, rows
+
+
+def group_variance(mu, rows, global_var=None, var_out=None, argmin_out=None):
+    """`dv_group_variance` on `mu` [N, D] (any strides, a view of q_zCx included) and int64 `rows` [V, L]: the
+    unbiased variance of every group into `var_out` [V, D], and / or into int32 `argmin_out` [V] the dim minimising
+    var / global_var over the dims with global_var >= FACTOR_SCORE_MIN_VAR."""
+    N.require_cuda_f32(mu, global_var, var_out)
+    n, d = mu.shape
+    V, L = rows.shape
+    if rows.dtype != torch.int64 or not rows.is_contiguous():
+        raise ValueError("group_variance: rows must be a contiguous int64 tensor")
+    N.call("dv_group_variance", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(rows), V, L, N.ptr(global_var),
+           FACTOR_SCORE_MIN_VAR, N.ptr(var_out), N.ptr(argmin_out), N.stream())
+
+
+def factor_vae_score(mu, lat_sizes, batch_size=64, num_train=10000, num_eval=5000, num_variance_estimate=10000,
+                     seed=0):
+    """FactorVAE score of the encoder means `mu` [N, D] (CUDA fp32, dataset index order) of the full factor grid
+    `lat_sizes` -> ({"train_accuracy", "eval_accuracy", "num_active_dims"}, helpers).  The draws come from a device
+    torch.Generator seeded with `seed`, in this order: the `num_variance_estimate` variance rows
+    (`torch.randint(N, (num_variance_estimate,))`), then `factor_vote_rows` for the training votes, then for the
+    evaluation votes; no vote is drawn when no dim is active.  The global generators are not touched."""
+    lat_sizes = _check_factor_grid(lat_sizes, mu.shape[0], mu.shape[1], batch_size, num_train, num_eval,
+                                   num_variance_estimate)
+    N.require_cuda_f32(mu)
+    n, D = mu.shape
+    K = len(lat_sizes)
+    gen = torch.Generator(device=mu.device)
+    gen.manual_seed(int(seed))
+    var_rows = torch.randint(n, (int(num_variance_estimate),), generator=gen, device=mu.device)
+    global_var = torch.empty(1, D, dtype=torch.float32, device=mu.device)
+    group_variance(mu, var_rows.view(1, -1), var_out=global_var)
+    global_var = global_var[0]
+    active = global_var >= FACTOR_SCORE_MIN_VAR
+    num_active = int(active.sum())
+    if num_active == 0:
+        train_votes = torch.zeros(K, D, dtype=torch.int64)
+        eval_votes = torch.zeros(K, D, dtype=torch.int64)
+    else:
+        train_factor, train_rows = factor_vote_rows(lat_sizes, int(num_train), int(batch_size), gen)
+        eval_factor, eval_rows = factor_vote_rows(lat_sizes, int(num_eval), int(batch_size), gen)
+        dims = torch.empty(int(num_train) + int(num_eval), dtype=torch.int32, device=mu.device)
+        group_variance(mu, torch.cat([train_rows, eval_rows]), global_var=global_var, argmin_out=dims)
+        cells = (torch.cat([train_factor, eval_factor]) * D + dims.long()).cpu()
+        train_votes = torch.bincount(cells[:num_train], minlength=K * D).view(K, D)
+        eval_votes = torch.bincount(cells[num_train:], minlength=K * D).view(K, D)
+    classifier, train_accuracy, eval_accuracy = factor_vote_accuracies(train_votes, eval_votes)
+    score = {"train_accuracy": train_accuracy, "eval_accuracy": eval_accuracy, "num_active_dims": num_active}
+    helpers = {"global_variances": global_var.cpu(), "active_dims": active.cpu(), "train_votes": train_votes,
+               "eval_votes": eval_votes, "classifier": classifier}
+    return score, helpers
+
+
+def factor_vote_accuracies(train_votes, eval_votes):
+    """(classifier [D], train accuracy, eval accuracy) of vote tables [K, D]: classifier[d] = argmax_k
+    train_votes[k, d], the lowest k on a tie; an accuracy is the share of a table's votes the classifier gets right."""
+    classifier = torch.argmax(train_votes, dim=0)
+    cols = torch.arange(train_votes.size(1))
+
+    def accuracy(votes):
+        total = int(votes.sum())
+        return int(votes[classifier, cols].sum()) / total if total else 0.0
+    return classifier, accuracy(train_votes), accuracy(eval_votes)
 
 
 class Evaluator:
@@ -103,18 +243,35 @@ class Evaluator:
         self._perm_queue = []         # injected sample indices (parity tests), consumed FIFO by _estimate_latent_entropies
         self.logger.info("Testing Device: {}".format(self.device))
 
-    def __call__(self, data_loader, is_metrics=False, is_losses=True):
+    def __call__(self, data_loader, is_metrics=False, is_losses=True, is_factor_score=False, factor_score_seed=0):
         """evaluate.py:59-96.  Like the reference, the first returned value is always None (it assigns the metrics to
-        a differently named variable, :77-79); the metrics are logged and written to metrics.log."""
+        a differently named variable, :77-79); the metrics are logged and written to metrics.log.
+        `is_factor_score=True` also writes the FactorVAE score (`compute_factor_vae_score` with its default settings
+        and `seed=factor_score_seed`) to factor_vae_score.log and its tables to factor_vae_score_helpers.pth; with
+        `is_metrics` the dataset is encoded once for both."""
         start = default_timer()
+        if is_factor_score:
+            check_factor_score(getattr(data_loader, "dataset", None), self.model.latent_dim)
         is_still_training = self.model.training
         self.model.eval()
         metric, losses = None, None
+        encoded = None
         if is_metrics:
             self.logger.info('Computing metrics...')
-            metrics = self.compute_metrics(data_loader)
+            lat_sizes, lat_names = self._known_factors(data_loader)
+            self.logger.info("Computing the empirical distribution q(z|x).")
+            encoded = self._compute_q_zCx(data_loader)
+            metrics = self._metrics_of(encoded, lat_sizes, lat_names)
             self.logger.info('Losses: {}'.format(metrics))
             save_metadata(metrics, self.save_dir, filename=METRICS_FILENAME)
+        if is_factor_score:
+            self.logger.info('Computing the FactorVAE score...')
+            if encoded is None:
+                encoded = self._compute_q_zCx(data_loader)
+            score, helpers = factor_vae_score(encoded[1][0], data_loader.dataset.lat_sizes, seed=factor_score_seed)
+            self.logger.info('FactorVAE score: {}'.format(score))
+            save_metadata(score, self.save_dir, filename=FACTOR_SCORE_FILENAME)
+            torch.save(helpers, os.path.join(self.save_dir, FACTOR_SCORE_HELPERS_FILE))
         if is_losses:
             self.logger.info('Computing losses...')
             losses = self.compute_losses(data_loader)
@@ -142,14 +299,31 @@ class Evaluator:
     # ---- MIG / AAM (evaluate.py:119-317) ------------------------------------------------------------------
     def compute_metrics(self, dataloader):
         """evaluate.py:119-161"""
+        lat_sizes, lat_names = self._known_factors(dataloader)
+        self.logger.info("Computing the empirical distribution q(z|x).")
+        return self._metrics_of(self._compute_q_zCx(dataloader), lat_sizes, lat_names)
+
+    def compute_factor_vae_score(self, dataloader, batch_size=64, num_train=10000, num_eval=5000,
+                                 num_variance_estimate=10000, seed=0):
+        """FactorVAE score (Kim & Mnih 2018, section 4) of the model's encoder means over `dataloader` (the dataset in
+        index order: DataLoader(shuffle=False) or DeviceLoader.in_order) -> {"train_accuracy", "eval_accuracy",
+        "num_active_dims"}; see `factor_vae_score` for the definition and the order of the draws."""
+        check_factor_score(getattr(dataloader, "dataset", None), self.model.latent_dim, batch_size, num_train, num_eval,
+                           num_variance_estimate)
+        mean = self._compute_q_zCx(dataloader)[1][0]
+        return factor_vae_score(mean, dataloader.dataset.lat_sizes, batch_size, num_train, num_eval,
+                                num_variance_estimate, seed)[0]
+
+    def _known_factors(self, dataloader):
         try:
-            lat_sizes = dataloader.dataset.lat_sizes
-            lat_names = dataloader.dataset.lat_names
+            return dataloader.dataset.lat_sizes, dataloader.dataset.lat_names
         except AttributeError:
             raise ValueError("Dataset needs to have known true factors of variations to compute the metric. This does not "
                              "seem to be the case for {}".format(type(dataloader.__dict__["dataset"]).__name__))
-        self.logger.info("Computing the empirical distribution q(z|x).")
-        samples_zCx, params_zCx = self._compute_q_zCx(dataloader)
+
+    def _metrics_of(self, encoded, lat_sizes, lat_names):
+        """MIG / AAM from `_compute_q_zCx`'s (samples, params)."""
+        samples_zCx, params_zCx = encoded
         len_dataset, latent_dim = samples_zCx.shape
 
         self.logger.info("Estimating the marginal entropy.")

@@ -318,6 +318,21 @@ size_t dv_latent_entropy_workspace_bytes(int N, int D, int S);
 int dv_latent_entropy(const float* zs, const float* mean, const float* logvar, int ld, int row_stride,
                       int N, int D, int S, float* H, float* logq_out, void* workspace, void* stream);
 
+/* ---- disentanglement metrics: FactorVAE score (Kim & Mnih 2018, section 4) ----------------------
+ * V groups of L gathered rows of mu [N, D] (element (n, d) at n*row_stride + d*ld, as dv_latent_entropy reads it; the
+ * interleaved q_zCx [N, D, 2] buffer is read in place).  rows: int64 [V][L], every entry in [0, N) (not checked: the
+ * caller builds them), repeats allowed.
+ *   var_out[g][d] = unbiased variance (ddof 1) of mu[rows[g][l]][d] over l, in the centred two-pass form around
+ *                   the group's first row (optional, [V][D])
+ *   argmin_out[g] = the d minimising var[g][d] / global_var[d] over the dims with global_var[d] >= min_var, the lowest
+ *                   d on a tie; -1 if no dim qualifies (optional, [V]; needs global_var [D])
+ * One launch, no workspace.  Deterministic (fixed-order reductions, no floating-point atomics), graph-capturable.
+ * DV_ERR_BAD_SHAPE: L < 2, V < 1, N < 1, D < 1 or D > 1024.
+ * DV_ERR_BAD_ARG: mu or rows NULL, both outputs NULL, argmin_out without global_var, or a pointer misaligned (rows
+ * 8 bytes, the others 4). */
+int dv_group_variance(const float* mu, int ld, int row_stride, int N, int D, const long long* rows, int V, int L,
+                      const float* global_var, float min_var, float* var_out, int* argmin_out, void* stream);
+
 /* ---- FactorVAE pieces ---------------------------------------------------------------------
  * dv_permute_dims replaces _permute_dims (losses.py:483-508): out[b][d] = z[perm[d][b]][d].
  * perms != NULL: int64 [D][B] (the reference's CPU randperm stream, trap T7).  perms == NULL:

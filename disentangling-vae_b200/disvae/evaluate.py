@@ -7,8 +7,10 @@ formulas on a [n_factors, latent_dim] table) is host code that mirrors the refer
 import contextlib
 import inspect
 import logging
+import math
 import os
 import tempfile
+import warnings
 from collections import defaultdict
 from functools import reduce
 from timeit import default_timer
@@ -27,6 +29,11 @@ FACTOR_SCORE_FILENAME = "factor_vae_score.log"
 FACTOR_SCORE_HELPERS_FILE = "factor_vae_score_helpers.pth"
 FACTOR_SCORE_MIN_VAR = 0.05                # a dim whose global variance is below this is inactive (factor_vae.py)
 FACTOR_SCORE_MAX_DIM = 1024                # dv_group_variance's limit
+SAP_SCORE_FILENAME = "sap_score.log"
+SAP_SCORE_HELPERS_FILE = "sap_score_helpers.pth"
+SAP_MAX_DIM = 1024                         # dv_sap_score_matrix's limits: latents,
+SAP_MAX_TRAIN = 32768                      # training rows staged in shared memory,
+SAP_MAX_CLASSES = 256                      # and values of a scored factor
 EVAL_SEED_STRIDE = 0x9E3779B97F4A7C15      # odd 64-bit constant: consecutive epochs get unrelated seeds
 
 
@@ -38,6 +45,11 @@ def epoch_metrics_filenames(epoch):
 def epoch_factor_score_filenames(epoch):
     """(`factor_vae_score-{epoch}.log`, `factor_vae_score_helpers-{epoch}.pth`): the score after epoch `epoch`."""
     return "factor_vae_score-{}.log".format(epoch), "factor_vae_score_helpers-{}.pth".format(epoch)
+
+
+def epoch_sap_score_filenames(epoch):
+    """(`sap_score-{epoch}.log`, `sap_score_helpers-{epoch}.pth`): the SAP score after epoch `epoch`."""
+    return "sap_score-{}.log".format(epoch), "sap_score_helpers-{}.pth".format(epoch)
 
 
 def evaluation_seed(noise_key, epoch):
@@ -97,18 +109,32 @@ def check_epoch_factor_score(factor_score, metrics_every, loader, latent_dim):
     check_factor_score(loader.dataset, latent_dim)
 
 
-def write_epoch_metrics(model, loader, epoch, batch_size, save_dir, logger, factor_score=False):
+def check_epoch_sap_score(sap_score, metrics_every, loader, latent_dim):
+    """ValueError unless the SAP score can be written with the metrics of every `metrics_every` epochs (after
+    `check_resident_metrics` has accepted `loader`).  No GPU work."""
+    if not sap_score:
+        return
+    if not metrics_every:
+        raise ValueError("sap_score=True needs metrics_every > 0: the score is written with the metrics of those epochs")
+    check_sap_score(loader.dataset, latent_dim)
+
+
+def write_epoch_metrics(model, loader, epoch, batch_size, save_dir, logger, factor_score=False, sap_score=False):
     """MIG / AAM of `model` over `loader.in_order(batch_size)` (a DeviceLoader) into `save_dir` as
     `epoch_metrics_filenames(epoch)`, with the index draws seeded by `evaluation_rng(.., model's noise key, epoch)`.
     `factor_score=True` also writes the FactorVAE score from the same encodings as `epoch_factor_score_filenames(epoch)`,
-    drawn with seed `evaluation_seed(model's noise key, epoch)`.  The model's train / eval mode is kept."""
+    and `sap_score=True` the SAP score as `epoch_sap_score_filenames(epoch)`, each drawn from its own generator seeded
+    with `evaluation_seed(model's noise key, epoch)`.  The model's train / eval mode is kept."""
     device = loader.device
     key = model._noise_state(device)[0]           # fixed at the first training step; this fixes it the same way
     moves = list(zip((METRICS_FILENAME, METRIC_HELPERS_FILE), epoch_metrics_filenames(epoch)))
     score_args = {}
     if factor_score:
         moves += zip((FACTOR_SCORE_FILENAME, FACTOR_SCORE_HELPERS_FILE), epoch_factor_score_filenames(epoch))
-        score_args = {"is_factor_score": True, "factor_score_seed": evaluation_seed(key, epoch)}
+        score_args.update(is_factor_score=True, factor_score_seed=evaluation_seed(key, epoch))
+    if sap_score:
+        moves += zip((SAP_SCORE_FILENAME, SAP_SCORE_HELPERS_FILE), epoch_sap_score_filenames(epoch))
+        score_args.update(is_sap_score=True, sap_score_seed=evaluation_seed(key, epoch))
     with tempfile.TemporaryDirectory(dir=save_dir) as tmp, evaluation_rng(device, key, epoch):
         Evaluator(model, None, device=device, logger=logger, save_dir=tmp, is_progress_bar=False)(
             loader.in_order(batch_size), is_metrics=True, is_losses=False, **score_args)
@@ -231,6 +257,133 @@ def factor_vote_accuracies(train_votes, eval_votes):
     return classifier, accuracy(train_votes), accuracy(eval_votes)
 
 
+# ---- SAP score (Kumar et al. 2018, section 3; the discrete variant of disentanglement_lib's sap_score.py) -----------
+def check_sap_score(dataset, latent_dim, num_train=10000, num_test=5000, C=0.01):
+    """ValueError unless the SAP score can be computed over `dataset` for a `latent_dim` model with these settings: the
+    dataset has known factors (`lat_sizes`, `lat_names`) and is their full grid.  No GPU work.  Returns lat_sizes as a
+    list of ints."""
+    if not (hasattr(dataset, "lat_sizes") and hasattr(dataset, "lat_names")):
+        raise ValueError("SAP score: the dataset %s has no lat_sizes / lat_names (known factors of variation)"
+                         % type(dataset).__name__)
+    return _check_sap_grid(dataset.lat_sizes, len(dataset), latent_dim, num_train, num_test, C)
+
+
+def _check_sap_grid(lat_sizes, n, latent_dim, num_train, num_test, C):
+    lat_sizes = [int(s) for s in lat_sizes]
+    if n != reduce(lambda x, y: x * y, lat_sizes, 1):
+        raise ValueError("SAP score: the dataset has %d items, not the %d of the full grid of its factors %s"
+                         % (n, reduce(lambda x, y: x * y, lat_sizes, 1), lat_sizes))
+    if all(s == 1 for s in lat_sizes):
+        raise ValueError("SAP score: every factor of %s has one value; there is nothing to predict" % lat_sizes)
+    if max(lat_sizes) > SAP_MAX_CLASSES:
+        raise ValueError("SAP score: a factor of %s has more than the kernel's limit of %d values"
+                         % (lat_sizes, SAP_MAX_CLASSES))
+    if int(latent_dim) < 2:
+        raise ValueError("SAP score: latent_dim must be at least 2 (the score compares the two most predictive dims), "
+                         "got %d" % int(latent_dim))
+    if int(latent_dim) > SAP_MAX_DIM:
+        raise ValueError("SAP score: latent_dim %d is above the kernel's limit of %d" % (int(latent_dim), SAP_MAX_DIM))
+    if int(num_train) < 2:
+        raise ValueError("SAP score: num_train must be at least 2, got %d" % int(num_train))
+    if int(num_train) > SAP_MAX_TRAIN:
+        raise ValueError("SAP score: num_train %d is above the kernel's limit of %d" % (int(num_train), SAP_MAX_TRAIN))
+    if int(num_test) < 1:
+        raise ValueError("SAP score: num_test must be at least 1, got %d" % int(num_test))
+    if not (math.isfinite(float(C)) and float(C) > 0):
+        raise ValueError("SAP score: C must be finite and positive, got %r" % (C,))
+    return lat_sizes
+
+
+def sap_labels(lat_sizes, train_rows, test_rows):
+    """Class labels of the scored factors (those of more than one value, ascending) for grid rows `train_rows` /
+    `test_rows` (C-order grid indices, the last factor fastest), all on the rows' device without a host sync ->
+    (factors [K'] list, train_cls int32 [K', num_train], test_cls int32 [K', num_test], n_classes int32 [K'],
+    counts int32 [K', S], present bool [K', S]) with S the largest size of a scored factor.  The classes of factor k are
+    the values seen among the training rows, ascending; a row's class is its value's place among them, -1 for a test
+    value no training row has; counts[k, c] is the training rows of class c and present[k, v] marks value v."""
+    device = train_rows.device
+    factors = [k for k, s in enumerate(lat_sizes) if s > 1]
+    S = max(lat_sizes[k] for k in factors)
+    strides = [reduce(lambda x, y: x * y, lat_sizes[k + 1:], 1) for k in range(len(lat_sizes))]
+    values = torch.arange(S, device=device)
+    train_cls, test_cls, counts, present = [], [], [], []
+    for k in factors:
+        vt = train_rows // strides[k] % lat_sizes[k]
+        ve = test_rows // strides[k] % lat_sizes[k]
+        cnt = (vt.unsqueeze(1) == values).sum(0)                  # [S]; values >= lat_sizes[k] count 0
+        seen = cnt > 0
+        place = torch.cumsum(seen, 0) - 1
+        train_cls.append(place[vt])
+        test_cls.append(torch.where(seen[ve], place[ve], -1))
+        counts.append(torch.zeros(S + 1, dtype=cnt.dtype, device=device).scatter_(
+            0, torch.where(seen, place, S), cnt)[:S])
+        present.append(seen)
+    present = torch.stack(present)
+    return (factors, torch.stack(train_cls).int(), torch.stack(test_cls).int(), present.sum(1).int(),
+            torch.stack(counts).int(), present)
+
+
+def sap_score_matrix(mu, train_rows, test_rows, train_cls, test_cls, n_classes, counts, C, coef=None, iters=None):
+    """`dv_sap_score_matrix` on `mu` [N, D] (any strides, a view of q_zCx included) -> the fp32 score [D, K'] of
+    `sap_labels`' classes; optionally the fitted lines into fp64 `coef` [D, K', S, 2] and the Newton steps into int32
+    `iters` [D, K', S]."""
+    N.require_cuda_f32(mu)
+    n, d = mu.shape
+    K, S = counts.shape
+    for name, t, dtype in (("train_rows", train_rows, torch.int64), ("test_rows", test_rows, torch.int64),
+                           ("train_cls", train_cls, torch.int32), ("test_cls", test_cls, torch.int32),
+                           ("n_classes", n_classes, torch.int32), ("counts", counts, torch.int32),
+                           ("coef", coef, torch.float64), ("iters", iters, torch.int32)):
+        if t is not None and (t.dtype != dtype or not t.is_contiguous() or not t.is_cuda):
+            raise ValueError("sap_score_matrix: %s must be a contiguous CUDA %s tensor" % (name, dtype))
+    score = torch.empty(d, K, dtype=torch.float32, device=mu.device)
+    N.call("dv_sap_score_matrix", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(train_rows), train_rows.numel(),
+           N.ptr(test_rows), test_rows.numel(), N.ptr(train_cls), N.ptr(test_cls), N.ptr(n_classes), N.ptr(counts), K,
+           S, float(C), N.ptr(score), N.ptr(coef), N.ptr(iters), N.stream())
+    return score
+
+
+def sap_from_matrix(score_matrix):
+    """SAP of a score matrix [D, K'] (D >= 2): the mean over factors of the largest minus the second largest score of
+    the factor's column, in fp64."""
+    m = torch.sort(score_matrix.double().cpu(), dim=0, descending=True)[0]
+    return float((m[0] - m[1]).mean())
+
+
+def sap_score(mu, lat_sizes, num_train=10000, num_test=5000, C=0.01, seed=0):
+    """SAP score of the encoder means `mu` [N, D] (CUDA fp32, dataset index order) of the full factor grid `lat_sizes`
+    -> ({"SAP"}, helpers).  The draws come from a device torch.Generator seeded with `seed`: `torch.randint(N,
+    (num_train,))` for the training rows, then `torch.randint(N, (num_test,))` for the test rows; the global generators
+    are not touched.  For every latent and scored factor `dv_sap_score_matrix` fits LinearSVC(C,
+    class_weight="balanced") exactly and scores it on the test rows; SAP is `sap_from_matrix` of that table.
+    helpers: "score_matrix" fp32 [D, K'], "factors" (the scored factor indices, ascending), "classes" int64 [K', S]
+    (each factor's training values, ascending, -1 beyond), "coef" fp64 [D, K', S, 2] (w, b of each problem: class c's
+    one-vs-rest problem in slot c, the two-class problem in slot 0, NaN beyond) and "solver_iterations" int32
+    [D, K', S] (Newton steps, -1 for a fit that did not converge, which also raises a RuntimeWarning)."""
+    lat_sizes = _check_sap_grid(lat_sizes, mu.shape[0], mu.shape[1], num_train, num_test, C)
+    N.require_cuda_f32(mu)
+    n, D = mu.shape
+    gen = torch.Generator(device=mu.device)
+    gen.manual_seed(int(seed))
+    train_rows = torch.randint(n, (int(num_train),), generator=gen, device=mu.device)
+    test_rows = torch.randint(n, (int(num_test),), generator=gen, device=mu.device)
+    factors, train_cls, test_cls, n_classes, counts, present = sap_labels(lat_sizes, train_rows, test_rows)
+    K, S = counts.shape
+    coef = torch.empty(D, K, S, 2, dtype=torch.float64, device=mu.device)
+    iters = torch.empty(D, K, S, dtype=torch.int32, device=mu.device)
+    matrix = sap_score_matrix(mu, train_rows, test_rows, train_cls, test_cls, n_classes, counts, C, coef, iters)
+    matrix, coef, iters, present = matrix.cpu(), coef.cpu(), iters.cpu(), present.cpu()
+    failed = int((iters < 0).sum())
+    if failed:
+        warnings.warn("SAP score: %d of the linear-SVM fits did not converge in the solver's step limit; see "
+                      "helpers['solver_iterations'] (-1)" % failed, RuntimeWarning)
+    values = torch.arange(S).expand(K, S)
+    classes = torch.sort(torch.where(present, values, S), dim=1)[0]           # the values seen, ascending, then S
+    helpers = {"score_matrix": matrix, "factors": torch.tensor(factors, dtype=torch.int64),
+               "classes": torch.where(classes < S, classes, -1), "coef": coef, "solver_iterations": iters}
+    return {"SAP": sap_from_matrix(matrix)}, helpers
+
+
 class Evaluator:
     def __init__(self, model, loss_f, device=torch.device("cpu"), logger=logging.getLogger(__name__),
                  save_dir="results", is_progress_bar=True):
@@ -243,15 +396,20 @@ class Evaluator:
         self._perm_queue = []         # injected sample indices (parity tests), consumed FIFO by _estimate_latent_entropies
         self.logger.info("Testing Device: {}".format(self.device))
 
-    def __call__(self, data_loader, is_metrics=False, is_losses=True, is_factor_score=False, factor_score_seed=0):
+    def __call__(self, data_loader, is_metrics=False, is_losses=True, is_factor_score=False, factor_score_seed=0,
+                 is_sap_score=False, sap_score_seed=0):
         """evaluate.py:59-96.  Like the reference, the first returned value is always None (it assigns the metrics to
         a differently named variable, :77-79); the metrics are logged and written to metrics.log.
         `is_factor_score=True` also writes the FactorVAE score (`compute_factor_vae_score` with its default settings
-        and `seed=factor_score_seed`) to factor_vae_score.log and its tables to factor_vae_score_helpers.pth; with
-        `is_metrics` the dataset is encoded once for both."""
+        and `seed=factor_score_seed`) to factor_vae_score.log and its tables to factor_vae_score_helpers.pth;
+        `is_sap_score=True` writes the SAP score (`compute_sap_score` with its default settings and
+        `seed=sap_score_seed`) to sap_score.log and its tables to sap_score_helpers.pth.  The dataset is encoded once
+        for all the scores asked for."""
         start = default_timer()
         if is_factor_score:
             check_factor_score(getattr(data_loader, "dataset", None), self.model.latent_dim)
+        if is_sap_score:
+            check_sap_score(getattr(data_loader, "dataset", None), self.model.latent_dim)
         is_still_training = self.model.training
         self.model.eval()
         metric, losses = None, None
@@ -272,6 +430,14 @@ class Evaluator:
             self.logger.info('FactorVAE score: {}'.format(score))
             save_metadata(score, self.save_dir, filename=FACTOR_SCORE_FILENAME)
             torch.save(helpers, os.path.join(self.save_dir, FACTOR_SCORE_HELPERS_FILE))
+        if is_sap_score:
+            self.logger.info('Computing the SAP score...')
+            if encoded is None:
+                encoded = self._compute_q_zCx(data_loader)
+            score, helpers = sap_score(encoded[1][0], data_loader.dataset.lat_sizes, seed=sap_score_seed)
+            self.logger.info('SAP score: {}'.format(score))
+            save_metadata(score, self.save_dir, filename=SAP_SCORE_FILENAME)
+            torch.save(helpers, os.path.join(self.save_dir, SAP_SCORE_HELPERS_FILE))
         if is_losses:
             self.logger.info('Computing losses...')
             losses = self.compute_losses(data_loader)
@@ -313,6 +479,14 @@ class Evaluator:
         mean = self._compute_q_zCx(dataloader)[1][0]
         return factor_vae_score(mean, dataloader.dataset.lat_sizes, batch_size, num_train, num_eval,
                                 num_variance_estimate, seed)[0]
+
+    def compute_sap_score(self, dataloader, num_train=10000, num_test=5000, C=0.01, seed=0):
+        """SAP score (Kumar et al. 2018, section 3) of the model's encoder means over `dataloader` (the dataset in index
+        order: DataLoader(shuffle=False) or DeviceLoader.in_order) -> {"SAP"}; see `sap_score` for the definition and
+        the order of the draws."""
+        check_sap_score(getattr(dataloader, "dataset", None), self.model.latent_dim, num_train, num_test, C)
+        mean = self._compute_q_zCx(dataloader)[1][0]
+        return sap_score(mean, dataloader.dataset.lat_sizes, num_train, num_test, C, seed)[0]
 
     def _known_factors(self, dataloader):
         try:

@@ -333,6 +333,34 @@ int dv_latent_entropy(const float* zs, const float* mean, const float* logvar, i
 int dv_group_variance(const float* mu, int ld, int row_stride, int N, int D, const long long* rows, int V, int L,
                       const float* global_var, float min_var, float* var_out, int* argmin_out, void* stream);
 
+/* ---- disentanglement metrics: SAP score (Kumar et al. 2018, section 3) --------------------------
+ * For every latent d and factor k (k < K): the exact fit of LinearSVC(C, class_weight="balanced") -- squared hinge, L2,
+ * the intercept a regularised feature of scale 1 -- on the 1-D training column x_i = mu[train_rows[i]][d] (element
+ * (n, d) at n*row_stride + d*ld, so the interleaved q_zCx buffer is read in place), then its accuracy on the test rows.
+ *   train_cls  int32 [K][num_train]: the class index (0 .. n_classes[k]-1, classes in ascending value) of each row
+ *   test_cls   int32 [K][num_test]: the class index of each test row, or -1 for a value absent from the training rows
+ *   n_classes  int32 [K] (1 .. class_stride), counts int32 [K][class_stride]: training rows of each class (> 0)
+ * Class weights cw_c = num_train / (n_classes * counts_c).  More than two classes: one-vs-rest, class c's problem with
+ * C_i = C*cw_c on its rows and plain C on the others (liblinear's convention); two classes: one problem, positive
+ * class 1, C_i = C*cw_{y_i}; one class: no fit.  Each problem minimises
+ *   1/2 (w^2 + b^2) + sum_i C_i max(0, 1 - s_i (w x_i + b))^2
+ * in fp64 by semismooth Newton (at most 64 steps) to |gradient| <= 1e-10 of its scale.  A test row is predicted as
+ * the argmax over classes of w_c x + b_c (lowest c on a tie), class 1 if w x + b > 0 for two classes, else class 0.
+ *   score [D][K] fp32: the share of the test rows predicted as their class
+ *   coef  fp64 [D][K][class_stride][2] (optional): (w, b) of problem p (the class for one-vs-rest, 0 for two
+ *         classes); NaN beyond the factor's problems
+ *   iters int32 [D][K][class_stride] (optional): Newton steps of problem p, -1 if it did not converge; 0 beyond
+ * Rows are in [0, N) and labels within their ranges (not checked: the caller builds them).  One launch of D*K CTAs, no
+ * workspace.  Deterministic (fixed-order reductions, no floating-point atomics), graph-capturable.
+ * DV_ERR_BAD_SHAPE: N < 1, D < 1, D > 1024, num_train < 1, num_train > 32768, num_test < 1, K < 1, class_stride < 1
+ * or class_stride > 256.
+ * DV_ERR_BAD_ARG: a required pointer NULL, C not finite and positive, or a pointer misaligned (rows and coef 8 bytes,
+ * the others 4). */
+int dv_sap_score_matrix(const float* mu, int ld, int row_stride, int N, int D, const long long* train_rows,
+                        int num_train, const long long* test_rows, int num_test, const int* train_cls,
+                        const int* test_cls, const int* n_classes, const int* counts, int K, int class_stride,
+                        double C, float* score, double* coef, int* iters, void* stream);
+
 /* ---- FactorVAE pieces ---------------------------------------------------------------------
  * dv_permute_dims replaces _permute_dims (losses.py:483-508): out[b][d] = z[perm[d][b]][d].
  * perms != NULL: int64 [D][B] (the reference's CPU randperm stream, trap T7).  perms == NULL:

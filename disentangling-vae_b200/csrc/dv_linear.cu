@@ -198,6 +198,12 @@ int wgrad(const float* g, const float* x, float* dw, float* dbias, float* ws, in
 
 using namespace dv;
 
+// The tensor-core GEMMs read their activation operand and the packed weight planes through TMA, which takes 16-byte
+// aligned global addresses only; the CUDA-core GEMM reads single floats.
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+// act of an input gradient: the activation whose derivative masks it
+static bool dgrad_act_ok(int act) { return act == DV_ACT_NONE || act == DV_ACT_RELU || act == DV_ACT_LEAKY; }
+
 extern "C" {
 
 // The tensor-core path packs w into the workspace (the layout of dv_linear_pack_multi) and runs on those planes.
@@ -217,6 +223,7 @@ int dv_linear_fwd(const float* x, const float* w, const float* bias, float* y, i
   if (act < DV_ACT_NONE || act > DV_ACT_LEAKY) return DV_ERR_BAD_ARG;
   if (ltc::nt_ok(K)) {
     if (!workspace) return DV_ERR_WORKSPACE;
+    if (!aligned16(x) || !aligned16(workspace)) return DV_ERR_BAD_ARG;
     float* packed = reinterpret_cast<float*>(workspace);
     const int rc = ltc::pack_multi(1, &w, &packed, &N, &K, as_stream(stream));
     if (rc != DV_OK) return rc;
@@ -232,8 +239,10 @@ int dv_linear_dgrad(const float* g, const float* w, const float* mask_src, float
                     int act, float slope, void* workspace, void* stream) {
   if (!g || !w || !dx) return DV_ERR_BAD_ARG;
   if (M <= 0 || N <= 0 || K <= 0) return DV_ERR_BAD_SHAPE;
+  if (!dgrad_act_ok(act)) return DV_ERR_BAD_ARG;
   if (ltc::nt_ok(N)) {
     if (!workspace) return DV_ERR_WORKSPACE;
+    if (!aligned16(g) || !aligned16(workspace)) return DV_ERR_BAD_ARG;
     float* packed = reinterpret_cast<float*>(workspace);
     const int rc = ltc::pack_multi(1, &w, &packed, &N, &K, as_stream(stream));
     if (rc != DV_OK) return rc;
@@ -265,6 +274,7 @@ int dv_linear_fwd_packed(const float* x, const float* w, const float* packed, co
   if (act < DV_ACT_NONE || act > DV_ACT_LEAKY) return DV_ERR_BAD_ARG;
   if (ltc::nt_ok(K)) {
     if (!packed) return DV_ERR_WORKSPACE;
+    if (!aligned16(x) || !aligned16(packed)) return DV_ERR_BAD_ARG;
     return ltc::fwd_packed(x, packed, bias, y, M, N, K, act, slope, as_stream(stream));
   }
   return dv_linear_fwd(x, w, bias, y, M, N, K, act, slope, nullptr, stream);       // CUDA-core path: reads w itself
@@ -274,8 +284,10 @@ int dv_linear_dgrad_packed(const float* g, const float* w, const float* packed, 
                            int K, int act, float slope, void* stream) {
   if (!g || !w || !dx) return DV_ERR_BAD_ARG;
   if (M <= 0 || N <= 0 || K <= 0) return DV_ERR_BAD_SHAPE;
+  if (!dgrad_act_ok(act)) return DV_ERR_BAD_ARG;
   if (ltc::nt_ok(N)) {
     if (!packed) return DV_ERR_WORKSPACE;
+    if (!aligned16(g) || !aligned16(packed)) return DV_ERR_BAD_ARG;
     return ltc::dgrad_packed(g, packed, mask_src, dx, M, N, K, act, slope, as_stream(stream));
   }
   return dv_linear_dgrad(g, w, mask_src, dx, M, N, K, act, slope, nullptr, stream);
@@ -295,6 +307,7 @@ int dv_linear_wgrad(const float* g, const float* x, float* dw, float* dbias, int
   cudaStream_t st = as_stream(stream);
   if (ltc::wgrad_ok(M, N, K)) {
     if (ltc::wgrad_workspace_bytes(M, N, K) > 0 && !workspace) return DV_ERR_WORKSPACE;
+    if (!aligned16(g) || !aligned16(x)) return DV_ERR_BAD_ARG;
     int S = 1;
     int rc = ltc::wgrad(g, x, dw, dbias, reinterpret_cast<float*>(workspace), M, N, K, &S, st);
     if (rc != DV_OK) return rc;

@@ -121,25 +121,32 @@ int dv_act_bwd(const float* dy, const float* y, float* g, long long n, int act, 
  */
 /* The shape selects the kernel.  A reduction length (K forward, N input gradient) that is a multiple of 4 and at
  * least 32 runs on the tensor cores (mma.sync tf32, 3xTF32); the call then packs w into `workspace`
- * (dv_linear_packed_floats(N, K) floats, 16-byte aligned, the layout of dv_linear_pack_multi).  Other shapes run on
- * the CUDA cores (FFMA); the query returns 0 for them and workspace may be NULL. */
+ * (dv_linear_packed_floats(N, K) floats, the layout of dv_linear_pack_multi) and reads the activation operand (x
+ * forward, g input gradient) through TMA: both must be 16-byte aligned, or the call returns DV_ERR_BAD_ARG before
+ * launching anything (DV_ERR_WORKSPACE when workspace is NULL).  Other shapes run on the CUDA cores (FFMA): the query
+ * returns 0 for them, workspace may be NULL and 4-byte aligned operands are enough. */
 size_t dv_linear_fwd_workspace_bytes(int M, int N, int K);
 size_t dv_linear_dgrad_workspace_bytes(int M, int N, int K);
 int dv_linear_fwd(const float* x, const float* w, const float* bias, float* y, int M, int N, int K,
                   int act, float slope, void* workspace, void* stream);
 /* dx[M,K] = (g[M,N] . w[N,K]) * act'(mask_src[M,K]); mask_src is the POST-activation output
- * of the previous layer (NULL: no mask); act in {NONE, RELU, LEAKY}. */
+ * of the previous layer (NULL: no mask); act in {NONE, RELU, LEAKY}, anything else (with or without a mask) is
+ * DV_ERR_BAD_ARG. */
 int dv_linear_dgrad(const float* g, const float* w, const float* mask_src, float* dx, int M, int N,
                     int K, int act, float slope, void* workspace, void* stream);
 /* dw[N,K] = g^T . x ; dbias[N] = column sums of g (may be NULL).  Small N*K problems are split over
- * the batch (deterministic split-K); workspace may be NULL when the query returns 0. */
+ * the batch (deterministic split-K); workspace may be NULL when the query returns 0.  N % 4 == 0, K % 4 == 0, K >= 32
+ * and M >= 32 run on the tensor cores, which read g and x through TMA: both must be 16-byte aligned there
+ * (DV_ERR_BAD_ARG otherwise, before any launch). */
 size_t dv_linear_wgrad_workspace_bytes(int M, int N, int K);
 int dv_linear_wgrad(const float* g, const float* x, float* dw, float* dbias, int M, int N, int K,
                     void* workspace, void* stream);
 /* Pre-packed weights: dv_linear_pack_multi splits n weight matrices (w[i]: [N[i], K[i]], HOST arrays of device
  * pointers / sizes) into the tensor-core hi/lo operand planes of BOTH directions in one launch, into caller-owned
  * buffers of dv_linear_packed_floats(N, K) floats (16-byte aligned); dv_linear_fwd_packed / dv_linear_dgrad_packed are
- * dv_linear_fwd / dv_linear_dgrad on those planes (w is still passed: shapes that run on the CUDA cores read it).
+ * dv_linear_fwd / dv_linear_dgrad on those planes (w is still passed: shapes that run on the CUDA cores read it), with
+ * the same refusals: on a tensor-core shape, NULL packed is DV_ERR_WORKSPACE, and packed or the activation operand
+ * not 16-byte aligned is DV_ERR_BAD_ARG.
  * One pack launch per network node per step instead of one per layer per direction. */
 size_t dv_linear_packed_floats(int N, int K);
 int dv_linear_pack_multi(int n, const void* const* w, void* const* packed, const int* N, const int* K, void* stream);

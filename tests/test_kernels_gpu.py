@@ -1,7 +1,6 @@
 """Per-kernel parity: every C-ABI entry point against the oracle's plain-PyTorch CPU ops on the
 same seeded inputs.  Tolerance: the north_star's 1e-4 relative (fp32); most kernels are far
 inside it.  Run on an H100:  pytest -m gpu."""
-import math
 
 import pytest
 import torch
@@ -239,52 +238,6 @@ def test_channel_sum_and_transpose_and_act_bwd(ops):
     yy = torch.sigmoid(torch.randn(4096) * 4)
     dy = torch.randn(4096)
     assert_close(ops.act_bwd(dy.to(dev()), yy.to(dev()), 2).cpu(), dy * (1 - yy) * yy, tol=1e-6)
-
-
-LIN_CASES = [(64, 256, 512), (7, 20, 256), (130, 256, 10), (33, 1000, 1000), (256, 2, 1000), (5, 128, 64), (1, 512, 256),
-             (1024, 256, 512), (1000, 20, 256), (513, 256, 10)]
-
-
-@pytest.mark.parametrize("M,N,K", LIN_CASES)
-def test_linear_fwd_dgrad_wgrad(ops, M, N, K):
-    torch.manual_seed(M + N + K)
-    x = torch.randn(M, K, requires_grad=True)
-    w = (torch.randn(N, K) / math.sqrt(K)).requires_grad_(True)
-    b = torch.randn(N, requires_grad=True)
-    for act, slope, f in [(0, 0.0, lambda t: t), (1, 0.0, torch.relu), (3, 0.2, lambda t: F.leaky_relu(t, 0.2))]:
-        y = ops.linear_fwd(x.detach().to(dev()), w.detach().to(dev()), b.detach().to(dev()), act, slope)
-        assert_close(y.cpu(), f(F.linear(x, w, b)), what="fwd act %d" % act)
-    g = torch.randn(M, N)
-    x.grad = w.grad = b.grad = None
-    (F.linear(x, w, b) * g).sum().backward()
-    dx = ops.linear_dgrad(g.to(dev()), w.detach().to(dev()), None, 0)
-    assert_close(dx.cpu(), x.grad, what="dgrad")
-    prev = torch.randn(M, K)
-    dxm = ops.linear_dgrad(g.to(dev()), w.detach().to(dev()), torch.relu(prev).to(dev()), 1)
-    assert_close(dxm.cpu(), x.grad * (prev > 0), what="dgrad relu mask")
-    dxl = ops.linear_dgrad(g.to(dev()), w.detach().to(dev()), F.leaky_relu(prev, 0.2).to(dev()), 3, 0.2)
-    assert_close(dxl.cpu(), x.grad * torch.where(prev > 0, 1.0, 0.2), what="dgrad leaky mask")
-    dw, db = ops.linear_wgrad(g.to(dev()), x.detach().to(dev()))
-    assert_close(dw.cpu(), w.grad, what="wgrad")
-    assert_close(db.cpu(), b.grad, what="bgrad")
-
-
-@pytest.mark.parametrize("M,N,K", [(1024, 256, 512), (256, 1000, 1000), (300, 1000, 12), (77, 512, 256)])
-def test_linear_tensor_core_accuracy_vs_fp64(ops, M, N, K):
-    """The tensor-core linear layers use the same error-compensated 3xTF32 scheme as the convolutions: <= 4e-6 of the
-    output scale against an fp64 reference (plain fp32 ~5e-7, single-pass tf32 ~5e-4)."""
-    torch.manual_seed(M * 7 + N + K)
-    x = torch.randn(M, K)
-    w = torch.randn(N, K) / math.sqrt(K)
-    b = torch.randn(N)
-    g = torch.randn(M, N)
-    y = ops.linear_fwd(x.to(dev()), w.to(dev()), b.to(dev()), 0)
-    assert_close(y.cpu(), F.linear(x.double(), w.double(), b.double()), tol=4e-6, what="fwd vs fp64")
-    dx = ops.linear_dgrad(g.to(dev()), w.to(dev()), None, 0)
-    assert_close(dx.cpu(), g.double() @ w.double(), tol=4e-6, what="dgrad vs fp64")
-    dw, db = ops.linear_wgrad(g.to(dev()), x.to(dev()))
-    assert_close(dw.cpu(), g.double().t() @ x.double(), tol=4e-6, what="wgrad vs fp64")
-    assert_close(db.cpu(), g.double().sum(0), tol=4e-6, what="dbias vs fp64")
 
 
 @pytest.mark.parametrize("dist", ["bernoulli", "gaussian", "laplace"])
@@ -628,24 +581,6 @@ def test_loss_combine_and_act_bwd_chansum(ops):
         assert_close(cs.cpu(), g_ref.double().sum((0, 2, 3)).float().cpu(), tol=2e-5, what="chansum")
         _, cs2 = ops.act_bwd_chansum(dy, y, 2)
         assert torch.equal(cs, cs2)
-
-
-def test_linear_prepacked_equals_per_call_pack(ops):
-    """dv_linear_pack_multi (every weight matrix of a node, both operand layouts, one launch) + dv_linear_fwd_packed /
-    dv_linear_dgrad_packed give bit-identical results to the per-call packs, incl. the shapes that stay on the CUDA cores."""
-    torch.manual_seed(8)
-    shapes = [(256, 512), (256, 256), (20, 256), (256, 10), (1000, 1000), (2, 1000), (1000, 10)]
-    ws = [(torch.randn(n, k) / math.sqrt(k)).to(dev()) for n, k in shapes]
-    packs = ops.linear_pack_multi(ws)
-    for (n, k), w, pk in zip(shapes, ws, packs):
-        M = 130
-        x = torch.randn(M, k, device=dev())
-        b = torch.randn(n, device=dev())
-        g = torch.randn(M, n, device=dev())
-        prev = torch.relu(torch.randn(M, k, device=dev()))
-        assert torch.equal(ops.linear_fwd(x, w, b, 1, packed=pk), ops.linear_fwd(x, w, b, 1))
-        assert torch.equal(ops.linear_dgrad(g, w, prev, 1, packed=pk), ops.linear_dgrad(g, w, prev, 1))
-        assert torch.equal(ops.linear_dgrad(g, w, None, 0, packed=pk), ops.linear_dgrad(g, w, None, 0))
 
 
 def test_conv_pack_multi_equals_per_layer_pack(ops):

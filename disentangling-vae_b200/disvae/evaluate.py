@@ -34,6 +34,10 @@ SAP_SCORE_HELPERS_FILE = "sap_score_helpers.pth"
 SAP_MAX_DIM = 1024                         # dv_sap_score_matrix's limits: latents,
 SAP_MAX_TRAIN = 32768                      # training rows staged in shared memory,
 SAP_MAX_CLASSES = 256                      # and values of a scored factor
+BETA_VAE_SCORE_FILENAME = "beta_vae_score.log"
+BETA_VAE_SCORE_HELPERS_FILE = "beta_vae_score_helpers.pth"
+BETA_VAE_MAX_DIM = 128                     # dv_logistic_fit's limits: latents,
+BETA_VAE_MAX_FACTORS = 32                  # and scored factors (classes)
 EVAL_SEED_STRIDE = 0x9E3779B97F4A7C15      # odd 64-bit constant: consecutive epochs get unrelated seeds
 
 
@@ -50,6 +54,11 @@ def epoch_factor_score_filenames(epoch):
 def epoch_sap_score_filenames(epoch):
     """(`sap_score-{epoch}.log`, `sap_score_helpers-{epoch}.pth`): the SAP score after epoch `epoch`."""
     return "sap_score-{}.log".format(epoch), "sap_score_helpers-{}.pth".format(epoch)
+
+
+def epoch_beta_vae_score_filenames(epoch):
+    """(`beta_vae_score-{epoch}.log`, `beta_vae_score_helpers-{epoch}.pth`): the beta-VAE score after epoch `epoch`."""
+    return "beta_vae_score-{}.log".format(epoch), "beta_vae_score_helpers-{}.pth".format(epoch)
 
 
 def evaluation_seed(noise_key, epoch):
@@ -119,12 +128,25 @@ def check_epoch_sap_score(sap_score, metrics_every, loader, latent_dim):
     check_sap_score(loader.dataset, latent_dim)
 
 
-def write_epoch_metrics(model, loader, epoch, batch_size, save_dir, logger, factor_score=False, sap_score=False):
+def check_epoch_beta_vae_score(beta_vae_score, metrics_every, loader, latent_dim):
+    """ValueError unless the beta-VAE score can be written with the metrics of every `metrics_every` epochs (after
+    `check_resident_metrics` has accepted `loader`).  No GPU work."""
+    if not beta_vae_score:
+        return
+    if not metrics_every:
+        raise ValueError("beta_vae_score=True needs metrics_every > 0: the score is written with the metrics of those "
+                         "epochs")
+    check_beta_vae_score(loader.dataset, latent_dim)
+
+
+def write_epoch_metrics(model, loader, epoch, batch_size, save_dir, logger, factor_score=False, sap_score=False,
+                        beta_vae_score=False):
     """MIG / AAM of `model` over `loader.in_order(batch_size)` (a DeviceLoader) into `save_dir` as
     `epoch_metrics_filenames(epoch)`, with the index draws seeded by `evaluation_rng(.., model's noise key, epoch)`.
     `factor_score=True` also writes the FactorVAE score from the same encodings as `epoch_factor_score_filenames(epoch)`,
-    and `sap_score=True` the SAP score as `epoch_sap_score_filenames(epoch)`, each drawn from its own generator seeded
-    with `evaluation_seed(model's noise key, epoch)`.  The model's train / eval mode is kept."""
+    `sap_score=True` the SAP score as `epoch_sap_score_filenames(epoch)` and `beta_vae_score=True` the beta-VAE score as
+    `epoch_beta_vae_score_filenames(epoch)`, each drawn from its own generator seeded with
+    `evaluation_seed(model's noise key, epoch)`.  The model's train / eval mode is kept."""
     device = loader.device
     key = model._noise_state(device)[0]           # fixed at the first training step; this fixes it the same way
     moves = list(zip((METRICS_FILENAME, METRIC_HELPERS_FILE), epoch_metrics_filenames(epoch)))
@@ -135,6 +157,9 @@ def write_epoch_metrics(model, loader, epoch, batch_size, save_dir, logger, fact
     if sap_score:
         moves += zip((SAP_SCORE_FILENAME, SAP_SCORE_HELPERS_FILE), epoch_sap_score_filenames(epoch))
         score_args.update(is_sap_score=True, sap_score_seed=evaluation_seed(key, epoch))
+    if beta_vae_score:
+        moves += zip((BETA_VAE_SCORE_FILENAME, BETA_VAE_SCORE_HELPERS_FILE), epoch_beta_vae_score_filenames(epoch))
+        score_args.update(is_beta_vae_score=True, beta_vae_score_seed=evaluation_seed(key, epoch))
     with tempfile.TemporaryDirectory(dir=save_dir) as tmp, evaluation_rng(device, key, epoch):
         Evaluator(model, None, device=device, logger=logger, save_dir=tmp, is_progress_bar=False)(
             loader.in_order(batch_size), is_metrics=True, is_losses=False, **score_args)
@@ -384,6 +409,142 @@ def sap_score(mu, lat_sizes, num_train=10000, num_test=5000, C=0.01, seed=0):
     return {"SAP": sap_from_matrix(matrix)}, helpers
 
 
+# ---- beta-VAE score (Higgins et al. 2017, section 3; the conventions of disentanglement_lib's beta_vae.py) ---------
+def check_beta_vae_score(dataset, latent_dim, batch_size=64, num_train=10000, num_eval=5000):
+    """ValueError unless the beta-VAE score can be computed over `dataset` for a `latent_dim` model with these
+    settings: the dataset has known factors (`lat_sizes`, `lat_names`), is their full grid and has between 2 and
+    BETA_VAE_MAX_FACTORS factors of more than one value.  No GPU work.  Returns lat_sizes as a list of ints."""
+    if not (hasattr(dataset, "lat_sizes") and hasattr(dataset, "lat_names")):
+        raise ValueError("beta-VAE score: the dataset %s has no lat_sizes / lat_names (known factors of variation)"
+                         % type(dataset).__name__)
+    return _check_beta_vae_grid(dataset.lat_sizes, len(dataset), latent_dim, batch_size, num_train, num_eval)
+
+
+def _check_beta_vae_grid(lat_sizes, n, latent_dim, batch_size, num_train, num_eval):
+    lat_sizes = [int(s) for s in lat_sizes]
+    if n != reduce(lambda x, y: x * y, lat_sizes, 1):
+        raise ValueError("beta-VAE score: the dataset has %d items, not the %d of the full grid of its factors %s"
+                         % (n, reduce(lambda x, y: x * y, lat_sizes, 1), lat_sizes))
+    scored = sum(s > 1 for s in lat_sizes)
+    if scored < 2:
+        raise ValueError("beta-VAE score: %s has %d factors of more than one value; the score needs at least 2 to "
+                         "tell apart" % (lat_sizes, scored))
+    if scored > BETA_VAE_MAX_FACTORS:
+        raise ValueError("beta-VAE score: %s has %d factors of more than one value, above the kernel's limit of %d"
+                         % (lat_sizes, scored, BETA_VAE_MAX_FACTORS))
+    if int(latent_dim) > BETA_VAE_MAX_DIM:
+        raise ValueError("beta-VAE score: latent_dim %d is above the kernel's limit of %d"
+                         % (int(latent_dim), BETA_VAE_MAX_DIM))
+    for name, value in (("batch_size", batch_size), ("num_train", num_train), ("num_eval", num_eval)):
+        if int(value) < 1:
+            raise ValueError("beta-VAE score: %s must be at least 1, got %d" % (name, int(value)))
+    return lat_sizes
+
+
+def beta_vae_points(lat_sizes, count, batch_size, generator):
+    """(label [count], rows_a, rows_b [count, batch_size]) of `count` points drawn from `generator` on its device: one
+    randint for the label of every point (its scored factor's place among the factors of more than one value), then
+    for every factor k, k = 0 .. K-1 in order (size-1 factors included), one randint [count, batch_size] for its `a`
+    values and one for its `b` values; factor k of a point on k takes the `a` values in `b` too.  Rows are the C-order
+    grid indices, the last factor fastest."""
+    device = generator.device
+    varying = torch.tensor([k for k, s in enumerate(lat_sizes) if s > 1], dtype=torch.int64, device=device)
+    label = torch.randint(len(varying), (count,), generator=generator, device=device)
+    factor = varying[label]
+    rows_a = torch.zeros(count, batch_size, dtype=torch.int64, device=device)
+    rows_b = torch.zeros(count, batch_size, dtype=torch.int64, device=device)
+    stride = reduce(lambda x, y: x * y, lat_sizes, 1)
+    for k, s in enumerate(lat_sizes):
+        stride //= s
+        a = torch.randint(s, (count, batch_size), generator=generator, device=device)
+        b = torch.randint(s, (count, batch_size), generator=generator, device=device)
+        b = torch.where((factor == k).unsqueeze(1), a, b)
+        rows_a += a * stride
+        rows_b += b * stride
+    return label, rows_a, rows_b
+
+
+def pair_abs_diff_mean(mu, rows_a, rows_b):
+    """`dv_pair_abs_diff_mean` on `mu` [N, D] (any strides, a view of q_zCx included) and int64 `rows_a`, `rows_b`
+    [V, L] -> fp64 x [V, D], x[v, d] = mean over l of |mu[rows_a[v, l], d] - mu[rows_b[v, l], d]|, added in order."""
+    N.require_cuda_f32(mu)
+    n, d = mu.shape
+    V, L = rows_a.shape
+    for name, t in (("rows_a", rows_a), ("rows_b", rows_b)):
+        if t.dtype != torch.int64 or not t.is_contiguous() or t.shape != (V, L):
+            raise ValueError("pair_abs_diff_mean: %s must be a contiguous int64 tensor of shape %s" % (name, (V, L)))
+    x = torch.empty(V, d, dtype=torch.float64, device=mu.device)
+    N.call("dv_pair_abs_diff_mean", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(rows_a), N.ptr(rows_b), V, L,
+           N.ptr(x), N.stream())
+    return x
+
+
+def logistic_fit(x, labels, n_classes, K, num_train):
+    """`dv_logistic_fit` on fp64 features `x` [V, D] (the first `num_train` rows train) with int32 class indices
+    `labels` [num_train] and the class count in int32 `n_classes` [1] on the device -> (coef fp64 [K, D + 1], pred
+    int32 [V], iters int32 [1]); see include/disvae_b200.h for the objective and the layout of coef."""
+    V, D = x.shape
+    for name, t, dtype in (("x", x, torch.float64), ("labels", labels, torch.int32),
+                           ("n_classes", n_classes, torch.int32)):
+        if t.dtype != dtype or not t.is_contiguous() or not t.is_cuda:
+            raise ValueError("logistic_fit: %s must be a contiguous CUDA %s tensor" % (name, dtype))
+    L = N.lib()
+    nbytes = L.dv_logistic_fit_workspace_bytes(int(num_train), D, int(K))
+    ws = torch.empty(max(nbytes, 8) // 8, dtype=torch.float64, device=x.device)
+    coef = torch.empty(int(K), D + 1, dtype=torch.float64, device=x.device)
+    pred = torch.empty(V, dtype=torch.int32, device=x.device)
+    iters = torch.empty(1, dtype=torch.int32, device=x.device)
+    N.call("dv_logistic_fit", N.ptr(x), D, int(num_train), V - int(num_train), N.ptr(labels), N.ptr(n_classes), int(K),
+           N.ptr(coef), N.ptr(pred), N.ptr(iters), N.ptr(ws), nbytes, N.stream())
+    return coef, pred, iters
+
+
+def beta_vae_score(mu, lat_sizes, batch_size=64, num_train=10000, num_eval=5000, seed=0):
+    """beta-VAE score of the encoder means `mu` [N, D] (CUDA fp32, dataset index order) of the full factor grid
+    `lat_sizes` -> ({"train_accuracy", "eval_accuracy"}, helpers).  The draws come from a device torch.Generator seeded
+    with `seed`: `beta_vae_points` for the `num_train` training points, then for the `num_eval` evaluation points; the
+    global generators are not touched.  A point's feature is `pair_abs_diff_mean` of its rows, and `logistic_fit` fits
+    LogisticRegression(C=1) exactly to the training points, over the scored factors seen among them.
+    helpers: "factors" int64 [K'] (the scored factors, ascending), "classes" int64 (the factors seen in training,
+    ascending), "coef" fp64 [rows, D] and "intercept" fp64 [rows] (rows = the classes for more than two, 1 for two
+    with classes[1] the positive class, 0 for one), "solver_iterations" int32 scalar (Newton steps, -1 for a fit that
+    did not converge, which also raises a RuntimeWarning), "train_confusion" and "eval_confusion" int64 [K', K'] (points by
+    true x predicted scored factor)."""
+    lat_sizes = _check_beta_vae_grid(lat_sizes, mu.shape[0], mu.shape[1], batch_size, num_train, num_eval)
+    N.require_cuda_f32(mu)
+    num_train, num_eval, batch_size = int(num_train), int(num_eval), int(batch_size)
+    device = mu.device
+    gen = torch.Generator(device=device)
+    gen.manual_seed(int(seed))
+    train_label, train_a, train_b = beta_vae_points(lat_sizes, num_train, batch_size, gen)
+    eval_label, eval_a, eval_b = beta_vae_points(lat_sizes, num_eval, batch_size, gen)
+    x = pair_abs_diff_mean(mu, torch.cat([train_a, eval_a]), torch.cat([train_b, eval_b]))
+    factors = [k for k, s in enumerate(lat_sizes) if s > 1]
+    K = len(factors)
+    seen = torch.bincount(train_label, minlength=K) > 0
+    place = torch.cumsum(seen, 0) - 1
+    classes = torch.sort(torch.where(seen, torch.arange(K, device=device), K))[0]    # seen labels, ascending, then K
+    n_classes = seen.sum().int().view(1)
+    coef, pred, iters = logistic_fit(x, place[train_label].int(), n_classes, K, num_train)
+    pred = classes[pred.long()]
+    truth = torch.cat([train_label, eval_label])
+    cells = truth * K + pred
+    train_conf = torch.bincount(cells[:num_train], minlength=K * K).view(K, K)
+    eval_conf = torch.bincount(cells[num_train:], minlength=K * K).view(K, K)
+    nc, steps = int(n_classes), int(iters)
+    train_conf, eval_conf, coef, classes = train_conf.cpu(), eval_conf.cpu(), coef.cpu(), classes.cpu()
+    if steps < 0:
+        warnings.warn("beta-VAE score: the logistic-regression fit did not converge in the solver's step limit; see "
+                      "helpers['solver_iterations'] (-1)", RuntimeWarning)
+    rows = nc if nc > 2 else nc - 1
+    factors = torch.tensor(factors, dtype=torch.int64)
+    helpers = {"factors": factors, "classes": factors[classes[:nc]], "coef": coef[:rows, :-1].clone(),
+               "intercept": coef[:rows, -1].clone(), "solver_iterations": iters.cpu()[0], "train_confusion": train_conf,
+               "eval_confusion": eval_conf}
+    score = {"train_accuracy": int(train_conf.trace()) / num_train, "eval_accuracy": int(eval_conf.trace()) / num_eval}
+    return score, helpers
+
+
 class Evaluator:
     def __init__(self, model, loss_f, device=torch.device("cpu"), logger=logging.getLogger(__name__),
                  save_dir="results", is_progress_bar=True):
@@ -397,19 +558,23 @@ class Evaluator:
         self.logger.info("Testing Device: {}".format(self.device))
 
     def __call__(self, data_loader, is_metrics=False, is_losses=True, is_factor_score=False, factor_score_seed=0,
-                 is_sap_score=False, sap_score_seed=0):
+                 is_sap_score=False, sap_score_seed=0, is_beta_vae_score=False, beta_vae_score_seed=0):
         """evaluate.py:59-96.  Like the reference, the first returned value is always None (it assigns the metrics to
         a differently named variable, :77-79); the metrics are logged and written to metrics.log.
         `is_factor_score=True` also writes the FactorVAE score (`compute_factor_vae_score` with its default settings
         and `seed=factor_score_seed`) to factor_vae_score.log and its tables to factor_vae_score_helpers.pth;
         `is_sap_score=True` writes the SAP score (`compute_sap_score` with its default settings and
-        `seed=sap_score_seed`) to sap_score.log and its tables to sap_score_helpers.pth.  The dataset is encoded once
-        for all the scores asked for."""
+        `seed=sap_score_seed`) to sap_score.log and its tables to sap_score_helpers.pth; `is_beta_vae_score=True` writes
+        the beta-VAE score (`compute_beta_vae_score` with its default settings and `seed=beta_vae_score_seed`) to
+        beta_vae_score.log and its tables to beta_vae_score_helpers.pth.  The dataset is encoded once for all the scores
+        asked for."""
         start = default_timer()
         if is_factor_score:
             check_factor_score(getattr(data_loader, "dataset", None), self.model.latent_dim)
         if is_sap_score:
             check_sap_score(getattr(data_loader, "dataset", None), self.model.latent_dim)
+        if is_beta_vae_score:
+            check_beta_vae_score(getattr(data_loader, "dataset", None), self.model.latent_dim)
         is_still_training = self.model.training
         self.model.eval()
         metric, losses = None, None
@@ -438,6 +603,14 @@ class Evaluator:
             self.logger.info('SAP score: {}'.format(score))
             save_metadata(score, self.save_dir, filename=SAP_SCORE_FILENAME)
             torch.save(helpers, os.path.join(self.save_dir, SAP_SCORE_HELPERS_FILE))
+        if is_beta_vae_score:
+            self.logger.info('Computing the beta-VAE score...')
+            if encoded is None:
+                encoded = self._compute_q_zCx(data_loader)
+            score, helpers = beta_vae_score(encoded[1][0], data_loader.dataset.lat_sizes, seed=beta_vae_score_seed)
+            self.logger.info('beta-VAE score: {}'.format(score))
+            save_metadata(score, self.save_dir, filename=BETA_VAE_SCORE_FILENAME)
+            torch.save(helpers, os.path.join(self.save_dir, BETA_VAE_SCORE_HELPERS_FILE))
         if is_losses:
             self.logger.info('Computing losses...')
             losses = self.compute_losses(data_loader)
@@ -487,6 +660,15 @@ class Evaluator:
         check_sap_score(getattr(dataloader, "dataset", None), self.model.latent_dim, num_train, num_test, C)
         mean = self._compute_q_zCx(dataloader)[1][0]
         return sap_score(mean, dataloader.dataset.lat_sizes, num_train, num_test, C, seed)[0]
+
+    def compute_beta_vae_score(self, dataloader, batch_size=64, num_train=10000, num_eval=5000, seed=0):
+        """beta-VAE score (Higgins et al. 2017, section 3) of the model's encoder means over `dataloader` (the dataset
+        in index order: DataLoader(shuffle=False) or DeviceLoader.in_order) -> {"train_accuracy", "eval_accuracy"};
+        see `beta_vae_score` for the definition and the order of the draws."""
+        check_beta_vae_score(getattr(dataloader, "dataset", None), self.model.latent_dim, batch_size, num_train,
+                             num_eval)
+        mean = self._compute_q_zCx(dataloader)[1][0]
+        return beta_vae_score(mean, dataloader.dataset.lat_sizes, batch_size, num_train, num_eval, seed)[0]
 
     def _known_factors(self, dataloader):
         try:

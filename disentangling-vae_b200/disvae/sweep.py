@@ -31,8 +31,9 @@ import torch
 
 from disvae import ops
 from disvae.data import DeviceLoader, device_loader_for
-from disvae.evaluate import (Evaluator, check_epoch_factor_score, check_epoch_sap_score, check_factor_score,
-                             check_resident_metrics, check_sap_score, evaluation_rng, evaluation_seed,
+from disvae.evaluate import (Evaluator, check_beta_vae_score, check_epoch_beta_vae_score, check_epoch_factor_score,
+                             check_epoch_sap_score, check_factor_score, check_resident_metrics, check_sap_score,
+                             evaluation_rng, evaluation_seed,
                              write_epoch_metrics)
 from disvae.fused import FusedAdam
 from disvae.models.losses import permutation_key
@@ -134,14 +135,14 @@ class Sweep:
         return entry[1]
 
     def __call__(self, data_loader, epochs=10, checkpoint_every=10, save_state=False, metrics_every=0,
-                 metrics_batch_size=1000, factor_score=False, sap_score=False):
+                 metrics_batch_size=1000, factor_score=False, sap_score=False, beta_vae_score=False):
         """Train every member for `epochs` epochs over `data_loader` (a DeviceLoader, or a DataLoader converted to one
         once per Sweep), like `Trainer.__call__` for each.  Calling again continues as a lone Trainer called again
         does: step counters, Adam state, Philox counters and the loader's epochs carry on.  `save_state=True` writes
         each member's training state into its own save_dir; members that loaded one continue from it.
         `metrics_every` writes each member's `metrics-{epoch}.log` as `Trainer.__call__` does, one member after
-        another on the caller's stream, over the one resident copy; `factor_score=True` and `sap_score=True` add each
-        member's FactorVAE and SAP scores of those epochs."""
+        another on the caller's stream, over the one resident copy; `factor_score=True`, `sap_score=True` and
+        `beta_vae_score=True` add each member's FactorVAE, SAP and beta-VAE scores of those epochs."""
         first, loader_state = self._resume()
         if loader_state is not None:
             check_loader_state(loader_state, data_loader, device_data=True)
@@ -151,6 +152,7 @@ class Sweep:
         for m in self.members:
             check_epoch_factor_score(factor_score, metrics_every, data_loader, m.model.latent_dim)
             check_epoch_sap_score(sap_score, metrics_every, data_loader, m.model.latent_dim)
+            check_epoch_beta_vae_score(beta_vae_score, metrics_every, data_loader, m.model.latent_dim)
         loader = self._loader(data_loader)
         for m in self.members:
             m._resume = None
@@ -160,16 +162,18 @@ class Sweep:
         start = default_timer()
         with torch.cuda.device(self.device):
             self._run(loader, first, epochs, checkpoint_every, save_state, start, metrics_every, metrics_batch_size,
-                      factor_score, sap_score)
+                      factor_score, sap_score, beta_vae_score)
 
-    def evaluate(self, is_metrics=True, is_losses=True, batch_size=1000, is_factor_score=False, is_sap_score=False):
+    def evaluate(self, is_metrics=True, is_losses=True, batch_size=1000, is_factor_score=False, is_sap_score=False,
+                 is_beta_vae_score=False):
         """Every member's `Evaluator(...)(loader.in_order(batch_size), is_metrics, is_losses)` over the loader of the
         latest call, into its save_dir (`metrics.log`, `metric_helpers.pth`, `test_losses.log`, as `main.py
         --is-eval-only` writes them), with the index draws seeded as the metrics after its latest epoch
         (`disvae.evaluate.evaluation_rng`); its `metrics.log` equals that epoch's `metrics-{epoch}.log`.
         `is_factor_score=True` also writes `factor_vae_score.log` and `factor_vae_score_helpers.pth`, seeded as the score
-        after its latest epoch (`disvae.evaluate.evaluation_seed`), and `is_sap_score=True` `sap_score.log` and
-        `sap_score_helpers.pth`, seeded the same way."""
+        after its latest epoch (`disvae.evaluate.evaluation_seed`), `is_sap_score=True` `sap_score.log` and
+        `sap_score_helpers.pth`, and `is_beta_vae_score=True` `beta_vae_score.log` and `beta_vae_score_helpers.pth`,
+        seeded the same way."""
         if self.loader is None:
             raise ValueError("Sweep.evaluate: the sweep has no loader yet; train it first (sweep(loader, ...))")
         if is_metrics:
@@ -182,6 +186,9 @@ class Sweep:
         if is_sap_score:
             for m in self.members:
                 check_sap_score(self.loader.dataset, m.model.latent_dim)
+        if is_beta_vae_score:
+            for m in self.members:
+                check_beta_vae_score(self.loader.dataset, m.model.latent_dim)
         with torch.cuda.device(self.device):
             for m in self.members:
                 key, epoch = m.model._noise_state(self.device)[0], m._next_epoch - 1
@@ -191,7 +198,9 @@ class Sweep:
                                                                  is_losses=is_losses, is_factor_score=is_factor_score,
                                                                  factor_score_seed=evaluation_seed(key, epoch),
                                                                  is_sap_score=is_sap_score,
-                                                                 sap_score_seed=evaluation_seed(key, epoch))
+                                                                 sap_score_seed=evaluation_seed(key, epoch),
+                                                                 is_beta_vae_score=is_beta_vae_score,
+                                                                 beta_vae_score_seed=evaluation_seed(key, epoch))
 
     def _resume(self):
         """(first epoch, saved loader state) of the members' loaded training states, (0, None) if none has one.
@@ -219,7 +228,7 @@ class Sweep:
             yield
 
     def _run(self, loader, first, epochs, checkpoint_every, save_state, start, metrics_every, metrics_batch_size,
-             factor_score, sap_score):
+             factor_score, sap_score, beta_vae_score):
         members = self.members
         main = torch.cuda.current_stream(self.device)
         if self.streams is None:
@@ -276,7 +285,7 @@ class Sweep:
                         main.wait_event(ev)
                     for m in members:                              # the next gather, on `main`, waits for these
                         write_epoch_metrics(m.model, loader, epoch, metrics_batch_size, m.save_dir, m.logger,
-                                            factor_score, sap_score)
+                                            factor_score, sap_score, beta_vae_score)
         finally:
             for ev in done:
                 if ev is not None:

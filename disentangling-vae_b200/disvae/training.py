@@ -21,7 +21,8 @@ import torch.distributed as dist
 from tqdm import trange
 
 from disvae import _native
-from disvae.evaluate import (check_epoch_factor_score, check_epoch_sap_score, check_resident_metrics,
+from disvae.evaluate import (check_epoch_beta_vae_score, check_epoch_factor_score, check_epoch_sap_score,
+                             check_resident_metrics,
                              write_epoch_metrics)
 from disvae.fused import FusedAdam
 from disvae.models.losses import DeviceLossLog
@@ -74,15 +75,16 @@ class Trainer():
         self.logger.info("Training Device: {}".format(self.device))
 
     def __call__(self, data_loader, epochs=10, checkpoint_every=10, save_state=False, metrics_every=0,
-                 metrics_batch_size=1000, factor_score=False, sap_score=False):
+                 metrics_batch_size=1000, factor_score=False, sap_score=False, beta_vae_score=False):
         """training.py:64-102.  `save_state=True` also writes the training state (`training_state_filename`) next to
         every checkpoint and after the last epoch.  After `load_training_state` the epochs are numbered on from the
         saved one and the loader continues the saved data order.  `metrics_every=k > 0` writes MIG / AAM of the model
         (`metrics-{epoch}.log`, `metric_helpers-{epoch}.pth`) after every epoch divisible by k and after the last one,
         computed from the loader's resident data (`disvae.evaluate.write_epoch_metrics`); `factor_score=True` adds the
-        FactorVAE score of those epochs (`factor_vae_score-{epoch}.log`, `factor_vae_score_helpers-{epoch}.pth`) and
-        `sap_score=True` the SAP score (`sap_score-{epoch}.log`, `sap_score_helpers-{epoch}.pth`).  Training itself is
-        unchanged."""
+        FactorVAE score of those epochs (`factor_vae_score-{epoch}.log`, `factor_vae_score_helpers-{epoch}.pth`),
+        `sap_score=True` the SAP score (`sap_score-{epoch}.log`, `sap_score_helpers-{epoch}.pth`) and
+        `beta_vae_score=True` the beta-VAE score (`beta_vae_score-{epoch}.log`, `beta_vae_score_helpers-{epoch}.pth`).
+        Training itself is unchanged."""
         start = default_timer()
         first, loader_state = (0, None) if self._resume is None else self._resume
         if loader_state is not None:
@@ -92,6 +94,7 @@ class Trainer():
             check_resident_metrics(data_loader, metrics_batch_size, self.device_data)
         check_epoch_factor_score(factor_score, metrics_every, data_loader, self.model.latent_dim)
         check_epoch_sap_score(sap_score, metrics_every, data_loader, self.model.latent_dim)
+        check_epoch_beta_vae_score(beta_vae_score, metrics_every, data_loader, self.model.latent_dim)
         self._resume = None
         if self.device_data and isinstance(data_loader, torch.utils.data.DataLoader):
             data_loader = self._device_loader(data_loader)
@@ -107,7 +110,7 @@ class Trainer():
                             save_state=save_state and (epoch % checkpoint_every == 0 or epoch == last))
             if metrics_every and (epoch % metrics_every == 0 or epoch == last):
                 write_epoch_metrics(self.model, data_loader, epoch, metrics_batch_size, self.save_dir, self.logger,
-                                    factor_score, sap_score)
+                                    factor_score, sap_score, beta_vae_score)
         self._end_training(start)
 
     def _end_epoch(self, epoch, storer, mean_epoch_loss, checkpoint_every, save_state=False):

@@ -368,6 +368,41 @@ int dv_sap_score_matrix(const float* mu, int ld, int row_stride, int N, int D, c
                         const int* test_cls, const int* n_classes, const int* counts, int K, int class_stride,
                         double C, float* score, double* coef, int* iters, void* stream);
 
+/* ---- disentanglement metrics: beta-VAE score (Higgins et al. 2017, section 3) -------------------
+ * dv_pair_abs_diff_mean: x[v][d] = (sum_{l < L} |mu[rows_a[v][l]][d] - mu[rows_b[v][l]][d]|) / L in fp64, the
+ * differences of the fp32 values taken in fp64 and added in ascending l (an in-order fp64 sum gives the same bits).
+ * mu is read as dv_group_variance reads it (element (n, d) at n*row_stride + d*ld; q_zCx in place).  rows_a, rows_b:
+ * int64 [V][L], every entry in [0, N) (not checked).  x: fp64 [V][D].  One launch, no workspace, deterministic,
+ * graph-capturable.
+ * DV_ERR_BAD_SHAPE: N < 1, D < 1, V < 1, L < 1 or V*D > INT_MAX.
+ * DV_ERR_BAD_ARG: a NULL pointer, or one misaligned (mu 4 bytes, the others 8). */
+int dv_pair_abs_diff_mean(const float* mu, int ld, int row_stride, int N, int D, const long long* rows_a,
+                          const long long* rows_b, int V, int L, double* x, void* stream);
+
+/* dv_logistic_fit: the exact minimiser of sklearn's LogisticRegression(C=1) objective (L2 on the weights, unpenalised
+ * intercept) on the first num_train rows of x (fp64 [num_train + num_eval][D]) and their class indices labels (int32
+ * [num_train], 0 .. nc-1), with nc = *n_classes read from device memory (1 .. K; clamped to that range).
+ *   nc > 2: multinomial, 1/2 |W|_F^2 + sum_i -log softmax(W x_i + b)_{y_i} over nc rows of (W, b), reported with
+ *           sum_c b_c = 0;
+ *   nc = 2: one binary model, 1/2 |w|^2 + sum_i log(1 + exp(-s_i (w.x_i + b))), s_i = +1 for class 1;
+ *   nc = 1: no fit.
+ * Solved in fp64 by truncated Newton (diagonally preconditioned conjugate gradient on Hessian-vector products over
+ * features centred on their training mean, Armijo line search), to max |gradient| <= 1e-10 of the largest scale of
+ * the gradient's parts (|weight| + sum_i |q_i x_i|).
+ *   coef  fp64 [K][D + 1]: row c = (W_c, b_c) for c < nc (nc > 2) or row 0 = (w, b) (nc = 2); NaN elsewhere
+ *   pred  int32 [num_train + num_eval]: argmax_c W_c x + b_c, the lowest c on a tie; class 1 if w.x + b > 0 for nc = 2;
+ *         0 for nc = 1
+ *   iters int32 [1]: Newton steps taken, -1 if 100 did not converge (or the line search failed); 0 for nc = 1
+ * workspace: dv_logistic_fit_workspace_bytes(num_train, D, K) bytes, 8-byte aligned, contents irrelevant.  One launch
+ * of one CTA.  Deterministic (fixed-order reductions, no floating-point atomics), graph-capturable.
+ * DV_ERR_BAD_SHAPE: num_train < 1, num_eval < 0, D < 1, D > 128, K < 1, K > 32, or (num_train + num_eval)*D > INT_MAX.
+ * DV_ERR_BAD_ARG: a NULL pointer, or one misaligned (x, coef and workspace 8 bytes, the others 4).
+ * DV_ERR_WORKSPACE: workspace NULL or smaller than the query. */
+size_t dv_logistic_fit_workspace_bytes(int num_train, int D, int K);   /* 0 for an unsupported shape */
+int dv_logistic_fit(const double* x, int D, int num_train, int num_eval, const int* labels, const int* n_classes,
+                    int K, double* coef, int* pred, int* iters, void* workspace, size_t workspace_bytes,
+                    void* stream);
+
 /* ---- FactorVAE pieces ---------------------------------------------------------------------
  * dv_permute_dims replaces _permute_dims (losses.py:483-508): out[b][d] = z[perm[d][b]][d].
  * perms != NULL: int64 [D][B] (the reference's CPU randperm stream, trap T7).  perms == NULL:

@@ -140,6 +140,12 @@ static bool conv_shape_ok(int B, int H, int W, int CH, int hi_nchw) {
   return false;
 }
 
+// The alignment contract of the conv entry points (include/disvae_b200.h): the tensor-core kernels read activations
+// and packed weights through TMA, the image kernels move activations, masks and workspaces as 16-byte vectors; bias,
+// weight-gradient, channel-sum and bit-word operands are read or written as single words.  NULL passes (optional
+// operands are checked for presence elsewhere).
+static bool aligned(const void* p, uintptr_t bytes) { return ((uintptr_t)p & (bytes - 1)) == 0; }
+
 }  // namespace dv
 
 namespace dv {
@@ -202,6 +208,10 @@ int dv_conv_down(const float* hi, const float* w_packed, const float* bias, cons
   if (mask_bits && !mask) return DV_ERR_BAD_ARG;               // the words accelerate the float mask, they do not replace it
   if (!conv_shape_ok(B, H, W, CH, hi_nchw)) return DV_ERR_BAD_SHAPE;
   if (act != DV_ACT_NONE && act != DV_ACT_RELU) return DV_ERR_BAD_ARG;
+  if (!aligned(hi, 16) || !aligned(w_packed, 16) || !aligned(mask, 16) || !aligned(lo, 16) ||
+      !aligned(colsum_workspace, 16) || !aligned(bias, 4) || !aligned(colsum_out, 4) || !aligned(mask_bits, 4) ||
+      !aligned(relu_bits_out, 4))
+    return DV_ERR_BAD_ARG;
   if (colsum_out && !colsum_workspace) return DV_ERR_WORKSPACE;
   cudaStream_t st = as_stream(stream);
   float* part = colsum_out ? reinterpret_cast<float*>(colsum_workspace) : nullptr;
@@ -223,6 +233,9 @@ int dv_conv_up(const float* lo, const float* w_packed, const float* bias, const 
   if (act != DV_ACT_NONE && act != DV_ACT_RELU && act != DV_ACT_SIGMOID) return DV_ERR_BAD_ARG;
   if (act == DV_ACT_SIGMOID && CH == 32) return DV_ERR_BAD_ARG;          // sigmoid only follows the image layer
   if ((mask || relu_bits_out) && CH != 32) return DV_ERR_BAD_ARG;        // mask epilogues of the 32-channel kernel only
+  if (!aligned(lo, 16) || !aligned(w_packed, 16) || !aligned(mask, 16) || !aligned(hi, 16) || !aligned(bias, 4) ||
+      !aligned(mask_bits, 4) || !aligned(relu_bits_out, 4))
+    return DV_ERR_BAD_ARG;
   if (CH == 32)
     return tc::conv_up_halo(lo, w_packed + kPackTcSection, bias, mask, hi, B, H, W, act, as_stream(stream), mask_bits,
                             relu_bits_out);
@@ -238,6 +251,8 @@ int dv_conv_wgrad(const float* lo, const float* hi, float* dw, float* dbias_lo, 
                   size_t workspace_bytes, int B, int H, int W, int CH, int hi_nchw, void* stream) {
   if (!lo || !hi || !dw || !workspace) return DV_ERR_BAD_ARG;
   if (!conv_shape_ok(B, H, W, CH, hi_nchw)) return DV_ERR_BAD_SHAPE;
+  if (!aligned(lo, 16) || !aligned(hi, 16) || !aligned(workspace, 16) || !aligned(dw, 4) || !aligned(dbias_lo, 4))
+    return DV_ERR_BAD_ARG;
   if (workspace_bytes < dv_conv_wgrad_workspace_bytes(B, H, W, CH)) return DV_ERR_WORKSPACE;
   float* ws = reinterpret_cast<float*>(workspace);
   cudaStream_t st = as_stream(stream);

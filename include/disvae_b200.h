@@ -73,6 +73,9 @@ long long dv_launch_count(void);
  *     32       4, 8 or 16             NHWC (hi_nchw == 0)
  * mask (optional, same shape/layout as the OUTPUT): out *= (mask > 0) -- the ReLU backward
  * of the layer that produced `mask`, fused into this epilogue.
+ * Alignment (one rule for every layer): activations (hi, lo), mask, w_packed and the workspaces must be 16-byte
+ * aligned; bias, dw, dbias_lo, colsum_out and the bit words (mask_bits, relu_bits_out) 4-byte aligned.  Otherwise
+ * dv_conv_down, dv_conv_up and dv_conv_wgrad return DV_ERR_BAD_ARG before launching anything.
  */
 size_t dv_conv_packed_floats(int CH);                         /* size of w_packed in floats */
 int dv_conv_pack_weights(const float* w, float* w_packed, int CH, void* stream);

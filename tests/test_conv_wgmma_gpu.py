@@ -1,6 +1,6 @@
-"""The 32-channel down and up convolutions (wgmma kernels of dv_conv_tc.cu) at the shapes of the training steps, with
-every epilogue those steps use, against fp64; and the determinism of a whole c2 training step across Trainers of one
-fresh process and with the weight-gradient side stream on or off."""
+"""The determinism of a whole c2 training step (whose 32-channel convolutions run on the wgmma kernels of
+dv_conv_tc.cu) across Trainers of one fresh process and with the weight-gradient side stream on or off.  The kernels
+themselves are checked against fp64 in test_conv_paths_gpu.py."""
 import collections
 import logging
 import os
@@ -10,89 +10,10 @@ import tempfile
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DEV = torch.device("cuda", 0)
-TOL = 4e-6          # of the output scale: fp32-grade (single-pass tf32 lands near 5e-4)
-
-
-def nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
-
-
-def rel_err(a, b):
-    a, b = a.double(), b.double()
-    return ((a - b).abs().max() / b.abs().max().clamp_min(1e-30)).item()
-
-
-def words(t):
-    """[t > 0] of a [..., 32] tensor as one int32 word per pixel (bit c = channel c)."""
-    bits = (t > 0).to(torch.int64) << torch.arange(32, device=t.device)
-    w = bits.sum(-1)
-    return torch.where(w >= 2 ** 31, w - 2 ** 32, w).to(torch.int32)
-
-
-# batch per GPU of c2 (1x64x64), c3 (3x64x64) and c5 (3x64x64, z=64); the 32-channel layers of both networks run at
-# lo 16, 8 and 4 on 64x64 images
-SHAPES = [(B, H) for B in (1024, 512, 256) for H in (16, 8, 4)]
-
-
-@pytest.mark.parametrize("B,H", SHAPES)
-def test_conv_down_epilogues_vs_fp64(B, H):
-    from disvae import ops
-    torch.manual_seed(B + H)
-    x = torch.randn(B, 32, 2 * H, 2 * H, device=DEV)
-    w = torch.randn(32, 32, 4, 4, device=DEV) * 0.1
-    b = torch.randn(32, device=DEV)
-    wp = ops.conv_pack(w, 32)
-    hi = nhwc(x)
-    ref = nhwc(F.conv2d(x.double(), w.double(), None, stride=2, padding=1))            # [B, H, H, 32]
-
-    # encoder forward: bias, ReLU, [out > 0] words for the backward pass
-    lo, bits = ops.conv_down(hi, wp, b, None, B, H, H, 32, 0, ops.ACT_RELU, want_bits=True)
-    want = torch.relu(ref + b.double())
-    assert rel_err(lo, want) <= TOL
-    assert torch.equal(bits, words(lo))
-    lo2, bits2 = ops.conv_down(hi, wp, b, None, B, H, H, 32, 0, ops.ACT_RELU, want_bits=True)
-    assert torch.equal(lo, lo2) and torch.equal(bits, bits2)
-
-    # decoder backward: no activation, float mask with its words, channel sums of the result
-    mask = torch.randn(B, H, H, 32, device=DEV)
-    g, cs = ops.conv_down(hi, wp, None, mask, B, H, H, 32, 0, ops.ACT_NONE, want_colsum=True, mask_bits=words(mask))
-    want = ref * (mask > 0)
-    assert rel_err(g, want) <= TOL
-    assert rel_err(cs, want.sum((0, 1, 2))) <= TOL
-    # ... and the float mask alone (the decoder's first layer)
-    g1 = ops.conv_down(hi, wp, None, mask, B, H, H, 32, 0, ops.ACT_NONE)
-    assert torch.equal(g1, g)
-
-
-@pytest.mark.parametrize("B,H", SHAPES)
-def test_conv_up_epilogues_vs_fp64(B, H):
-    from disvae import ops
-    torch.manual_seed(B + H + 1)
-    lo_nchw = torch.randn(B, 32, H, H, device=DEV)
-    w = torch.randn(32, 32, 4, 4, device=DEV) * 0.1
-    b = torch.randn(32, device=DEV)
-    wp = ops.conv_pack(w, 32)
-    lo = nhwc(lo_nchw)
-    ref = nhwc(F.conv_transpose2d(lo_nchw.double(), w.double(), None, stride=2, padding=1))   # [B, 2H, 2H, 32]
-
-    # decoder forward: bias, ReLU, [out > 0] words
-    hi, bits = ops.conv_up(lo, wp, b, None, B, H, H, 32, 0, ops.ACT_RELU, want_bits=True)
-    want = torch.relu(ref + b.double())
-    assert rel_err(hi, want) <= TOL
-    assert torch.equal(bits, words(hi))
-    hi2, bits2 = ops.conv_up(lo, wp, b, None, B, H, H, 32, 0, ops.ACT_RELU, want_bits=True)
-    assert torch.equal(hi, hi2) and torch.equal(bits, bits2)
-
-    # encoder backward: no activation, float mask with its words, and the float mask alone
-    mask = torch.randn(B, 2 * H, 2 * H, 32, device=DEV)
-    g = ops.conv_up(lo, wp, None, mask, B, H, H, 32, 0, ops.ACT_NONE, mask_bits=words(mask))
-    assert rel_err(g, ref * (mask > 0)) <= TOL
-    assert torch.equal(ops.conv_up(lo, wp, None, mask, B, H, H, 32, 0, ops.ACT_NONE), g)
 
 
 def _c2_trainer(seed):

@@ -29,199 +29,10 @@ def assert_close(a, b, tol=RTOL, what=""):
     assert e <= tol, "%s: rel err %.3e > %.1e" % (what, e, tol)
 
 
-def nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
-
-
-def nchw(t):
-    return t.permute(0, 3, 1, 2).contiguous()
-
-
 @pytest.fixture(scope="module")
 def ops():
     from disvae import ops as _ops
     return _ops
-
-
-def relu_words(t):
-    """[t > 0] of a [..., 32] tensor as one int32 word per pixel (bit c = channel c)."""
-    w = ((t > 0).long() << torch.arange(32, device=t.device)).sum(-1)
-    return torch.where(w >= 2 ** 31, w - 2 ** 32, w).int()
-
-
-CONV_CASES = [  # (B, H(lo), CH)
-    (3, 16, 1), (2, 32, 3), (5, 16, 32), (4, 8, 32), (7, 4, 32), (3, 2 * 2, 32), (2, 32, 1), (1, 16, 3),
-    (170, 16, 32),      # 340 tiles of 128 pixels: several tiles per persistent CTA (pipeline phase wrap-around)
-    (301, 8, 32), (1201, 4, 32),
-    (40, 32, 1), (40, 32, 3),      # image-boundary layers, 320 tiles
-    (100, 32, 1),                  # halo up kernel: 1100 tiles, > 5 per CTA (every shared-memory stage is reused)
-    (330, 32, 1), (300, 16, 3),    # col2im up kernel: several images per persistent CTA (carry row reset between images)
-]
-
-
-@pytest.mark.parametrize("B,H,CH", CONV_CASES)
-@pytest.mark.parametrize("act", [0, 1])
-def test_conv_down_matches_conv2d(ops, B, H, CH, act):
-    torch.manual_seed(B * 100 + H + CH)
-    x = torch.randn(B, CH, 2 * H, 2 * H)
-    w = torch.randn(32, CH, 4, 4) * 0.1
-    b = torch.randn(32)
-    ref = F.conv2d(x, w, b, stride=2, padding=1)
-    if act:
-        ref = torch.relu(ref)
-    wp = ops.conv_pack(w.to(dev()), CH)
-    hi = x.to(dev()) if CH < 32 else nhwc(x).to(dev())
-    lo = ops.conv_down(hi, wp, b.to(dev()), None, B, H, H, CH, int(CH < 32), act)
-    assert_close(nchw(lo.cpu()), ref, what="down")
-    # mask epilogue (ReLU backward of the producer of `mask`)
-    mask = torch.randn(B, 32, H, H)
-    lo2 = ops.conv_down(hi, wp, None, nhwc(mask).to(dev()), B, H, H, CH, int(CH < 32), 0)
-    ref2 = F.conv2d(x, w, None, stride=2, padding=1) * (mask > 0)
-    assert_close(nchw(lo2.cpu()), ref2, what="down+mask")
-    # channel sums of the output from the same launch (bias gradient of the previous ConvTranspose2d)
-    lo3, cs = ops.conv_down(hi, wp, None, nhwc(mask).to(dev()), B, H, H, CH, int(CH < 32), 0, want_colsum=True)
-    assert torch.equal(lo3, lo2)
-    assert_close(cs.cpu(), ref2.double().sum((0, 2, 3)).float(), tol=2e-5, what="down+mask column sums")
-    _, cs2 = ops.conv_down(hi, wp, None, nhwc(mask).to(dev()), B, H, H, CH, int(CH < 32), 0, want_colsum=True)
-    assert torch.equal(cs, cs2)                                # fixed reduction order
-    # ReLU masks as one word per pixel: produced by the forward epilogue, consumed instead of the 128-byte float rows
-    lo4, bits = ops.conv_down(hi, wp, b.to(dev()), None, B, H, H, CH, int(CH < 32), act, want_bits=True)
-    assert torch.equal(lo4, lo)
-    assert torch.equal(bits, relu_words(lo4))
-    mbits = relu_words(nhwc(mask).to(dev()))
-    lo5, cs5 = ops.conv_down(hi, wp, None, nhwc(mask).to(dev()), B, H, H, CH, int(CH < 32), 0, want_colsum=True, mask_bits=mbits)
-    assert torch.equal(lo5, lo2) and torch.equal(cs5, cs)
-
-
-@pytest.mark.parametrize("B,H,CH", CONV_CASES)
-@pytest.mark.parametrize("act", [0, 1, 2])
-def test_conv_up_matches_conv_transpose2d(ops, B, H, CH, act):
-    torch.manual_seed(B * 100 + H + CH + 7)
-    lo = torch.randn(B, 32, H, H)
-    w = torch.randn(32, CH, 4, 4) * 0.1
-    b = torch.randn(CH)
-    ref = F.conv_transpose2d(lo, w, b, stride=2, padding=1)
-    ref = torch.relu(ref) if act == 1 else (torch.sigmoid(ref) if act == 2 else ref)
-    wp = ops.conv_pack(w.to(dev()), CH)
-    if CH == 32 and act == 2:                                  # the sigmoid only ever follows the image layer
-        with pytest.raises(RuntimeError, match="bad argument"):
-            ops.conv_up(nhwc(lo).to(dev()), wp, b.to(dev()), None, B, H, H, CH, 0, act)
-        return
-    hi = ops.conv_up(nhwc(lo).to(dev()), wp, b.to(dev()), None, B, H, H, CH, int(CH < 32), act)
-    got = hi.cpu() if CH < 32 else nchw(hi.cpu())
-    assert_close(got, ref, what="up")
-    if CH == 32:
-        mask = torch.randn(B, 32, 2 * H, 2 * H)
-        hi2 = ops.conv_up(nhwc(lo).to(dev()), wp, None, nhwc(mask).to(dev()), B, H, H, CH, 0, 0)
-        ref2 = F.conv_transpose2d(lo, w, None, stride=2, padding=1) * (mask > 0)
-        assert_close(nchw(hi2.cpu()), ref2, what="up+mask")
-        hi3 = ops.conv_up(nhwc(lo).to(dev()), wp, None, nhwc(mask).to(dev()), B, H, H, CH, 0, 0,
-                          mask_bits=relu_words(nhwc(mask).to(dev())))
-        assert torch.equal(hi3, hi2)
-        hi4, bits = ops.conv_up(nhwc(lo).to(dev()), wp, b.to(dev()), None, B, H, H, CH, 0, act, want_bits=True)
-        assert torch.equal(hi4, hi) and torch.equal(bits, relu_words(hi4))
-
-
-@pytest.mark.parametrize("B,H,CH", CONV_CASES + [(64, 16, 32), (33, 32, 3)])
-def test_conv_wgrad_matches_autograd(ops, B, H, CH):
-    torch.manual_seed(B * 100 + H + CH + 13)
-    x = torch.randn(B, CH, 2 * H, 2 * H)
-    w = torch.zeros(32, CH, 4, 4, requires_grad=True)
-    b = torch.zeros(32, requires_grad=True)
-    g = torch.randn(B, 32, H, H)
-    (F.conv2d(x, w, b, stride=2, padding=1) * g).sum().backward()
-    hi = x.to(dev()) if CH < 32 else nhwc(x).to(dev())
-    dw, db = ops.conv_wgrad(nhwc(g).to(dev()), hi, B, H, H, CH, int(CH < 32), True)
-    assert_close(dw.cpu(), w.grad, what="dw")
-    assert_close(db.cpu(), b.grad, what="db")
-    # determinism of the split-K reduction
-    dw2, _ = ops.conv_wgrad(nhwc(g).to(dev()), hi, B, H, H, CH, int(CH < 32), True)
-    assert torch.equal(dw, dw2)
-
-
-@pytest.mark.parametrize("B,H,CH", [(5, 32, 1), (333, 32, 1), (150, 32, 3), (77, 16, 1), (200, 16, 3)])
-def test_conv_up_small_fp32_grade_accuracy(ops, B, H, CH):
-    """Decoder output layer (col2im tensor-core kernel): <= 4e-6 of the output scale against fp64, pre-activation
-    and through the sigmoid."""
-    torch.manual_seed(B + H + CH)
-    lo = torch.randn(B, 32, H, H)
-    w = torch.randn(32, CH, 4, 4) * 0.1
-    b = torch.randn(CH)
-    wp = ops.conv_pack(w.to(dev()), CH)
-    ref = F.conv_transpose2d(lo.double(), w.double(), b.double(), stride=2, padding=1)
-    got = ops.conv_up(nhwc(lo).to(dev()), wp, b.to(dev()), None, B, H, H, CH, 1, 0).cpu()
-    assert_close(got, ref, tol=4e-6, what="up small vs fp64")
-    got_s = ops.conv_up(nhwc(lo).to(dev()), wp, b.to(dev()), None, B, H, H, CH, 1, 2).cpu()
-    assert_close(got_s, torch.sigmoid(ref), tol=4e-6, what="up small sigmoid vs fp64")
-
-
-@pytest.mark.parametrize("B,H", [(16, 16), (9, 8), (40, 4), (200, 16), (330, 16), (700, 8)])
-def test_conv32_kernels_fp32_grade_accuracy(ops, B, H):
-    """The tensor-core (3xTF32) path must stay at fp32-grade accuracy, not tf32-grade: error against an
-    fp64 reference <= 4e-6 of the output scale (plain fp32 lands around 5e-7, single-pass tf32 at 5e-4)."""
-    torch.manual_seed(B + H)
-    x = torch.randn(B, 32, 2 * H, 2 * H)
-    lo = torch.randn(B, 32, H, H)
-    w = torch.randn(32, 32, 4, 4) * 0.1
-    wp = ops.conv_pack(w.to(dev()), 32)
-    ref_d = F.conv2d(x.double(), w.double(), None, stride=2, padding=1)
-    got_d = nchw(ops.conv_down(nhwc(x).to(dev()), wp, None, None, B, H, H, 32, 0, 0).cpu())
-    assert_close(got_d, ref_d, tol=4e-6, what="down vs fp64")
-    ref_u = F.conv_transpose2d(lo.double(), w.double(), None, stride=2, padding=1)
-    got_u = nchw(ops.conv_up(nhwc(lo).to(dev()), wp, None, None, B, H, H, 32, 0, 0).cpu())
-    assert_close(got_u, ref_u, tol=4e-6, what="up vs fp64")
-    wz = torch.zeros(32, 32, 4, 4, dtype=torch.float64, requires_grad=True)
-    (F.conv2d(x.double(), wz, None, stride=2, padding=1) * lo.double()).sum().backward()
-    dw, db = ops.conv_wgrad(nhwc(lo).to(dev()), nhwc(x).to(dev()), B, H, H, 32, 0, True)
-    assert_close(dw.cpu(), wz.grad, tol=4e-6, what="wgrad vs fp64")
-    assert_close(db.cpu(), lo.double().sum((0, 2, 3)), tol=4e-6, what="dbias vs fp64")
-
-
-def test_conv_transpose_weight_gradient_is_same_kernel(ops):
-    """dW of ConvTranspose2d(32 -> CH) == wgrad(lo = its input, hi = grad of its output)."""
-    torch.manual_seed(3)
-    for CH, H in ((3, 16), (32, 8)):                          # the decoder's last layer on 32x32 images, a 32->32 layer
-        B = 4
-        lo = torch.randn(B, 32, H, H)
-        w = torch.zeros(32, CH, 4, 4, requires_grad=True)
-        g = torch.randn(B, CH, 2 * H, 2 * H)
-        (F.conv_transpose2d(lo, w, None, stride=2, padding=1) * g).sum().backward()
-        hi = g.to(dev()) if CH < 32 else nhwc(g).to(dev())
-        dw, _ = ops.conv_wgrad(nhwc(lo).to(dev()), hi, B, H, H, CH, int(CH < 32), False)
-        assert_close(dw.cpu(), w.grad, what="convT dw CH=%d" % CH)
-
-
-def test_conv_entry_points_refuse_shapes_outside_the_burgess_layers():
-    """The conv entry points take exactly the layers of the Burgess networks on 32x32 and 64x64 images (CH in {1,3}:
-    lo 16 or 32; CH = 32: lo 4, 8 or 16; lo square) and refuse everything else before launching anything.  The image
-    layer's up kernel has no mask epilogue, so a float mask there is refused as well.  Every buffer is a real device
-    buffer of the size the geometry needs."""
-    from disvae import _native as N
-    L, st, p = N.lib(), N.stream(), (lambda t: t.data_ptr())
-    BAD_SHAPE, BAD_ARG = -1, -2
-
-    def buffers(B, H, W, CH):
-        hi = torch.randn(B * CH * 4 * H * W, device=dev())
-        lo = torch.randn(B * H * W * 32, device=dev())
-        wp = torch.zeros(L.dv_conv_packed_floats(CH), device=dev())
-        return hi, lo, wp
-
-    for B, H, W, CH in [(2, 8, 8, 3), (2, 64, 64, 1), (2, 32, 32, 32), (2, 8, 16, 32), (2, 32, 16, 3)]:
-        nchw = int(CH != 32)
-        hi, lo, wp = buffers(B, H, W, CH)
-        dw = torch.empty(32 * CH * 16, device=dev())
-        ws = torch.empty(2 * 132 * (16 * CH + 1) * 32, device=dev())
-        what = "B=%d H=%d W=%d CH=%d" % (B, H, W, CH)
-        assert L.dv_conv_down(p(hi), p(wp), None, None, p(lo), B, H, W, CH, nchw, 0, None, None, None, None, st) == BAD_SHAPE, what
-        assert L.dv_conv_up(p(lo), p(wp), None, None, p(hi), B, H, W, CH, nchw, 0, None, None, st) == BAD_SHAPE, what
-        assert L.dv_conv_wgrad_workspace_bytes(B, H, W, CH) == 0, what
-        assert L.dv_conv_wgrad(p(lo), p(hi), p(dw), None, p(ws), ws.numel() * 4, B, H, W, CH, nchw, st) == BAD_SHAPE, what
-    for CH in (1, 3):
-        B, H = 2, 16
-        hi, lo, wp = buffers(B, H, H, CH)
-        mask = torch.ones_like(hi)
-        assert L.dv_conv_up(p(lo), p(wp), None, p(mask), p(hi), B, H, H, CH, 1, 0, None, None, st) == BAD_ARG, CH
-    torch.cuda.synchronize()
 
 
 def test_channel_sum_and_transpose_and_act_bwd(ops):

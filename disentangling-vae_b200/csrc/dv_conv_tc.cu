@@ -30,6 +30,33 @@ constexpr int kSmemMax = 232448;             // 227 KB per block on sm_90
 
 __device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers * 32) : "memory"); }
 
+// The two consumer warpgroups of the up kernel take their epilogues in turn, so that while one drains its
+// accumulators and stores, the other has MMAs queued on the tensor cores.  Named barrier 2 passes the turn from
+// warpgroup 0 to warpgroup 1, barrier 3 from 1 to 0; the passing warpgroup arrives, the other waits (128 + 128
+// threads).  Every pass is followed by a wait of the passer before its next pass, so a barrier never collects two
+// passes of one warpgroup.  Start-up: warpgroup 0 passes once in the middle of its first output phase and warpgroup 1
+// waits for that before its first MMA, then passes straight back: warpgroup 1 runs half a phase behind.
+// Warpgroup 0 takes the last pass with one more wait before it exits.
+__device__ __forceinline__ void epilogue_turn_wait(int wg) { named_bar_sync(3 - wg, kConsumers * 32); }
+__device__ __forceinline__ void epilogue_turn_pass(int wg) { named_bar_arrive(2 + wg, kConsumers * 32); }
+
+// The ReLU-backward mask of output pixel p for this thread's channels (8 nt + 2 t + e) as a bit word: mask_bits[p]
+// when given, else [mask > 0] of the float mask, else all ones (also for a pixel past the end).  Called ahead of the
+// MMAs whose outputs it masks (down: before the tile's taps, up: before the phase's products), so the loads run under them.
+__device__ __forceinline__ uint32_t mask_word(const uint32_t* __restrict__ mask_bits, const float* __restrict__ mask,
+                                              long long p, bool valid, int t) {
+  if (!valid || (!mask_bits && !mask)) return 0xffffffffu;
+  if (mask_bits) return __ldg(mask_bits + p);
+  uint32_t mb = 0u;
+#pragma unroll
+  for (int nt = 0; nt < 4; ++nt) {
+    const int c = nt * 8 + 2 * t;
+    const float2 m2 = __ldg(reinterpret_cast<const float2*>(mask + p * 32 + c));
+    mb |= (m2.x > 0.f ? 1u : 0u) << c | (m2.y > 0.f ? 1u : 0u) << (c + 1);
+  }
+  return mb;
+}
+
 // Once a product's commit groups are complete: its hi*hi is added to the fp32 total.  tot[4 nt + e] (like every
 // accumulator here) is element e of n-tile nt in the m16n8 accumulator layout.
 __device__ __forceinline__ void fold_tap(float (&tot)[16], float (&acc)[16]) {
@@ -156,6 +183,17 @@ conv_down32_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     if (++stage == kDownStages) { stage = 0; phase ^= 1; }
   };
   for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
+    // the ReLU-backward mask of this thread's two rows, one word per pixel (bit c = channel c), requested before the
+    // tile's 16 taps so that its latency hides under them
+    long long p[2];
+    bool valid[2];
+    uint32_t mb[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      p[h] = (long long)tile * 128 + r0 + 8 * h;
+      valid[h] = p[h] < g.total_px;
+      mb[h] = mask_word(mask_bits, mask, p[h], valid[h], t);
+    }
     float tot[16] = {}, corr[16], acc[2][16];
 #pragma unroll
     for (int i = 0; i < 16; ++i) acc[1][i] = 0.f;           // folded while tap 0 runs
@@ -169,11 +207,6 @@ conv_down32_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     fence_regs(corr);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const long long p = (long long)tile * 128 + r0 + 8 * h;
-      const bool valid = p < g.total_px;
-      uint32_t mb = 0xffffffffu;                             // ReLU-backward mask as one word per pixel (bit c = channel c)
-      if (mask_bits && valid) mb = __ldg(mask_bits + p);
-      const float* mk = (mask && !mask_bits && valid) ? mask + p * 32 : nullptr;
       uint32_t ob = 0u;
 #pragma unroll
       for (int nt = 0; nt < 4; ++nt) {
@@ -183,20 +216,16 @@ conv_down32_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         for (int e = 0; e < 2; ++e) {
           float x = (tot[4 * nt + 2 * h + e] + corr[4 * nt + 2 * h + e]) + bars->bias[c + e];
           if (act == DV_ACT_RELU) x = fmaxf(x, 0.f);
-          v[e] = ((mb >> (c + e)) & 1u) ? x : 0.f;
+          v[e] = ((mb[h] >> (c + e)) & 1u) ? x : 0.f;
         }
-        if (mk) {
-          const float2 m2 = __ldg(reinterpret_cast<const float2*>(mk + c));
-          v[0] = m2.x > 0.f ? v[0] : 0.f; v[1] = m2.y > 0.f ? v[1] : 0.f;
-        }
-        if (valid) *reinterpret_cast<float2*>(lo + p * 32 + c) = make_float2(v[0], v[1]);
+        if (valid[h]) *reinterpret_cast<float2*>(lo + p[h] * 32 + c) = make_float2(v[0], v[1]);
         else v[0] = v[1] = 0.f;
         ob |= (v[0] > 0.f ? 1u : 0u) << c | (v[1] > 0.f ? 1u : 0u) << (c + 1);
         csum[nt][0] += v[0]; csum[nt][1] += v[1];
       }
       ob |= __shfl_xor_sync(0xffffffffu, ob, 1);
       ob |= __shfl_xor_sync(0xffffffffu, ob, 2);
-      if (bits_out && valid && t == 0) bits_out[p] = ob;     // [x > 0] of the stored pixel: the next backward pass's mask
+      if (bits_out && valid[h] && t == 0) bits_out[p[h]] = ob;  // [x > 0] of the stored pixel: the next backward pass's mask
     }
   }
   if (colsum_part) {                                         // fixed-order reduction: lanes of a quad column, then warps
@@ -474,6 +503,9 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
   }
   uint32_t ah[16], al[16];
   mbar_wait(&bars->b_full, 0);
+  const int wg = warp >> 2;
+  if (wg == 1) { epilogue_turn_wait(1); epilogue_turn_pass(1); }
+  bool lead = wg == 0;                                       // warpgroup 0 before its start-up pass
   uint32_t t_seq = 0;
   for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x, ++t_seq) {
     const int stage = t_seq % kHaloStages;
@@ -487,6 +519,21 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
 #pragma unroll 1
     for (int pidx = 0; pidx < 4; ++pidx) {
       const int ph = pidx >> 1, pw = pidx & 1;
+      // output pixel of this thread's row h in this phase (valid: inside the batch and the tile's rows)
+      auto out_pixel = [&](int h, bool& valid) -> long long {
+        const int r = warp * 16 + gq + 8 * h, tr = r / g.W;
+        const int tb = tr / g.TR, rr = tr - tb * g.TR;
+        const int b = b0 + tb, i = i0 + rr, j = r - tr * g.W;
+        valid = r < g.valid_rows && b < g.B && i < g.H;
+        return valid ? ((long long)(b * HH + 2 * i + ph) * WW + 2 * j + pw) : 0;
+      };
+      uint32_t mb[2];                                        // requested before the phase's products, used after them
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        bool valid;
+        const long long opix = out_pixel(h, valid);
+        mb[h] = mask_word(mask_bits, mask, opix, valid, t);
+      }
       float tot[16] = {}, corr[16], acc[2][16];
 #pragma unroll
       for (int i = 0; i < 16; ++i) acc[1][i] = 0.f;         // folded while product 0 runs
@@ -503,20 +550,16 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
           keep[h] = ok ? 0xffffffffu : 0u;
         }
         product(acc[q & 1], acc[(q + 1) & 1], corr, tot, ah, al, a_base, p[0], p[1], keep[0], keep[1], t, b_base, q);
+        if (q == 1 && lead) { epilogue_turn_pass(0); lead = false; }
       }
+      epilogue_turn_wait(wg);
       wgmma_wait<0>();
       fold_tap(tot, acc[1]);
       fence_regs(corr);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int r = warp * 16 + gq + 8 * h, tr = r / g.W;
-        const int tb = tr / g.TR, rr = tr - tb * g.TR;
-        const int b = b0 + tb, i = i0 + rr, j = r - tr * g.W;
-        const bool valid = r < g.valid_rows && b < g.B && i < g.H;
-        const long long opix = valid ? ((long long)(b * HH + 2 * i + ph) * WW + 2 * j + pw) : 0;
-        uint32_t mb = 0xffffffffu;
-        if (mask_bits && valid) mb = __ldg(mask_bits + opix);
-        const float* mk = (mask && !mask_bits && valid) ? mask + opix * 32 : nullptr;
+        bool valid;
+        const long long opix = out_pixel(h, valid);
         uint32_t ob = 0u;
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) {
@@ -526,11 +569,7 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
           for (int e = 0; e < 2; ++e) {
             float x = (tot[4 * nt + 2 * h + e] + corr[4 * nt + 2 * h + e]) + bars->bias[c + e];
             if (act == DV_ACT_RELU) x = fmaxf(x, 0.f);
-            v[e] = ((mb >> (c + e)) & 1u) ? x : 0.f;
-          }
-          if (mk) {
-            const float2 m2 = __ldg(reinterpret_cast<const float2*>(mk + c));
-            v[0] = m2.x > 0.f ? v[0] : 0.f; v[1] = m2.y > 0.f ? v[1] : 0.f;
+            v[e] = ((mb[h] >> (c + e)) & 1u) ? x : 0.f;
           }
           if (valid) *reinterpret_cast<float2*>(hi_out + opix * 32 + c) = make_float2(v[0], v[1]);
           ob |= (v[0] > 0.f ? 1u : 0u) << c | (v[1] > 0.f ? 1u : 0u) << (c + 1);
@@ -539,10 +578,12 @@ conv_up_halo_mma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
         ob |= __shfl_xor_sync(0xffffffffu, ob, 2);
         if (bits_out && valid && t == 0) bits_out[opix] = ob;  // [x > 0] of the stored pixel
       }
+      epilogue_turn_pass(wg);
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&bars->raw_empty[stage]);
   }
+  if (wg == 0) epilogue_turn_wait(0);
 }
 
 // ---- weight packing ----------------------------------------------------------------------

@@ -42,6 +42,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// ---- named barriers -----------------------------------------------------------------
+// Barrier `id` completes once `count` threads (whole warps) have reached it: bar.sync counts this warp and waits,
+// bar.arrive counts it and goes on (the signalling side of a producer / consumer hand-off).
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // one 32-bit word of shared memory (explicit ld.shared: 32-bit address arithmetic)
 __device__ __forceinline__ uint32_t lds32(uint32_t smem_addr) {
   uint32_t v;

@@ -10,6 +10,7 @@
 // Reference call sites replaced: disvae/models/encoders.py:73-77 (Conv2d+ReLU),
 // disvae/models/decoders.py:77-82 (ConvTranspose2d+ReLU/sigmoid) and their autograd
 // backward (disvae/training.py:157).
+#include <climits>
 #include "dv_common.cuh"
 
 namespace dv {
@@ -115,7 +116,7 @@ __global__ void act_bwd_kernel(const float* __restrict__ dy, const float* __rest
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float yv = y[i], d = dy[i];
     float r;
-    if (act == DV_ACT_SIGMOID) r = d * ((1.f - yv) * yv);      // aten sigmoid_backward: grad * (1 - y) * y
+    if (act == DV_ACT_SIGMOID) r = (d * (1.f - yv)) * yv;      // aten sigmoid_backward: grad * (1 - y) * y, left to right
     else if (act == DV_ACT_RELU) r = yv > 0.f ? d : 0.f;
     else if (act == DV_ACT_LEAKY) r = yv > 0.f ? d : d * slope;
     else r = d;
@@ -272,8 +273,8 @@ int dv_channel_sum(const float* x, float* out, long long rows, int C, int nchw, 
   cudaStream_t st = as_stream(stream);
   int nb;
   if (nchw) {
-    if (hw <= 0) return DV_ERR_BAD_SHAPE;
-    nb = (int)(rows < kCsBlocks ? rows : kCsBlocks);
+    if (hw <= 0 || rows > INT_MAX) return DV_ERR_BAD_SHAPE;   // the kernel counts images in int
+    nb =(int)(rows < kCsBlocks ? rows : kCsBlocks);
     channel_sum_nchw_kernel<<<nb, 256, 0, st>>>(x, partial, (int)rows, C, hw);
   } else {
     nb = grid_for(rows, 8, kCsBlocks);
@@ -287,7 +288,7 @@ int dv_channel_sum(const float* x, float* out, long long rows, int C, int nchw, 
 
 int dv_flat_transpose(const float* src, float* dst, int B, int C, int S, int to_nhwc, void* stream) {
   if (!src || !dst) return DV_ERR_BAD_ARG;
-  if (B <= 0 || C <= 0 || S <= 0) return DV_ERR_BAD_SHAPE;
+  if (B <= 0 || C <= 0 || S <= 0 || (long long)C * S > INT_MAX) return DV_ERR_BAD_SHAPE;   // C * S indexes in int
   const long long n = (long long)B * C * S;
   flat_transpose_kernel<<<grid_for(n, 256, 8 * kNumSMs), 256, 0, as_stream(stream)>>>(src, dst, n, C, S, to_nhwc);
   return check_launch();
@@ -296,6 +297,7 @@ int dv_flat_transpose(const float* src, float* dst, int B, int C, int S, int to_
 int dv_act_bwd(const float* dy, const float* y, float* g, long long n, int act, float slope, void* stream) {
   if (!dy || !y || !g) return DV_ERR_BAD_ARG;
   if (n <= 0) return DV_ERR_BAD_SHAPE;
+  if (act != DV_ACT_NONE && act != DV_ACT_RELU && act != DV_ACT_SIGMOID && act != DV_ACT_LEAKY) return DV_ERR_BAD_ARG;
   act_bwd_kernel<<<grid_for(n, 256, 16 * kNumSMs), 256, 0, as_stream(stream)>>>(dy, y, g, n, act, slope);
   return check_launch();
 }

@@ -15,6 +15,7 @@
 //   dv_act_bwd_chansum    ConvTranspose2d output layer backward prologue: g = dy * act'(y) (decoders.py:82 sigmoid) fused
 //                         with the per-channel sum of g (that layer's bias gradient) -- one pass instead of two
 #include <algorithm>
+#include <climits>
 #include "dv_common.cuh"
 
 namespace dv {
@@ -208,9 +209,9 @@ act_bwd_chansum_kernel(const float* __restrict__ dy, const float* __restrict__ y
     for (int i = threadIdx.x; i < hw4; i += blockDim.x) {
       const float4 d = dy4[i], yv = y4[i];
       float4 r;
-      if (act == DV_ACT_SIGMOID) {                             // aten sigmoid_backward: grad * (1 - y) * y
-        r.x = d.x * ((1.f - yv.x) * yv.x); r.y = d.y * ((1.f - yv.y) * yv.y);
-        r.z = d.z * ((1.f - yv.z) * yv.z); r.w = d.w * ((1.f - yv.w) * yv.w);
+      if (act == DV_ACT_SIGMOID) {                             // aten sigmoid_backward: grad * (1 - y) * y, left to right
+        r.x = (d.x * (1.f - yv.x)) * yv.x; r.y = (d.y * (1.f - yv.y)) * yv.y;
+        r.z = (d.z * (1.f - yv.z)) * yv.z; r.w = (d.w * (1.f - yv.w)) * yv.w;
       } else if (act == DV_ACT_RELU) {
         r.x = yv.x > 0.f ? d.x : 0.f; r.y = yv.y > 0.f ? d.y : 0.f; r.z = yv.z > 0.f ? d.z : 0.f; r.w = yv.w > 0.f ? d.w : 0.f;
       } else if (act == DV_ACT_LEAKY) {
@@ -378,7 +379,12 @@ int dv_loss_record(const long long* step, const dv_loss_log* log, void* stream) 
 int dv_act_bwd_chansum(const float* dy, const float* y, float* g, int B, int C, int hw, int act, float slope, float* chansum,
                        void* workspace, void* stream) {
   if (!dy || !y || !g || !chansum || !workspace) return DV_ERR_BAD_ARG;
-  if (B < 1 || C < 1 || C > 4 || hw < 4 || (hw & 3)) return DV_ERR_BAD_SHAPE;
+  if (B < 1 || C < 1 || C > 4 || hw < 4 || (hw & 3) || (long long)B * C > INT_MAX) return DV_ERR_BAD_SHAPE;
+  if (act != DV_ACT_NONE && act != DV_ACT_RELU && act != DV_ACT_SIGMOID && act != DV_ACT_LEAKY) return DV_ERR_BAD_ARG;
+  // dy, y and g move as float4; the partial rows and the sums as single words
+  if (((uintptr_t)dy & 15) || ((uintptr_t)y & 15) || ((uintptr_t)g & 15) || ((uintptr_t)chansum & 3) ||
+      ((uintptr_t)workspace & 3))
+    return DV_ERR_BAD_ARG;
   const int planes = B * C;
   const int grid = planes < 296 ? planes : 296;                // <= dv_channel_sum_workspace_bytes() / 128 partial rows
   float* partial = reinterpret_cast<float*>(workspace);

@@ -109,13 +109,21 @@ size_t dv_conv_wgrad_workspace_bytes(int B, int H, int W, int CH);
 int dv_conv_wgrad(const float* lo, const float* hi, float* dw, float* dbias_lo, void* workspace,
                   size_t workspace_bytes, int B, int H, int W, int CH, int hi_nchw, void* stream);
 /* out[C] = sum over all pixels of x; x is [rows, C] pixel-major (nchw == 0) or
- * [B, C, HW] (nchw != 0, rows = B, hw given).  Bias gradients of the ConvTranspose2d layers. */
+ * [B, C, HW] (nchw != 0, rows = B, hw given).  Bias gradients of the ConvTranspose2d layers.
+ * DV_ERR_BAD_SHAPE: C < 1, C > 32, rows < 1, or (nchw != 0) hw < 1 or rows > INT_MAX. */
 size_t dv_channel_sum_workspace_bytes(void);
 int dv_channel_sum(const float* x, float* out, long long rows, int C, int nchw, int hw,
                    void* workspace, void* stream);
-/* [B,32,4,4] <-> [B,4,4,32] re-ordering at the conv/linear seam (encoders.py:80, decoders.py:74) */
+/* [B,32,4,4] <-> [B,4,4,32] re-ordering at the conv/linear seam (encoders.py:80, decoders.py:74): [B][C][S] ->
+ * [B][S][C] (to_nhwc != 0) or back.  DV_ERR_BAD_SHAPE: B, C or S < 1, or C * S > INT_MAX. */
 int dv_flat_transpose(const float* src, float* dst, int B, int C, int S, int to_nhwc, void* stream);
-/* g = dy * act'(y) for y = act(.) : sigmoid (decoders.py:82) backward.  n elements. */
+/* g = dy * act'(y) for y = act(.) over n elements, as autograd computes it from the activation's output y:
+ *   SIGMOID  aten sigmoid_backward, (dy * (1 - y)) * y in that order (decoders.py:82)
+ *   RELU     dy where y > 0, else +0 (aten threshold_backward(dy, y, 0), except at y = NaN: 0 here, dy there;
+ *            every ReLU mask of this library is [y > 0])
+ *   LEAKY    dy where y > 0, else dy * slope (aten leaky_relu_backward with self_is_result)
+ *   NONE     dy
+ * DV_ERR_BAD_ARG: a NULL pointer or act outside these four.  DV_ERR_BAD_SHAPE: n < 1. */
 int dv_act_bwd(const float* dy, const float* y, float* g, long long n, int act, float slope, void* stream);
 
 /* ---- fully connected -------------------------------------------------------------
@@ -313,7 +321,11 @@ int dv_betab_loss_bwd(const float* g, const float* rec_kl, const float* consts, 
  * combination (FactorVAE's discriminator loss). */
 int dv_loss_record(const long long* step, const dv_loss_log* log, void* stream);
 /* g = dy * act'(y) over an NCHW tensor [B, C <= 4, hw] fused with chansum[c] = sum_{b,hw} g (the bias gradient of the
- * ConvTranspose2d that produced y; decoders.py:82).  workspace: dv_channel_sum_workspace_bytes(). */
+ * ConvTranspose2d that produced y; decoders.py:82).  g is bit-identical to dv_act_bwd's (same act codes and rounding).
+ * workspace: dv_channel_sum_workspace_bytes().
+ * DV_ERR_BAD_SHAPE: B < 1, C < 1, C > 4, hw < 4, hw % 4 != 0 or B * C > INT_MAX.
+ * DV_ERR_BAD_ARG: a NULL pointer, act outside {NONE, RELU, SIGMOID, LEAKY}, dy, y or g not 16-byte aligned (they move
+ * as float4), chansum or workspace not 4-byte aligned; nothing is launched then. */
 int dv_act_bwd_chansum(const float* dy, const float* y, float* g, int B, int C, int hw, int act, float slope,
                        float* chansum, void* workspace, void* stream);
 

@@ -35,22 +35,6 @@ def ops():
     return _ops
 
 
-def test_channel_sum_and_transpose_and_act_bwd(ops):
-    torch.manual_seed(5)
-    x = torch.randn(1000, 32)
-    assert_close(ops.channel_sum(x.to(dev()), 1000, 32, 0, 0).cpu(), x.sum(0), tol=1e-5)
-    y = torch.randn(37, 3, 64 * 64)
-    assert_close(ops.channel_sum(y.to(dev()), 37, 3, 1, 64 * 64).cpu(), y.sum((0, 2)), tol=1e-5)
-    t = torch.randn(9, 32, 16)                                 # [B, C, S] NCHW-flat
-    got = ops.flat_transpose(t.view(9, 512).to(dev()), 9, to_nhwc=True).cpu().view(9, 16, 32)
-    assert torch.equal(got, t.permute(0, 2, 1))
-    back = ops.flat_transpose(got.reshape(9, 512).to(dev()), 9, to_nhwc=False).cpu().view(9, 32, 16)
-    assert torch.equal(back, t)
-    yy = torch.sigmoid(torch.randn(4096) * 4)
-    dy = torch.randn(4096)
-    assert_close(ops.act_bwd(dy.to(dev()), yy.to(dev()), 2).cpu(), dy * (1 - yy) * yy, tol=1e-6)
-
-
 @pytest.mark.parametrize("dist", ["bernoulli", "gaussian", "laplace"])
 def test_vae_loss_kernel(ops, golden, dist):
     from disvae._native import DIST
@@ -359,39 +343,6 @@ def test_u8_to_f32_is_totensor(ops):
         assert torch.equal(got, u.float().div(255))
     u = torch.arange(256, dtype=torch.uint8).repeat(64)          # every byte value
     assert torch.equal(ops.u8_to_f32(u.to(dev())).cpu(), u.float().div(255))
-
-
-def test_loss_combine_and_act_bwd_chansum(ops):
-    torch.manual_seed(1)
-    a = torch.randn(12, requires_grad=True)
-    b = torch.randn(3, requires_grad=True)
-    ca, cb = [1.0, 0.37], [1.0, 6.0, 0.25]
-    ref = ca[0] * a[0] + ca[1] * a[1] + (cb[0] * b[0] + cb[1] * b[1] + cb[2] * b[2])
-    (ref * 1.7).backward()
-    ad, bd = a.detach().to(dev()).requires_grad_(True), b.detach().to(dev()).requires_grad_(True)
-    got = ops.LossCombineFn.apply(ad, bd, ca, cb)
-    assert abs(got.item() - ref.item()) <= 1e-6 * abs(ref.item())
-    (got * 1.7).backward()
-    assert torch.allclose(ad.grad.cpu(), a.grad, rtol=1e-6, atol=0) and torch.allclose(bd.grad.cpu(), b.grad, rtol=1e-6, atol=0)
-    # 0-dim second operand (FactorVAE tc), and none at all
-    t = torch.tensor(0.8, requires_grad=True)
-    td = t.detach().to(dev()).requires_grad_(True)
-    got2 = ops.LossCombineFn.apply(ad.detach(), td, [1.0, 1.0], [6.4])
-    assert abs(got2.item() - (a[0] + a[1] + 6.4 * t).item()) < 1e-5
-    got2.backward()
-    assert abs(td.grad.item() - 6.4) < 1e-6 and td.grad.shape == td.shape
-    got3 = ops.LossCombineFn.apply(ad.detach(), None, [1.0, 4.0], None)
-    assert abs(got3.item() - (a[0] + 4 * a[1]).item()) < 1e-5
-    # sigmoid backward + per-channel sums in one pass == the two separate kernels
-    for B, C, S in ((37, 3, 64), (5, 1, 32), (300, 1, 64)):
-        y = torch.sigmoid(torch.randn(B, C, S, S) * 3).to(dev())
-        dy = torch.randn(B, C, S, S).to(dev())
-        g, cs = ops.act_bwd_chansum(dy, y, 2)
-        g_ref = ops.act_bwd(dy, y, 2)
-        assert torch.equal(g, g_ref)
-        assert_close(cs.cpu(), g_ref.double().sum((0, 2, 3)).float().cpu(), tol=2e-5, what="chansum")
-        _, cs2 = ops.act_bwd_chansum(dy, y, 2)
-        assert torch.equal(cs, cs2)
 
 
 def test_conv_pack_multi_equals_per_layer_pack(ops):

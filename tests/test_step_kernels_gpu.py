@@ -8,7 +8,6 @@ references written here, at training shapes and at the input edges where fp32 ke
 - dv_reparam_fwd/bwd: z = mu + exp(lv/2) eps, with eps injected or drawn on the device from Philox4x32-10 at the
   counters offset + i, restated on the host (`host_eps`).
 - dv_factor_tc_*, dv_factor_ce_* (csrc/dv_factor.cu): the FactorVAE heads, one 256-thread block for any h.
-- dv_act_bwd_chansum (csrc/dv_glue.cu): the output layer's sigmoid backward fused with the bias gradient.
 - dv_adam_step, dv_adam_multi and disvae.fused.FusedAdam against CPU torch.optim.Adam(foreach=False).
 
 Every direct C-ABI call here writes into buffers followed by a band of sentinel NaN bit patterns that must survive.
@@ -38,7 +37,6 @@ KL_TOL = 1e-6          # KL per dimension and total, relative to 0.5 sum(1 + |lv
 GRAD_ULPS = 8          # gradients and z, per element, in units of U times the magnitude of the terms
 EPS_TOL = 1e-6         # device noise, per element, relative to 1 + |eps|
 FACTOR_TOL = 2e-7      # TC and CE values, relative to the magnitude summed
-CHANSUM_TOL = 1e-7     # per-channel sums, relative to sum |g|
 ADAM_ULPS = 2          # one Adam step from identical state, exp_avg and exp_avg_sq per element
 ADAM_P_ULPS = 4        # ... p per element: m / denom, the step size and the subtraction each round once more
 ADAM_CHAIN_TOL = 2e-6  # 200 Adam steps, per element, relative to |p0| + the path |p| travelled
@@ -730,45 +728,7 @@ def test_factor_heads_match_the_fp64_reference(h, regime):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# 4. output-layer prologue
-# ---------------------------------------------------------------------------------------------------------------------
-@pytest.mark.gpu
-@pytest.mark.parametrize("C", [1, 3])
-@pytest.mark.parametrize("B", [1, 97, 2048])
-def test_act_bwd_chansum(B, C):
-    """g bit-identical to act_bwd; per-channel sums vs fp64 within CHANSUM_TOL sum|g|.  B x C planes of 64 x 64 run
-    on min(planes, 296) blocks, which the workspace rows it writes show."""
-    from disvae import ops
-    N = _native()
-    g0 = torch.Generator().manual_seed(B * C)
-    y = torch.sigmoid(3 * torch.randn(B, C, 64, 64, generator=g0)).cuda()
-    dy = torch.randn(B, C, 64, 64, generator=g0).cuda()
-    g, cs = ops.act_bwd_chansum(dy, y, N.ACT_SIGMOID)
-    assert torch.equal(_bits(g), _bits(ops.act_bwd(dy, y, N.ACT_SIGMOID)))
-    gd = g.double().cpu()
-    want = gd.sum((0, 2, 3))
-    mag = gd.abs().sum((0, 2, 3))
-    e = ((cs.double().cpu() - want).abs() / mag).max().item()
-    # raw call on guarded buffers: same bits, grid visible in the partial rows
-    ws_floats = N.lib().dv_channel_sum_workspace_bytes() // 4
-    n = y.numel()
-    dyg, yg, gg, csg, ws = _guarded_copy(dy), _guarded_copy(y), _guarded(n), _guarded(C), _guarded(ws_floats)
-    before = N.lib().dv_launch_count()
-    N.call("dv_act_bwd_chansum", dyg.data_ptr(), yg.data_ptr(), gg.data_ptr(), B, C, 64 * 64, N.ACT_SIGMOID, 0.0,
-           csg.data_ptr(), ws.data_ptr(), N.stream())
-    assert N.lib().dv_launch_count() - before == 2
-    torch.cuda.synchronize()
-    assert _intact(gg, n) and _intact(csg, C) and _intact(ws, ws_floats)
-    assert torch.equal(_bits(gg[:n]), _bits(g.view(-1))) and torch.equal(_bits(csg[:C]), _bits(cs))
-    rows = ws[:ws_floats].view(-1, 32)
-    grid = min(B * C, 296)
-    assert torch.isfinite(rows[:grid, :C]).all() and torch.isnan(rows[grid:]).all()
-    print("act_bwd_chansum B=%d C=%d grid %d: chansum err %.2e" % (B, C, grid, e))
-    assert e <= CHANSUM_TOL, e
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# 5. Adam
+# 4. Adam
 # ---------------------------------------------------------------------------------------------------------------------
 def _adam_state(n, step0, seed):
     g = torch.Generator().manual_seed(seed)

@@ -2,14 +2,18 @@
 // Observations", eq. 6 for DIP-VAE-I and the second form of section 3 for DIP-VAE-II).  The reference has no DIP-VAE;
 // the entry points are declared in include/disvae_b200.h.
 //
-//   c_b   = mu_b - m,  m = s + mean_b(mu_b - s) with s = mu_0 (row 0): near s the differences are exact in fp32, so the
-//           offset of a column never enters a rounded sum (a plain fp32 mean of 2048 values near 100 is off by 1e-5..1e-4)
+//   c_b   = (mu_b - m1) - r,  m1 = s + mean_b(mu_b - s) with s = mu_0 (row 0),  r = mean_b(mu_b - m1)
+//           Near s the differences are exact in fp32, so the offset of a column never enters a rounded sum (a plain
+//           fp32 mean of 2048 values near 100 is off by 1e-5..1e-4).  But when row 0 is an outlier every mu_b - s is
+//           rounded at the outlier's scale and m1 is off by about that much; the second pass takes the differences
+//           from m1, which is within a few ulps of the batch's spread of the true mean, so c_b is within a few u |c_b|
+//           plus the mean's rounding of the spread, wherever the column sits and whichever row comes first.
 //   C     = (1/B) sum_b c_b c_b^T            (+ diag(mean_b exp(logvar_b)) for DIP-VAE-II)
 //   od    = sum_{i != j} C_ij^2,   dd = sum_i (C_ii - 1)^2
 //   d/dmu_b     = (2/B) G c_b,  G_ij = 2 g_od C_ij (i != j),  G_ii = 2 g_dd (C_ii - 1)
 //   d/dlogvar_bi = G_ii exp(logvar_bi) / B   (DIP-VAE-II)
 //
-// Forward: two launches.  dip_mean_kernel takes the shifted column means (one CTA per column) and zeroes the counters;
+// Forward: two launches.  dip_mean_kernel takes m1 and r (one CTA per column, two passes) and zeroes the counters;
 // dip_cov_kernel runs one CTA per (32x32 tile of C, chunk of the batch), writes the tile's partial sum over its chunk
 // and the last CTA of a tile (counter) sums the chunks in chunk order; the last tile (second counter) sums the tiles'
 // (od, dd) in tile order.  Backward: one launch, one CTA per 32 rows x 32 columns of the mu gradient.  Every sum has a
@@ -25,15 +29,16 @@ constexpr int kDipTileElems = kDipTile * kDipTile;
 constexpr int kDipThreads = 256;                   // 32 rows x 8 threads, 4 columns each (stride 8)
 constexpr int kDipTargetCtas = 2 * kNumSMs;        // the batch is split until the covariance pass has about this many CTAs
 constexpr int kDipMinChunk = 64;                   // ... or its chunks have this many rows
+constexpr int kDipMaxB = 65535 * kDipTile;         // the backward's grid y is ceil(B / 32)
 
 size_t round4(size_t n) { return (n + 3) & ~size_t(3); }
 
-// Workspace layout (floats, each piece a multiple of 16 bytes): counters [ntiles + 1] (unsigned), r [D] (shifted column
-// means), v [D] (column means of exp(logvar), DIP-VAE-II), C [D][D], chunk partials [nchunks][ntiles][32 * 32],
-// tile (od, dd) [ntiles][2].
+// Workspace layout (floats, each piece a multiple of 16 bytes): counters [ntiles + 1] (unsigned), m1 [D] (shifted
+// column means), r [D] (column means of mu - m1), v [D] (column means of exp(logvar), DIP-VAE-II), C [D][D], chunk
+// partials [nchunks][ntiles][32 * 32], tile (od, dd) [ntiles][2].
 struct DipPlan {
   int tps, ntiles, chunk, nchunks;
-  size_t r, v, c, part, red, total;
+  size_t m, r, v, c, part, red, total;
 };
 
 DipPlan dip_plan(int B, int D) {
@@ -47,7 +52,8 @@ DipPlan dip_plan(int B, int D) {
   const int rows = (B + want - 1) / want;
   p.chunk = (rows + kDipTile - 1) / kDipTile * kDipTile;
   p.nchunks = (B + p.chunk - 1) / p.chunk;
-  p.r = round4((size_t)p.ntiles + 1);
+  p.m = round4((size_t)p.ntiles + 1);
+  p.r = p.m + round4(D);
   p.v = p.r + round4(D);
   p.c = p.v + round4(D);
   p.part = p.c + round4((size_t)D * D);
@@ -72,11 +78,14 @@ __device__ __forceinline__ float2 dip_block_sum2(float a, float b, float2* red /
   return t;
 }
 
-// One CTA per column d: r[d] = mean_b(mu[b][d] - mu[0][d]), v[d] = mean_b exp(logvar[b][d]) (DIP-VAE-II).
+// One CTA per column d: m1[d] = mu[0][d] + mean_b(mu[b][d] - mu[0][d]), r[d] = mean_b(mu[b][d] - m1[d]),
+// v[d] = mean_b exp(logvar[b][d]) (DIP-VAE-II).
 __global__ void __launch_bounds__(kDipThreads)
 dip_mean_kernel(const float* __restrict__ mu, const float* __restrict__ logvar, int ld, int rs, int B, int dip_type,
-                float* __restrict__ r, float* __restrict__ v, unsigned* __restrict__ cnt, int ncnt) {
+                float* __restrict__ m, float* __restrict__ r, float* __restrict__ v, unsigned* __restrict__ cnt,
+                int ncnt) {
   __shared__ float2 wred[kDipThreads / 32];
+  __shared__ float m1_s;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < ncnt; i += gridDim.x * blockDim.x) cnt[i] = 0u;
   const int d = blockIdx.x;
   const float s = mu[(long long)d * ld];
@@ -88,16 +97,25 @@ dip_mean_kernel(const float* __restrict__ mu, const float* __restrict__ logvar, 
     if (dip_type == DV_DIP_II) e += expf(logvar[o]);
   }
   const float2 sum = dip_block_sum2(t, e, wred);
+  if (threadIdx.x == 0) m1_s = s + sum.x / (float)B;
+  __syncthreads();
+  const float m1 = m1_s;
+  float t2 = 0.f;
+#pragma unroll 4
+  for (int b = threadIdx.x; b < B; b += kDipThreads) t2 += mu[(long long)b * rs + (long long)d * ld] - m1;
+  const float2 sum2 = dip_block_sum2(t2, 0.f, wred);
   if (threadIdx.x == 0) {
-    r[d] = sum.x / (float)B;
+    m[d] = m1;
+    r[d] = sum2.x / (float)B;
     v[d] = sum.y / (float)B;
   }
 }
 
 __global__ void __launch_bounds__(kDipThreads)
 dip_cov_kernel(const float* __restrict__ mu, int ld, int rs, int B, int D, int dip_type, int tps, int chunk,
-               const float* __restrict__ r, const float* __restrict__ v, float* __restrict__ C, float* __restrict__ part,
-               float* __restrict__ red, unsigned* __restrict__ cnt, float* __restrict__ terms) {
+               const float* __restrict__ m, const float* __restrict__ r, const float* __restrict__ v,
+               float* __restrict__ C, float* __restrict__ part, float* __restrict__ red, unsigned* __restrict__ cnt,
+               float* __restrict__ terms) {
   __shared__ float sa[kDipTile][kDipTile + 1], sb[kDipTile][kDipTile + 1];
   __shared__ float shift[2][kDipTile], rmean[2][kDipTile];
   __shared__ float2 wred[kDipThreads / 32];
@@ -107,7 +125,7 @@ dip_cov_kernel(const float* __restrict__ mu, int ld, int rs, int B, int D, int d
   const int t = threadIdx.x, ty = t >> 3, tx = t & 7;
   if (t < 2 * kDipTile) {
     const int side = t >> 5, col = (side ? j0 : i0) + (t & 31);
-    shift[side][t & 31] = col < D ? mu[(long long)col * ld] : 0.f;
+    shift[side][t & 31] = col < D ? m[col] : 0.f;
     rmean[side][t & 31] = col < D ? r[col] : 0.f;
   }
   __syncthreads();
@@ -194,8 +212,8 @@ dip_cov_kernel(const float* __restrict__ mu, int ld, int rs, int B, int D, int d
 
 __global__ void __launch_bounds__(kDipThreads)
 dip_bwd_kernel(const float* __restrict__ mu, const float* __restrict__ logvar, int ld, int rs, int B, int D, int dip_type,
-               const float* __restrict__ r, const float* __restrict__ C, const float* __restrict__ g_terms,
-               float* __restrict__ g_mu, float* __restrict__ g_logvar) {
+               const float* __restrict__ m, const float* __restrict__ r, const float* __restrict__ C,
+               const float* __restrict__ g_terms, float* __restrict__ g_mu, float* __restrict__ g_logvar) {
   __shared__ float sc[kDipTile][kDipTile + 1];     // centred mu [b][j]
   __shared__ float sg[kDipTile][kDipTile + 1];     // G [j][i]
   const int i0 = blockIdx.x * kDipTile, b0 = blockIdx.y * kDipTile;
@@ -208,7 +226,7 @@ dip_bwd_kernel(const float* __restrict__ mu, const float* __restrict__ logvar, i
       const int e = t + kDipThreads * k, row = e >> 5, col = e & 31;
       const int b = b0 + row, j = j0 + col;
       float x = 0.f;
-      if (b < B && j < D) x = (mu[(long long)b * rs + (long long)j * ld] - mu[(long long)j * ld]) - r[j];
+      if (b < B && j < D) x = (mu[(long long)b * rs + (long long)j * ld] - m[j]) - r[j];
       sc[row][col] = x;
       const int jj = j0 + row, ii = i0 + col;
       float g = 0.f;
@@ -249,8 +267,10 @@ dip_bwd_kernel(const float* __restrict__ mu, const float* __restrict__ logvar, i
 
 bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
 
-int dip_check(const float* mu, const float* logvar, int B, int D, int dip_type, const void* ws) {
-  if (B < 1 || D < 1 || D > 1024 || (dip_type != DV_DIP_I && dip_type != DV_DIP_II)) return DV_ERR_BAD_SHAPE;
+bool bad_dims(int B, int D) { return B < 1 || B > kDipMaxB || D < 1 || D > 1024; }
+
+int dip_check(const float* mu, const float* logvar, int ld, int rs, int B, int D, int dip_type, const void* ws) {
+  if (bad_dims(B, D) || ld < 1 || rs < 1 || (dip_type != DV_DIP_I && dip_type != DV_DIP_II)) return DV_ERR_BAD_SHAPE;
   if (!mu || !logvar || !ws) return DV_ERR_BAD_ARG;
   if (misaligned(mu, 4) || misaligned(logvar, 4) || misaligned(ws, 16)) return DV_ERR_BAD_ARG;
   return DV_OK;
@@ -264,39 +284,39 @@ using namespace dv;
 extern "C" {
 
 size_t dv_dip_workspace_bytes(int B, int D) {
-  if (B < 1 || D < 1 || D > 1024) return 0;
+  if (bad_dims(B, D)) return 0;
   return dip_plan(B, D).total * sizeof(float);
 }
 
 int dv_dip_fwd(const float* mu, const float* logvar, int ld, int row_stride, int B, int D, int dip_type,
                float* terms_out, void* workspace, void* stream) {
-  int rc = dip_check(mu, logvar, B, D, dip_type, workspace);
+  int rc = dip_check(mu, logvar, ld, row_stride, B, D, dip_type, workspace);
   if (rc != DV_OK) return rc;
   if (!terms_out || misaligned(terms_out, 4)) return DV_ERR_BAD_ARG;
   const DipPlan p = dip_plan(B, D);
   float* ws = reinterpret_cast<float*>(workspace);
   unsigned* cnt = reinterpret_cast<unsigned*>(ws);
-  dip_mean_kernel<<<D, kDipThreads, 0, as_stream(stream)>>>(mu, logvar, ld, row_stride, B, dip_type, ws + p.r, ws + p.v,
-                                                            cnt, p.ntiles + 1);
+  dip_mean_kernel<<<D, kDipThreads, 0, as_stream(stream)>>>(mu, logvar, ld, row_stride, B, dip_type, ws + p.m, ws + p.r,
+                                                            ws + p.v, cnt, p.ntiles + 1);
   rc = check_launch();
   if (rc != DV_OK) return rc;
   dip_cov_kernel<<<dim3(p.ntiles, p.nchunks), kDipThreads, 0, as_stream(stream)>>>(
-      mu, ld, row_stride, B, D, dip_type, p.tps, p.chunk, ws + p.r, ws + p.v, ws + p.c, ws + p.part, ws + p.red, cnt,
-      terms_out);
+      mu, ld, row_stride, B, D, dip_type, p.tps, p.chunk, ws + p.m, ws + p.r, ws + p.v, ws + p.c, ws + p.part,
+      ws + p.red, cnt, terms_out);
   return check_launch();
 }
 
 int dv_dip_bwd(const float* mu, const float* logvar, int ld, int row_stride, int B, int D, int dip_type,
                const float* g_terms, float* g_mu, float* g_logvar, const void* workspace, void* stream) {
-  int rc = dip_check(mu, logvar, B, D, dip_type, workspace);
+  int rc = dip_check(mu, logvar, ld, row_stride, B, D, dip_type, workspace);
   if (rc != DV_OK) return rc;
   if (!g_terms || misaligned(g_terms, 4) || misaligned(g_mu, 4) || misaligned(g_logvar, 4)) return DV_ERR_BAD_ARG;
   if (!g_mu && !g_logvar) return DV_OK;
   const DipPlan p = dip_plan(B, D);
   const float* ws = reinterpret_cast<const float*>(workspace);
   dip_bwd_kernel<<<dim3((D + kDipTile - 1) / kDipTile, (B + kDipTile - 1) / kDipTile), kDipThreads, 0,
-                   as_stream(stream)>>>(mu, logvar, ld, row_stride, B, D, dip_type, ws + p.r, ws + p.c, g_terms, g_mu,
-                                        g_logvar);
+                   as_stream(stream)>>>(mu, logvar, ld, row_stride, B, D, dip_type, ws + p.m, ws + p.r, ws + p.c,
+                                        g_terms, g_mu, g_logvar);
   return check_launch();
 }
 

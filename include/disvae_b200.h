@@ -238,21 +238,23 @@ int dv_btcvae_bwd_rows(int B, int D, int row0, int nrows, long long n_data, int 
  * Concepts from Unlabeled Observations"), the regulariser of eq. 6 (DIP-VAE-I) and of the second form in section 3
  * (DIP-VAE-II), on the batch of encoder outputs mu / logvar [B, D] (element (b, d) at b*row_stride + d*ld, as for
  * dv_vae_loss_fwd: the interleaved encoder output is read in place):
- *   Cov_mu = (1/B) sum_b (mu_b - m)(mu_b - m)^T   (biased; centred two-pass form, m = mu_0 + mean_b(mu_b - mu_0))
+ *   Cov_mu = (1/B) sum_b c_b c_b^T   (biased; c_b = (mu_b - m1) - mean_b(mu_b - m1), m1 = mu_0 + mean_b(mu_b - mu_0):
+ *            centred on an accurate mean, whatever the offset of a column and whichever row comes first)
  *   C = Cov_mu (DV_DIP_I)  or  Cov_mu + diag(mean_b exp(logvar_b)) (DV_DIP_II)
  *   terms_out[0] = od = sum_{i != j} C_ij^2,   terms_out[1] = dd = sum_i (C_ii - 1)^2   (unweighted)
  * The weights lambda_od, lambda_d and the annealing are applied by the caller (dv_loss_combine_sched_fwd).
  * workspace: dv_dip_workspace_bytes(B, D) bytes, 16-byte aligned, contents irrelevant on entry; the forward leaves the
  * column means and C in it for dv_dip_bwd, so pass the SAME workspace untouched.  Deterministic (fixed-order
  * reductions, no floating-point atomics).  logvar is read only by DV_DIP_II but must be a valid pointer for both.
- * DV_ERR_BAD_SHAPE: B < 1, D < 1, D > 1024 or dip_type not DV_DIP_I / DV_DIP_II.
+ * DV_ERR_BAD_SHAPE: B < 1, B > 65535 * 32 = 2097120 (the backward runs one CTA row per 32 rows of the batch), D < 1,
+ * D > 1024, ld < 1, row_stride < 1, or dip_type not DV_DIP_I / DV_DIP_II.
  * DV_ERR_BAD_ARG: a NULL required pointer, or mu / logvar / terms / gradients not 4-byte or workspace not 16-byte aligned.
  * Backward: g_terms = device float[2], the upstream gradient of (od, dd) (the lambdas and the annealing included);
- *   g_mu[b] = (2/B) G (mu_b - m) with G_ij = 2 g_terms[0] C_ij (i != j), G_ii = 2 g_terms[1] (C_ii - 1);
+ *   g_mu[b] = (2/B) G c_b with G_ij = 2 g_terms[0] C_ij (i != j), G_ii = 2 g_terms[1] (C_ii - 1);
  *   g_logvar[b][i] = G_ii exp(logvar[b][i]) / B for DV_DIP_II, 0 for DV_DIP_I.
  *   Outputs contiguous [B, D]; either may be NULL (both NULL: nothing is launched). */
 enum { DV_DIP_I = 1, DV_DIP_II = 2 };
-size_t dv_dip_workspace_bytes(int B, int D);      /* 0 for an unsupported shape */
+size_t dv_dip_workspace_bytes(int B, int D);      /* 0 for an unsupported B or D */
 int dv_dip_fwd(const float* mu, const float* logvar, int ld, int row_stride, int B, int D, int dip_type,
                float* terms_out, void* workspace, void* stream);
 int dv_dip_bwd(const float* mu, const float* logvar, int ld, int row_stride, int B, int D, int dip_type,

@@ -1,7 +1,7 @@
-"""DIP-VAE-I / DIP-VAE-II on the GPU: the covariance-penalty kernels against fp64 at training shapes and input edges,
-whole-model gradients against the fp64 oracle on the same ReLU branch, and the loss on every path a loss runs on --
-CUDA graph against eager (annealed, recording, uint8 batches), a sweep against lone runs, a resumed run against an
-uninterrupted one, and the Evaluator's test_losses.log."""
+"""DIP-VAE-I / DIP-VAE-II on the GPU: whole-model gradients against the fp64 oracle on the same ReLU branch, and the
+loss on every path a loss runs on -- CUDA graph against eager (annealed, recording, uint8 batches), a sweep against
+lone runs, a resumed run against an uninterrupted one, and the Evaluator's test_losses.log.  The covariance-penalty
+kernels themselves are tested path by path in test_dip_paths_gpu.py."""
 import json
 import logging
 import os
@@ -14,8 +14,6 @@ from oracle import disvae_oracle as O
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-DV_ERR_BAD_SHAPE, DV_ERR_BAD_ARG = -1, -2
-G_TERMS = (0.7, 1.3)                       # upstream gradient of (od, dd) in the kernel tests
 
 
 def dip64(mu, logvar, dip_type):
@@ -27,111 +25,6 @@ def dip64(mu, logvar, dip_type):
         C = C + torch.diag(logvar.exp().mean(0))
     d = torch.diagonal(C)
     return ((C - torch.diag(d)) ** 2).sum(), ((d - 1) ** 2).sum()
-
-
-# ---- the kernels against fp64 ----------------------------------------------------------------------------------------
-SHAPES = [(1, 10), (2, 10), (33, 7), (64, 10), (1000, 10), (1024, 10), (256, 64), (2048, 64), (1024, 1), (512, 1024)]
-REGIMES = ["normal", "offset", "collapsed", "collinear", "wide_logvar"]
-
-
-def _inputs(B, D, regime, seed):
-    g = torch.Generator().manual_seed(seed)
-    mu = torch.randn(B, D, generator=g)
-    lv = 0.5 * torch.randn(B, D, generator=g)
-    if regime == "offset":
-        mu = 100 + 0.01 * torch.randn(B, D, generator=g)
-    elif regime == "collapsed":
-        mu[:, D // 2] = 3.25
-    elif regime == "collinear":
-        mu[:, 1:] = mu[:, :1] + 1e-3 * torch.randn(B, D - 1, generator=g)
-    elif regime == "wide_logvar":
-        lv = torch.rand(B, D, generator=g) * 30 - 20
-    return mu, lv
-
-
-def _run(mu, lv, dip_type, interleaved=True):
-    """ops.DipFn on the encoder's interleaved [B, D, 2] layout (or contiguous mu / logvar) -> (terms, g_mu, g_logvar)."""
-    from disvae import ops
-    if interleaved:
-        ml = torch.stack([mu, lv], dim=-1).to(DEV).requires_grad_(True)
-        m, l = ml[..., 0], ml[..., 1]
-    else:
-        m, l = mu.to(DEV).requires_grad_(True), lv.to(DEV).requires_grad_(True)
-    terms = ops.DipFn.apply(m, l, dip_type)
-    terms.backward(torch.tensor(G_TERMS, device=DEV))
-    if interleaved:
-        return terms.detach(), ml.grad[..., 0].contiguous(), ml.grad[..., 1].contiguous()
-    return terms.detach(), m.grad, l.grad if l.grad is not None else torch.zeros_like(l)
-
-
-def _within(got, want, scale, tol, what):
-    err = (got.detach().double().cpu() - want).abs().max().item()
-    assert err <= tol * scale, "%s: |err| %.3e > %.1e x %.3e" % (what, err, tol, scale)
-
-
-@pytest.mark.parametrize("regime", REGIMES)
-@pytest.mark.parametrize("dip_type", ["I", "II"])
-@pytest.mark.parametrize("B,D", SHAPES, ids=["%dx%d" % s for s in SHAPES])
-def test_kernel_matches_fp64(B, D, dip_type, regime):
-    if regime == "wide_logvar" and dip_type == "I":
-        pytest.skip("DIP-VAE-I does not read logvar")
-    if regime == "collinear" and D < 2:
-        pytest.skip("one column")
-    mu, lv = _inputs(B, D, regime, seed=B * 7919 + D + len(regime))
-    m64, l64 = mu.double().requires_grad_(True), lv.double().requires_grad_(True)
-    od, dd = dip64(m64, l64, dip_type)
-    (G_TERMS[0] * od + G_TERMS[1] * dd).backward()
-    g_lv64 = l64.grad if l64.grad is not None else torch.zeros_like(l64)      # DIP-VAE-I: no dependence on logvar
-    terms, g_mu, g_lv = _run(mu, lv, dip_type)
-    _within(terms[0], od.detach(), max(abs(od.item()), 1.0), 1e-5, "od")
-    _within(terms[1], dd.detach(), max(abs(dd.item()), 1.0), 1e-5, "dd")
-    _within(g_mu, m64.grad, m64.grad.abs().max().item(), 1e-5, "g_mu")
-    _within(g_lv, g_lv64, g_lv64.abs().max().item(), 1e-5, "g_logvar")
-    if dip_type == "I":
-        assert not g_lv.any()
-    if B == 1:
-        assert not g_mu.any()                              # Cov_mu of one row is 0
-    # bit-identical on a second call, and from contiguous inputs
-    for again in (_run(mu, lv, dip_type), _run(mu, lv, dip_type, interleaved=False)):
-        for a, b in zip(again, (terms, g_mu, g_lv)):
-            assert torch.equal(a, b)
-
-
-def test_refusals_launch_nothing():
-    """Bad shapes, bad types and NULL or misaligned pointers come back as status codes with no launch."""
-    from disvae import _native as N
-    L, S = N.lib(), N.stream()
-    buf = torch.zeros(1 << 16, device=DEV)
-    a = buf.data_ptr()
-    terms = torch.full((2,), 7.0, device=DEV)
-    B, D = 8, 4
-
-    def refused(rc_want, fn, *args):
-        before = L.dv_launch_count()
-        rc = getattr(L, fn)(*args)
-        torch.cuda.synchronize()
-        assert rc == rc_want and L.dv_launch_count() == before, (fn, args, rc)
-
-    def fwd(mu=a, lv=a, B_=B, D_=D, t=1, out=terms.data_ptr(), ws=a):
-        return (mu, lv, 2, 2 * D_, B_, D_, t, out, ws, S)
-
-    def bwd(mu=a, lv=a, B_=B, D_=D, t=2, g=a, gm=a, gl=a, ws=a):
-        return (mu, lv, 2, 2 * D_, B_, D_, t, g, gm, gl, ws, S)
-
-    for shape in (dict(B_=0), dict(B_=-1), dict(D_=0), dict(D_=1025), dict(t=0), dict(t=3)):
-        refused(DV_ERR_BAD_SHAPE, "dv_dip_fwd", *fwd(**shape))
-        refused(DV_ERR_BAD_SHAPE, "dv_dip_bwd", *bwd(**shape))
-    for bad in (dict(mu=None), dict(lv=None), dict(out=None), dict(ws=None), dict(mu=a + 2), dict(lv=a + 1),
-                dict(out=terms.data_ptr() + 2), dict(ws=a + 4)):
-        refused(DV_ERR_BAD_ARG, "dv_dip_fwd", *fwd(**bad))
-    for bad in (dict(mu=None), dict(lv=None), dict(g=None), dict(ws=None), dict(g=a + 2), dict(gm=a + 2),
-                dict(gl=a + 3), dict(ws=a + 8)):
-        refused(DV_ERR_BAD_ARG, "dv_dip_bwd", *bwd(**bad))
-    refused(0, "dv_dip_bwd", *bwd(gm=None, gl=None))           # nothing asked for: nothing launched
-    assert torch.equal(terms, torch.full((2,), 7.0, device=DEV))
-    for b, d in ((0, 10), (10, 0), (10, 1025)):
-        assert L.dv_dip_workspace_bytes(b, d) == 0
-    assert L.dv_dip_workspace_bytes(1, 1) > 0 and L.dv_dip_workspace_bytes(2048, 1024) % 16 == 0
 
 
 # ---- whole-model gradients against the fp64 oracle on the same branch ---------------------------------------------

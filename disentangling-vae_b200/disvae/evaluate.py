@@ -14,6 +14,7 @@ import warnings
 from collections import defaultdict
 from functools import reduce
 from timeit import default_timer
+from typing import Callable, NamedTuple
 
 import torch
 from tqdm import tqdm
@@ -25,17 +26,11 @@ from disvae.utils.modelIO import save_metadata
 TEST_LOSSES_FILE = "test_losses.log"
 METRICS_FILENAME = "metrics.log"
 METRIC_HELPERS_FILE = "metric_helpers.pth"
-FACTOR_SCORE_FILENAME = "factor_vae_score.log"
-FACTOR_SCORE_HELPERS_FILE = "factor_vae_score_helpers.pth"
 FACTOR_SCORE_MIN_VAR = 0.05                # a dim whose global variance is below this is inactive (factor_vae.py)
 FACTOR_SCORE_MAX_DIM = 1024                # dv_group_variance's limit
-SAP_SCORE_FILENAME = "sap_score.log"
-SAP_SCORE_HELPERS_FILE = "sap_score_helpers.pth"
 SAP_MAX_DIM = 1024                         # dv_sap_score_matrix's limits: latents,
 SAP_MAX_TRAIN = 32768                      # training rows staged in shared memory,
 SAP_MAX_CLASSES = 256                      # and values of a scored factor
-BETA_VAE_SCORE_FILENAME = "beta_vae_score.log"
-BETA_VAE_SCORE_HELPERS_FILE = "beta_vae_score_helpers.pth"
 BETA_VAE_MAX_DIM = 128                     # dv_logistic_fit's limits: latents,
 BETA_VAE_MAX_FACTORS = 32                  # and scored factors (classes)
 EVAL_SEED_STRIDE = 0x9E3779B97F4A7C15      # odd 64-bit constant: consecutive epochs get unrelated seeds
@@ -46,19 +41,10 @@ def epoch_metrics_filenames(epoch):
     return "metrics-{}.log".format(epoch), "metric_helpers-{}.pth".format(epoch)
 
 
-def epoch_factor_score_filenames(epoch):
-    """(`factor_vae_score-{epoch}.log`, `factor_vae_score_helpers-{epoch}.pth`): the score after epoch `epoch`."""
-    return "factor_vae_score-{}.log".format(epoch), "factor_vae_score_helpers-{}.pth".format(epoch)
-
-
-def epoch_sap_score_filenames(epoch):
-    """(`sap_score-{epoch}.log`, `sap_score_helpers-{epoch}.pth`): the SAP score after epoch `epoch`."""
-    return "sap_score-{}.log".format(epoch), "sap_score_helpers-{}.pth".format(epoch)
-
-
-def epoch_beta_vae_score_filenames(epoch):
-    """(`beta_vae_score-{epoch}.log`, `beta_vae_score_helpers-{epoch}.pth`): the beta-VAE score after epoch `epoch`."""
-    return "beta_vae_score-{}.log".format(epoch), "beta_vae_score_helpers-{}.pth".format(epoch)
+def epoch_score_filenames(score, epoch):
+    """(`{stem}-{epoch}.log`, `{stem}_helpers-{epoch}.pth`): the files of `score` (an entry of SCORES) written after
+    training epoch `epoch`."""
+    return "{}-{}.log".format(score.stem, epoch), "{}_helpers-{}.pth".format(score.stem, epoch)
 
 
 def evaluation_seed(noise_key, epoch):
@@ -107,64 +93,66 @@ def check_resident_metrics(loader, metrics_batch_size, device_data):
         raise ValueError("metrics_batch_size must be positive, got %d" % int(metrics_batch_size))
 
 
-def check_epoch_factor_score(factor_score, metrics_every, loader, latent_dim):
-    """ValueError unless the FactorVAE score can be written with the metrics of every `metrics_every` epochs (after
-    `check_resident_metrics` has accepted `loader`).  No GPU work."""
-    if not factor_score:
-        return
-    if not metrics_every:
-        raise ValueError("factor_score=True needs metrics_every > 0: the score is written with the metrics of those "
-                         "epochs")
-    check_factor_score(loader.dataset, latent_dim)
+def select_scores(switches, prefix=""):
+    """The entries of SCORES, in table order, whose switch `prefix + flag` is true in the mapping `switches` (a
+    caller's keyword arguments: `factor_score=...` for a Trainer, `is_factor_score=...` for an Evaluator)."""
+    return tuple(s for s in SCORES if switches[prefix + s.flag])
 
 
-def check_epoch_sap_score(sap_score, metrics_every, loader, latent_dim):
-    """ValueError unless the SAP score can be written with the metrics of every `metrics_every` epochs (after
-    `check_resident_metrics` has accepted `loader`).  No GPU work."""
-    if not sap_score:
-        return
-    if not metrics_every:
-        raise ValueError("sap_score=True needs metrics_every > 0: the score is written with the metrics of those epochs")
-    check_sap_score(loader.dataset, latent_dim)
+def score_evaluator_args(scores, seed):
+    """The Evaluator keywords that write every score of `scores`, each drawn from a generator seeded with `seed`."""
+    args = {}
+    for s in scores:
+        args.update({"is_" + s.flag: True, s.flag + "_seed": seed})
+    return args
 
 
-def check_epoch_beta_vae_score(beta_vae_score, metrics_every, loader, latent_dim):
-    """ValueError unless the beta-VAE score can be written with the metrics of every `metrics_every` epochs (after
-    `check_resident_metrics` has accepted `loader`).  No GPU work."""
-    if not beta_vae_score:
-        return
-    if not metrics_every:
-        raise ValueError("beta_vae_score=True needs metrics_every > 0: the score is written with the metrics of those "
-                         "epochs")
-    check_beta_vae_score(loader.dataset, latent_dim)
+def check_epoch_scores(scores, metrics_every, loader, latent_dim):
+    """ValueError unless every score of `scores` (entries of SCORES) can be written with the metrics of every
+    `metrics_every` epochs (after `check_resident_metrics` has accepted `loader`).  No GPU work."""
+    for s in scores:
+        if not metrics_every:
+            raise ValueError("%s=True needs metrics_every > 0: the score is written with the metrics of those epochs"
+                             % s.flag)
+        s.check(loader.dataset, latent_dim)
 
 
-def write_epoch_metrics(model, loader, epoch, batch_size, save_dir, logger, factor_score=False, sap_score=False,
-                        beta_vae_score=False):
+def write_epoch_metrics(model, loader, epoch, batch_size, save_dir, logger, scores=()):
     """MIG / AAM of `model` over `loader.in_order(batch_size)` (a DeviceLoader) into `save_dir` as
     `epoch_metrics_filenames(epoch)`, with the index draws seeded by `evaluation_rng(.., model's noise key, epoch)`.
-    `factor_score=True` also writes the FactorVAE score from the same encodings as `epoch_factor_score_filenames(epoch)`,
-    `sap_score=True` the SAP score as `epoch_sap_score_filenames(epoch)` and `beta_vae_score=True` the beta-VAE score as
-    `epoch_beta_vae_score_filenames(epoch)`, each drawn from its own generator seeded with
-    `evaluation_seed(model's noise key, epoch)`.  The model's train / eval mode is kept."""
+    Every score of `scores` (entries of SCORES) is written from the same encodings as `epoch_score_filenames(score,
+    epoch)`, each drawn from its own generator seeded with `evaluation_seed(model's noise key, epoch)`.  The model's
+    train / eval mode is kept."""
     device = loader.device
     key = model._noise_state(device)[0]           # fixed at the first training step; this fixes it the same way
     moves = list(zip((METRICS_FILENAME, METRIC_HELPERS_FILE), epoch_metrics_filenames(epoch)))
-    score_args = {}
-    if factor_score:
-        moves += zip((FACTOR_SCORE_FILENAME, FACTOR_SCORE_HELPERS_FILE), epoch_factor_score_filenames(epoch))
-        score_args.update(is_factor_score=True, factor_score_seed=evaluation_seed(key, epoch))
-    if sap_score:
-        moves += zip((SAP_SCORE_FILENAME, SAP_SCORE_HELPERS_FILE), epoch_sap_score_filenames(epoch))
-        score_args.update(is_sap_score=True, sap_score_seed=evaluation_seed(key, epoch))
-    if beta_vae_score:
-        moves += zip((BETA_VAE_SCORE_FILENAME, BETA_VAE_SCORE_HELPERS_FILE), epoch_beta_vae_score_filenames(epoch))
-        score_args.update(is_beta_vae_score=True, beta_vae_score_seed=evaluation_seed(key, epoch))
+    for s in scores:
+        moves += zip((s.filename, s.helpers_file), epoch_score_filenames(s, epoch))
     with tempfile.TemporaryDirectory(dir=save_dir) as tmp, evaluation_rng(device, key, epoch):
         Evaluator(model, None, device=device, logger=logger, save_dir=tmp, is_progress_bar=False)(
-            loader.in_order(batch_size), is_metrics=True, is_losses=False, **score_args)
+            loader.in_order(batch_size), is_metrics=True, is_losses=False,
+            **score_evaluator_args(scores, evaluation_seed(key, epoch)))
         for src, dst in moves:
             os.replace(os.path.join(tmp, src), os.path.join(save_dir, dst))
+
+
+# ---- what every score needs of the dataset ------------------------------------------------------------------------
+def _dataset_lat_sizes(label, dataset):
+    """`dataset.lat_sizes`; ValueError prefixed with the score's `label` unless the dataset has known factors."""
+    if not (hasattr(dataset, "lat_sizes") and hasattr(dataset, "lat_names")):
+        raise ValueError("%s: the dataset %s has no lat_sizes / lat_names (known factors of variation)"
+                         % (label, type(dataset).__name__))
+    return dataset.lat_sizes
+
+
+def _full_grid(label, lat_sizes, n):
+    """`lat_sizes` as a list of ints; ValueError prefixed with the score's `label` unless `n` items are their full
+    grid."""
+    lat_sizes = [int(s) for s in lat_sizes]
+    if n != reduce(lambda x, y: x * y, lat_sizes, 1):
+        raise ValueError("%s: the dataset has %d items, not the %d of the full grid of its factors %s"
+                         % (label, n, reduce(lambda x, y: x * y, lat_sizes, 1), lat_sizes))
+    return lat_sizes
 
 
 # ---- FactorVAE score (Kim & Mnih 2018, section 4; the conventions of disentanglement_lib's factor_vae.py) ----------
@@ -173,18 +161,12 @@ def check_factor_score(dataset, latent_dim, batch_size=64, num_train=10000, num_
     """ValueError unless the FactorVAE score can be computed over `dataset` for a `latent_dim` model with these
     settings: the dataset has known factors (`lat_sizes`, `lat_names`), is their full grid, and has a factor of more
     than one value.  No GPU work.  Returns lat_sizes as a list of ints."""
-    if not (hasattr(dataset, "lat_sizes") and hasattr(dataset, "lat_names")):
-        raise ValueError("FactorVAE score: the dataset %s has no lat_sizes / lat_names (known factors of variation)"
-                         % type(dataset).__name__)
-    return _check_factor_grid(dataset.lat_sizes, len(dataset), latent_dim, batch_size, num_train, num_eval,
-                              num_variance_estimate)
+    return _check_factor_grid(_dataset_lat_sizes("FactorVAE score", dataset), len(dataset), latent_dim, batch_size,
+                              num_train, num_eval, num_variance_estimate)
 
 
 def _check_factor_grid(lat_sizes, n, latent_dim, batch_size, num_train, num_eval, num_variance_estimate):
-    lat_sizes = [int(s) for s in lat_sizes]
-    if n != reduce(lambda x, y: x * y, lat_sizes, 1):
-        raise ValueError("FactorVAE score: the dataset has %d items, not the %d of the full grid of its factors %s"
-                         % (n, reduce(lambda x, y: x * y, lat_sizes, 1), lat_sizes))
+    lat_sizes = _full_grid("FactorVAE score", lat_sizes, n)
     if all(s == 1 for s in lat_sizes):
         raise ValueError("FactorVAE score: every factor of %s has one value; there is nothing to vote on" % lat_sizes)
     for name, value, least in (("batch_size", batch_size, 2), ("num_train", num_train, 1), ("num_eval", num_eval, 1),
@@ -287,17 +269,11 @@ def check_sap_score(dataset, latent_dim, num_train=10000, num_test=5000, C=0.01)
     """ValueError unless the SAP score can be computed over `dataset` for a `latent_dim` model with these settings: the
     dataset has known factors (`lat_sizes`, `lat_names`) and is their full grid.  No GPU work.  Returns lat_sizes as a
     list of ints."""
-    if not (hasattr(dataset, "lat_sizes") and hasattr(dataset, "lat_names")):
-        raise ValueError("SAP score: the dataset %s has no lat_sizes / lat_names (known factors of variation)"
-                         % type(dataset).__name__)
-    return _check_sap_grid(dataset.lat_sizes, len(dataset), latent_dim, num_train, num_test, C)
+    return _check_sap_grid(_dataset_lat_sizes("SAP score", dataset), len(dataset), latent_dim, num_train, num_test, C)
 
 
 def _check_sap_grid(lat_sizes, n, latent_dim, num_train, num_test, C):
-    lat_sizes = [int(s) for s in lat_sizes]
-    if n != reduce(lambda x, y: x * y, lat_sizes, 1):
-        raise ValueError("SAP score: the dataset has %d items, not the %d of the full grid of its factors %s"
-                         % (n, reduce(lambda x, y: x * y, lat_sizes, 1), lat_sizes))
+    lat_sizes = _full_grid("SAP score", lat_sizes, n)
     if all(s == 1 for s in lat_sizes):
         raise ValueError("SAP score: every factor of %s has one value; there is nothing to predict" % lat_sizes)
     if max(lat_sizes) > SAP_MAX_CLASSES:
@@ -414,17 +390,12 @@ def check_beta_vae_score(dataset, latent_dim, batch_size=64, num_train=10000, nu
     """ValueError unless the beta-VAE score can be computed over `dataset` for a `latent_dim` model with these
     settings: the dataset has known factors (`lat_sizes`, `lat_names`), is their full grid and has between 2 and
     BETA_VAE_MAX_FACTORS factors of more than one value.  No GPU work.  Returns lat_sizes as a list of ints."""
-    if not (hasattr(dataset, "lat_sizes") and hasattr(dataset, "lat_names")):
-        raise ValueError("beta-VAE score: the dataset %s has no lat_sizes / lat_names (known factors of variation)"
-                         % type(dataset).__name__)
-    return _check_beta_vae_grid(dataset.lat_sizes, len(dataset), latent_dim, batch_size, num_train, num_eval)
+    return _check_beta_vae_grid(_dataset_lat_sizes("beta-VAE score", dataset), len(dataset), latent_dim, batch_size,
+                                num_train, num_eval)
 
 
 def _check_beta_vae_grid(lat_sizes, n, latent_dim, batch_size, num_train, num_eval):
-    lat_sizes = [int(s) for s in lat_sizes]
-    if n != reduce(lambda x, y: x * y, lat_sizes, 1):
-        raise ValueError("beta-VAE score: the dataset has %d items, not the %d of the full grid of its factors %s"
-                         % (n, reduce(lambda x, y: x * y, lat_sizes, 1), lat_sizes))
+    lat_sizes = _full_grid("beta-VAE score", lat_sizes, n)
     scored = sum(s > 1 for s in lat_sizes)
     if scored < 2:
         raise ValueError("beta-VAE score: %s has %d factors of more than one value; the score needs at least 2 to "
@@ -545,6 +516,35 @@ def beta_vae_score(mu, lat_sizes, batch_size=64, num_train=10000, num_eval=5000,
     return score, helpers
 
 
+# ---- the scores the Evaluator, training and sweeps write ----------------------------------------------------------
+class Score(NamedTuple):
+    """A disentanglement score the Evaluator writes beside MIG / AAM.  `flag` names its switches: the Evaluator's
+    `is_{flag}` and `{flag}_seed`, and `{flag}` of training and sweeps.  Its files are `{stem}.log` and
+    `{stem}_helpers.pth`, during training `epoch_score_filenames`.  `label` names it in the log.  `check(dataset,
+    latent_dim)` refuses, before any GPU work, what `compute(mu, lat_sizes, seed=...)` cannot score at its default
+    settings."""
+    flag: str
+    stem: str
+    label: str
+    check: Callable
+    compute: Callable
+
+    @property
+    def filename(self):
+        return self.stem + ".log"
+
+    @property
+    def helpers_file(self):
+        return self.stem + "_helpers.pth"
+
+
+SCORES = (
+    Score("factor_score", "factor_vae_score", "FactorVAE score", check_factor_score, factor_vae_score),
+    Score("sap_score", "sap_score", "SAP score", check_sap_score, sap_score),
+    Score("beta_vae_score", "beta_vae_score", "beta-VAE score", check_beta_vae_score, beta_vae_score),
+)
+
+
 class Evaluator:
     def __init__(self, model, loss_f, device=torch.device("cpu"), logger=logging.getLogger(__name__),
                  save_dir="results", is_progress_bar=True):
@@ -561,20 +561,15 @@ class Evaluator:
                  is_sap_score=False, sap_score_seed=0, is_beta_vae_score=False, beta_vae_score_seed=0):
         """evaluate.py:59-96.  Like the reference, the first returned value is always None (it assigns the metrics to
         a differently named variable, :77-79); the metrics are logged and written to metrics.log.
-        `is_factor_score=True` also writes the FactorVAE score (`compute_factor_vae_score` with its default settings
-        and `seed=factor_score_seed`) to factor_vae_score.log and its tables to factor_vae_score_helpers.pth;
-        `is_sap_score=True` writes the SAP score (`compute_sap_score` with its default settings and
-        `seed=sap_score_seed`) to sap_score.log and its tables to sap_score_helpers.pth; `is_beta_vae_score=True` writes
-        the beta-VAE score (`compute_beta_vae_score` with its default settings and `seed=beta_vae_score_seed`) to
-        beta_vae_score.log and its tables to beta_vae_score_helpers.pth.  The dataset is encoded once for all the scores
-        asked for."""
+        For every entry of SCORES, `is_{flag}=True` also writes that score (`compute_factor_vae_score`,
+        `compute_sap_score` or `compute_beta_vae_score` with its default settings and `seed={flag}_seed`) to
+        `{stem}.log` and its tables to `{stem}_helpers.pth`: factor_vae_score, sap_score and beta_vae_score.  The
+        checks of every score asked for run before any GPU work, and the dataset is encoded once for all of them."""
+        args = locals()                           # the per-score keywords are is_{flag} and {flag}_seed
+        scores = select_scores(args, "is_")
         start = default_timer()
-        if is_factor_score:
-            check_factor_score(getattr(data_loader, "dataset", None), self.model.latent_dim)
-        if is_sap_score:
-            check_sap_score(getattr(data_loader, "dataset", None), self.model.latent_dim)
-        if is_beta_vae_score:
-            check_beta_vae_score(getattr(data_loader, "dataset", None), self.model.latent_dim)
+        for s in scores:
+            s.check(getattr(data_loader, "dataset", None), self.model.latent_dim)
         is_still_training = self.model.training
         self.model.eval()
         metric, losses = None, None
@@ -587,30 +582,14 @@ class Evaluator:
             metrics = self._metrics_of(encoded, lat_sizes, lat_names)
             self.logger.info('Losses: {}'.format(metrics))
             save_metadata(metrics, self.save_dir, filename=METRICS_FILENAME)
-        if is_factor_score:
-            self.logger.info('Computing the FactorVAE score...')
+        for s in scores:
+            self.logger.info('Computing the {}...'.format(s.label))
             if encoded is None:
                 encoded = self._compute_q_zCx(data_loader)
-            score, helpers = factor_vae_score(encoded[1][0], data_loader.dataset.lat_sizes, seed=factor_score_seed)
-            self.logger.info('FactorVAE score: {}'.format(score))
-            save_metadata(score, self.save_dir, filename=FACTOR_SCORE_FILENAME)
-            torch.save(helpers, os.path.join(self.save_dir, FACTOR_SCORE_HELPERS_FILE))
-        if is_sap_score:
-            self.logger.info('Computing the SAP score...')
-            if encoded is None:
-                encoded = self._compute_q_zCx(data_loader)
-            score, helpers = sap_score(encoded[1][0], data_loader.dataset.lat_sizes, seed=sap_score_seed)
-            self.logger.info('SAP score: {}'.format(score))
-            save_metadata(score, self.save_dir, filename=SAP_SCORE_FILENAME)
-            torch.save(helpers, os.path.join(self.save_dir, SAP_SCORE_HELPERS_FILE))
-        if is_beta_vae_score:
-            self.logger.info('Computing the beta-VAE score...')
-            if encoded is None:
-                encoded = self._compute_q_zCx(data_loader)
-            score, helpers = beta_vae_score(encoded[1][0], data_loader.dataset.lat_sizes, seed=beta_vae_score_seed)
-            self.logger.info('beta-VAE score: {}'.format(score))
-            save_metadata(score, self.save_dir, filename=BETA_VAE_SCORE_FILENAME)
-            torch.save(helpers, os.path.join(self.save_dir, BETA_VAE_SCORE_HELPERS_FILE))
+            score, helpers = s.compute(encoded[1][0], data_loader.dataset.lat_sizes, seed=args[s.flag + "_seed"])
+            self.logger.info('{}: {}'.format(s.label, score))
+            save_metadata(score, self.save_dir, filename=s.filename)
+            torch.save(helpers, os.path.join(self.save_dir, s.helpers_file))
         if is_losses:
             self.logger.info('Computing losses...')
             losses = self.compute_losses(data_loader)
@@ -647,28 +626,28 @@ class Evaluator:
         """FactorVAE score (Kim & Mnih 2018, section 4) of the model's encoder means over `dataloader` (the dataset in
         index order: DataLoader(shuffle=False) or DeviceLoader.in_order) -> {"train_accuracy", "eval_accuracy",
         "num_active_dims"}; see `factor_vae_score` for the definition and the order of the draws."""
-        check_factor_score(getattr(dataloader, "dataset", None), self.model.latent_dim, batch_size, num_train, num_eval,
-                           num_variance_estimate)
-        mean = self._compute_q_zCx(dataloader)[1][0]
-        return factor_vae_score(mean, dataloader.dataset.lat_sizes, batch_size, num_train, num_eval,
-                                num_variance_estimate, seed)[0]
+        return self._score(check_factor_score, factor_vae_score, dataloader, seed, batch_size=batch_size,
+                           num_train=num_train, num_eval=num_eval, num_variance_estimate=num_variance_estimate)
 
     def compute_sap_score(self, dataloader, num_train=10000, num_test=5000, C=0.01, seed=0):
         """SAP score (Kumar et al. 2018, section 3) of the model's encoder means over `dataloader` (the dataset in index
         order: DataLoader(shuffle=False) or DeviceLoader.in_order) -> {"SAP"}; see `sap_score` for the definition and
         the order of the draws."""
-        check_sap_score(getattr(dataloader, "dataset", None), self.model.latent_dim, num_train, num_test, C)
-        mean = self._compute_q_zCx(dataloader)[1][0]
-        return sap_score(mean, dataloader.dataset.lat_sizes, num_train, num_test, C, seed)[0]
+        return self._score(check_sap_score, sap_score, dataloader, seed, num_train=num_train, num_test=num_test, C=C)
 
     def compute_beta_vae_score(self, dataloader, batch_size=64, num_train=10000, num_eval=5000, seed=0):
         """beta-VAE score (Higgins et al. 2017, section 3) of the model's encoder means over `dataloader` (the dataset
         in index order: DataLoader(shuffle=False) or DeviceLoader.in_order) -> {"train_accuracy", "eval_accuracy"};
         see `beta_vae_score` for the definition and the order of the draws."""
-        check_beta_vae_score(getattr(dataloader, "dataset", None), self.model.latent_dim, batch_size, num_train,
-                             num_eval)
+        return self._score(check_beta_vae_score, beta_vae_score, dataloader, seed, batch_size=batch_size,
+                           num_train=num_train, num_eval=num_eval)
+
+    def _score(self, check, compute, dataloader, seed, **settings):
+        """`compute(encoder means, lat_sizes, seed=seed, **settings)`'s score, after `check(dataset, latent_dim,
+        **settings)` has accepted the dataset."""
+        check(getattr(dataloader, "dataset", None), self.model.latent_dim, **settings)
         mean = self._compute_q_zCx(dataloader)[1][0]
-        return beta_vae_score(mean, dataloader.dataset.lat_sizes, batch_size, num_train, num_eval, seed)[0]
+        return compute(mean, dataloader.dataset.lat_sizes, seed=seed, **settings)[0]
 
     def _known_factors(self, dataloader):
         try:

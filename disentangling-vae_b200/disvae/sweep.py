@@ -31,10 +31,8 @@ import torch
 
 from disvae import ops
 from disvae.data import DeviceLoader, device_loader_for
-from disvae.evaluate import (Evaluator, check_beta_vae_score, check_epoch_beta_vae_score, check_epoch_factor_score,
-                             check_epoch_sap_score, check_factor_score, check_resident_metrics, check_sap_score,
-                             evaluation_rng, evaluation_seed,
-                             write_epoch_metrics)
+from disvae.evaluate import (Evaluator, check_epoch_scores, check_resident_metrics, evaluation_rng, evaluation_seed,
+                             score_evaluator_args, select_scores, write_epoch_metrics)
 from disvae.fused import FusedAdam
 from disvae.models.losses import permutation_key
 from disvae.models.vae import noise_key
@@ -143,6 +141,7 @@ class Sweep:
         `metrics_every` writes each member's `metrics-{epoch}.log` as `Trainer.__call__` does, one member after
         another on the caller's stream, over the one resident copy; `factor_score=True`, `sap_score=True` and
         `beta_vae_score=True` add each member's FactorVAE, SAP and beta-VAE scores of those epochs."""
+        scores = select_scores(locals())
         first, loader_state = self._resume()
         if loader_state is not None:
             check_loader_state(loader_state, data_loader, device_data=True)
@@ -150,9 +149,7 @@ class Sweep:
         if metrics_every:
             check_resident_metrics(data_loader, metrics_batch_size, device_data=True)
         for m in self.members:
-            check_epoch_factor_score(factor_score, metrics_every, data_loader, m.model.latent_dim)
-            check_epoch_sap_score(sap_score, metrics_every, data_loader, m.model.latent_dim)
-            check_epoch_beta_vae_score(beta_vae_score, metrics_every, data_loader, m.model.latent_dim)
+            check_epoch_scores(scores, metrics_every, data_loader, m.model.latent_dim)
         loader = self._loader(data_loader)
         for m in self.members:
             m._resume = None
@@ -162,7 +159,7 @@ class Sweep:
         start = default_timer()
         with torch.cuda.device(self.device):
             self._run(loader, first, epochs, checkpoint_every, save_state, start, metrics_every, metrics_batch_size,
-                      factor_score, sap_score, beta_vae_score)
+                      scores)
 
     def evaluate(self, is_metrics=True, is_losses=True, batch_size=1000, is_factor_score=False, is_sap_score=False,
                  is_beta_vae_score=False):
@@ -174,33 +171,24 @@ class Sweep:
         after its latest epoch (`disvae.evaluate.evaluation_seed`), `is_sap_score=True` `sap_score.log` and
         `sap_score_helpers.pth`, and `is_beta_vae_score=True` `beta_vae_score.log` and `beta_vae_score_helpers.pth`,
         seeded the same way."""
+        scores = select_scores(locals(), "is_")
         if self.loader is None:
             raise ValueError("Sweep.evaluate: the sweep has no loader yet; train it first (sweep(loader, ...))")
         if is_metrics:
             check_resident_metrics(self.loader, batch_size, device_data=True)
         elif int(batch_size) < 1:
             raise ValueError("Sweep.evaluate: batch_size must be positive, got %d" % int(batch_size))
-        if is_factor_score:
+        for s in scores:
             for m in self.members:
-                check_factor_score(self.loader.dataset, m.model.latent_dim)
-        if is_sap_score:
-            for m in self.members:
-                check_sap_score(self.loader.dataset, m.model.latent_dim)
-        if is_beta_vae_score:
-            for m in self.members:
-                check_beta_vae_score(self.loader.dataset, m.model.latent_dim)
+                s.check(self.loader.dataset, m.model.latent_dim)
         with torch.cuda.device(self.device):
             for m in self.members:
                 key, epoch = m.model._noise_state(self.device)[0], m._next_epoch - 1
+                score_args = score_evaluator_args(scores, evaluation_seed(key, epoch))
                 with evaluation_rng(self.device, key, epoch):
                     Evaluator(m.model, m.loss_f, device=self.device, logger=m.logger, save_dir=m.save_dir,
                               is_progress_bar=m.is_progress_bar)(self.loader.in_order(batch_size), is_metrics=is_metrics,
-                                                                 is_losses=is_losses, is_factor_score=is_factor_score,
-                                                                 factor_score_seed=evaluation_seed(key, epoch),
-                                                                 is_sap_score=is_sap_score,
-                                                                 sap_score_seed=evaluation_seed(key, epoch),
-                                                                 is_beta_vae_score=is_beta_vae_score,
-                                                                 beta_vae_score_seed=evaluation_seed(key, epoch))
+                                                                 is_losses=is_losses, **score_args)
 
     def _resume(self):
         """(first epoch, saved loader state) of the members' loaded training states, (0, None) if none has one.
@@ -228,7 +216,7 @@ class Sweep:
             yield
 
     def _run(self, loader, first, epochs, checkpoint_every, save_state, start, metrics_every, metrics_batch_size,
-             factor_score, sap_score, beta_vae_score):
+             scores):
         members = self.members
         main = torch.cuda.current_stream(self.device)
         if self.streams is None:
@@ -284,8 +272,7 @@ class Sweep:
                     for ev in done:                                # every member has ended the epoch
                         main.wait_event(ev)
                     for m in members:                              # the next gather, on `main`, waits for these
-                        write_epoch_metrics(m.model, loader, epoch, metrics_batch_size, m.save_dir, m.logger,
-                                            factor_score, sap_score, beta_vae_score)
+                        write_epoch_metrics(m.model, loader, epoch, metrics_batch_size, m.save_dir, m.logger, scores)
         finally:
             for ev in done:
                 if ev is not None:

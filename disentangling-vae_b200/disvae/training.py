@@ -21,9 +21,7 @@ import torch.distributed as dist
 from tqdm import trange
 
 from disvae import _native
-from disvae.evaluate import (check_epoch_beta_vae_score, check_epoch_factor_score, check_epoch_sap_score,
-                             check_resident_metrics,
-                             write_epoch_metrics)
+from disvae.evaluate import check_epoch_scores, check_resident_metrics, select_scores, write_epoch_metrics
 from disvae.fused import FusedAdam
 from disvae.models.losses import DeviceLossLog
 from disvae.parallel import GradAverage, broadcast_parameters, is_distributed
@@ -85,6 +83,7 @@ class Trainer():
         `sap_score=True` the SAP score (`sap_score-{epoch}.log`, `sap_score_helpers-{epoch}.pth`) and
         `beta_vae_score=True` the beta-VAE score (`beta_vae_score-{epoch}.log`, `beta_vae_score_helpers-{epoch}.pth`).
         Training itself is unchanged."""
+        scores = select_scores(locals())
         start = default_timer()
         first, loader_state = (0, None) if self._resume is None else self._resume
         if loader_state is not None:
@@ -92,9 +91,7 @@ class Trainer():
         check_metrics_every(metrics_every)
         if metrics_every:
             check_resident_metrics(data_loader, metrics_batch_size, self.device_data)
-        check_epoch_factor_score(factor_score, metrics_every, data_loader, self.model.latent_dim)
-        check_epoch_sap_score(sap_score, metrics_every, data_loader, self.model.latent_dim)
-        check_epoch_beta_vae_score(beta_vae_score, metrics_every, data_loader, self.model.latent_dim)
+        check_epoch_scores(scores, metrics_every, data_loader, self.model.latent_dim)
         self._resume = None
         if self.device_data and isinstance(data_loader, torch.utils.data.DataLoader):
             data_loader = self._device_loader(data_loader)
@@ -110,7 +107,7 @@ class Trainer():
                             save_state=save_state and (epoch % checkpoint_every == 0 or epoch == last))
             if metrics_every and (epoch % metrics_every == 0 or epoch == last):
                 write_epoch_metrics(self.model, data_loader, epoch, metrics_batch_size, self.save_dir, self.logger,
-                                    factor_score, sap_score, beta_vae_score)
+                                    scores)
         self._end_training(start)
 
     def _end_epoch(self, epoch, storer, mean_epoch_loss, checkpoint_every, save_state=False):

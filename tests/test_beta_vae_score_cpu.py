@@ -9,7 +9,7 @@ import torch
 
 import beta_vae_reference as R
 from disvae import evaluate
-from test_factor_score_cpu import _bare_sweep, _device_loader, _evaluator, _Grid, _trainer, no_gpu  # noqa: F401
+from score_stubs import _evaluator, _Grid, no_gpu  # noqa: F401
 
 
 # (dataset, latent_dim, settings, message) of every refusal
@@ -49,50 +49,6 @@ def test_score_function_refusals_before_gpu_work(no_gpu, case):
     if len(ds) <= 10 ** 6:                          # not the 2^33-item grid
         with pytest.raises(ValueError, match=msg):
             evaluate.beta_vae_score(torch.zeros(len(ds), latent_dim), ds.lat_sizes, **settings)
-
-
-def test_trainer_refusals_before_gpu_work(tmp_path, no_gpu):
-    tr = _trainer(tmp_path)
-    good = _device_loader(_Grid([100, 100]))
-    with pytest.raises(ValueError, match="beta_vae_score=True needs metrics_every > 0"):
-        tr(good, epochs=1, beta_vae_score=True)
-    for ds, msg in ((_Grid([100, 100], n=10001), "has 10001 items, not the 10000"),
-                    (_Grid([1, 10000]), "has 1 factors of more than one value"),
-                    (_Grid([10000], factors=False), "no lat_sizes / lat_names")):
-        with pytest.raises(ValueError, match=msg):
-            tr(_device_loader(ds), epochs=1, metrics_every=1, beta_vae_score=True)
-    assert tr.loss_f.n_train_steps == 0 and tr._data_loader is None and good.epoch == 3
-
-
-def test_trainer_refuses_a_latent_dim_above_the_limit(tmp_path, no_gpu):
-    tr = _trainer(tmp_path)
-    tr.model.latent_dim = 129
-    with pytest.raises(ValueError, match="latent_dim 129 is above the kernel's limit of 128"):
-        tr(_device_loader(_Grid([100, 100])), epochs=1, metrics_every=1, beta_vae_score=True)
-
-
-def test_trainer_refuses_beta_vae_score_under_distributed(tmp_path, no_gpu, monkeypatch):
-    monkeypatch.setattr(evaluate, "is_distributed", lambda: True)
-    tr = _trainer(tmp_path)
-    with pytest.raises(ValueError, match="not supported under torch.distributed"):
-        tr(_device_loader(_Grid([100, 100])), epochs=1, metrics_every=1, beta_vae_score=True)
-    with pytest.raises(ValueError, match="beta_vae_score=True needs metrics_every > 0"):
-        tr(_device_loader(_Grid([100, 100])), epochs=1, beta_vae_score=True)
-    sw = _bare_sweep([_trainer(tmp_path, "a")])
-    with pytest.raises(ValueError, match="not supported under torch.distributed"):
-        sw(_device_loader(_Grid([100, 100])), epochs=1, metrics_every=1, beta_vae_score=True)
-
-
-def test_sweep_refusals_before_gpu_work(tmp_path, no_gpu):
-    sw = _bare_sweep([_trainer(tmp_path, "a"), _trainer(tmp_path, "b")])
-    with pytest.raises(ValueError, match="beta_vae_score=True needs metrics_every > 0"):
-        sw(_device_loader(_Grid([100, 100])), epochs=1, beta_vae_score=True)
-    with pytest.raises(ValueError, match="has 10001 items, not the 10000"):
-        sw(_device_loader(_Grid([100, 100], n=10001)), epochs=1, metrics_every=1, beta_vae_score=True)
-    assert sw.loader is None and not sw._device_loaders
-    sw.loader = _device_loader(_Grid([100, 100], n=10001))
-    with pytest.raises(ValueError, match="has 10001 items, not the 10000"):
-        sw.evaluate(is_metrics=False, is_losses=False, is_beta_vae_score=True)
 
 
 # ---- the draw order -----------------------------------------------------------------------------------------------

@@ -2,16 +2,11 @@
 q_zCx layout and a contiguous one; `dv_logistic_fit` against the fp64 dense Newton solve of
 tests/beta_vae_reference.py at the shapes a user meets and at the limits; bit-identical repeats and refusals that
 launch nothing; known answers of `beta_vae_score`; the Evaluator's score files over a DataLoader and over resident
-data, beside MIG / AAM, the FactorVAE score and SAP; and `beta_vae_score=True` in training, in a sweep and across a
-resume.
-
-Run as a script (`python tests/test_beta_vae_score_gpu.py PHASE SAVE_DIR OUT`) it trains the resume case's stopped
-("first") or continued ("resume") run in a fresh process and saves its result to OUT.
+data, beside MIG / AAM, the FactorVAE score and SAP.  The score in training, in sweeps and across a resume is tested
+with the others in test_scores_gpu.py.
 """
 import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -20,8 +15,6 @@ import torch
 import beta_vae_reference as R
 
 pytestmark = pytest.mark.gpu
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 DEV = torch.device("cuda", 0)
 DV_ERR_BAD_SHAPE, DV_ERR_BAD_ARG, DV_ERR_WORKSPACE = -1, -2, -3
 COEF_RTOL = 1e-7          # |(W, b) - fp64 (W, b)|_inf against the fp64 solution's |(W, b)|_inf
@@ -269,9 +262,8 @@ def test_aligned_code_scores_one(layout):
 
 
 # ---- the Evaluator on a Burgess model ----------------------------------------------------------------------------
-from test_eval_resident_gpu import (EPOCHS, IMG, K, _assert_same_state, _checkpoint_model, _dataset,  # noqa: E402
-                                    _evaluator, _loader, _loss, _member, _n_samples, _read, _state)
-from test_sap_score_gpu import _assert_same_eval_files  # noqa: E402
+from test_eval_resident_gpu import (K, _assert_same_eval_files, _checkpoint_model, _dataset, _evaluator,  # noqa: E402
+                                    _loader, _loss, _n_samples)
 
 SCORE_FILES = [("beta_vae_score.log",) * 2, ("beta_vae_score_helpers.pth",) * 2]
 OTHER_FILES = [(f, f) for f in ("factor_vae_score.log", "factor_vae_score_helpers.pth", "sap_score.log",
@@ -300,9 +292,9 @@ def test_evaluator_score_files(tmp_path, monkeypatch):
                 data, is_metrics=True, is_losses=True, is_factor_score=True, factor_score_seed=21, is_sap_score=True,
                 sap_score_seed=21, beta_vae_score_seed=21, **kw)
             assert len(passes) == 1, name                      # one encoding for MIG / AAM and every score
-    _assert_same_eval_files(tmp_path / "dev", tmp_path / "host", SCORE_FILES, "dev vs host")
+    _assert_same_eval_files(tmp_path / "dev", tmp_path / "host", SCORE_FILES, "dev vs host", nan_equal=True)
     names = [(f, f) for f in ("metrics.log", "metric_helpers.pth", "test_losses.log")] + OTHER_FILES
-    _assert_same_eval_files(tmp_path / "host", tmp_path / "plain", names, "with vs without the score")
+    _assert_same_eval_files(tmp_path / "host", tmp_path / "plain", names, "with vs without the score", nan_equal=True)
     assert not os.path.exists(tmp_path / "plain" / "beta_vae_score.log")
     score = json.load(open(tmp_path / "host" / "beta_vae_score.log"))
     helpers = torch.load(tmp_path / "host" / "beta_vae_score_helpers.pth", weights_only=False)
@@ -326,115 +318,3 @@ def test_evaluator_score_files(tmp_path, monkeypatch):
     assert abs(score["train_accuracy"] - right[:10000].mean()) <= loose / 10000 + 1e-12
     assert abs(score["eval_accuracy"] - right[10000:].mean()) <= loose / 5000 + 1e-12
     assert ev.compute_beta_vae_score(loader(ds, 1000), seed=21) == score
-
-
-# ---- training, sweeps, resume -------------------------------------------------------------------------------------
-def _standalone_score(kind, save_dir, epoch, noise_key, out_dir):
-    """The documented reproduction of beta_vae_score-{epoch}.log: model-{epoch}.pt in a fresh model, an Evaluator over
-    DataLoader(dataset, 1000, shuffle=False) with seed evaluation_seed(noise key, epoch)."""
-    import disvae
-    from disvae.evaluate import evaluation_seed
-    from synthetic_factors import loader
-    m = disvae.init_specific_model("Burgess", IMG, 10)
-    m.load_state_dict(torch.load(os.path.join(save_dir, "model-%d.pt" % epoch), weights_only=True))
-    _evaluator(m.to(DEV), _loss(kind, K ** 4), out_dir)(loader(_dataset(), 1000), is_metrics=False, is_losses=False,
-                                                        is_beta_vae_score=True,
-                                                        beta_vae_score_seed=evaluation_seed(noise_key, epoch))
-
-
-def _epoch_names(epochs=EPOCHS):
-    return [("beta_vae_score-%d.log" % e,) * 2 for e in range(epochs)] + \
-        [("beta_vae_score_helpers-%d.pth" % e,) * 2 for e in range(epochs)] + \
-        [("metrics-%d.log" % e,) * 2 for e in range(epochs)]
-
-
-def test_beta_vae_score_leaves_training_unchanged(tmp_path):
-    seed = 17
-    runs = {}
-    with _n_samples(512):
-        for on in (False, True):
-            tr = _member("btcvae", seed, tmp_path / ("bvae%d" % on))
-            torch.manual_seed(seed)
-            tr(_loader(), epochs=EPOCHS, checkpoint_every=1, metrics_every=1, factor_score=True, sap_score=True,
-               beta_vae_score=on)
-            runs[on] = tr
-    _assert_same_state(_state(runs[True]), _state(runs[False]), "beta_vae_score on vs off")
-    kept = ("metrics-%d.log", "metric_helpers-%d.pth", "factor_vae_score-%d.log", "factor_vae_score_helpers-%d.pth",
-            "sap_score-%d.log", "sap_score_helpers-%d.pth", "model-%d.pt")
-    names = [(f % e,) * 2 for e in range(EPOCHS) for f in kept if not f.endswith(".pt")]
-    _assert_same_eval_files(runs[True].save_dir, runs[False].save_dir, names + [("train_losses.log",) * 2],
-                            "metrics with and without the score")
-    for e in range(EPOCHS):
-        a = torch.load(os.path.join(runs[True].save_dir, "model-%d.pt" % e), weights_only=True)
-        b = torch.load(os.path.join(runs[False].save_dir, "model-%d.pt" % e), weights_only=True)
-        assert a.keys() == b.keys() and all(torch.equal(a[k], b[k]) for k in a), e
-    assert not any(f.startswith("beta_vae_score") for f in os.listdir(runs[False].save_dir))
-    key = runs[True].training_state()["noise"]["key"]
-    for e in range(EPOCHS):
-        out = tmp_path / ("standalone%d" % e)
-        _standalone_score("btcvae", runs[True].save_dir, e, key, out)
-        pairs = [("beta_vae_score-%d.log" % e, "beta_vae_score.log"),
-                 ("beta_vae_score_helpers-%d.pth" % e, "beta_vae_score_helpers.pth")]
-        _assert_same_eval_files(runs[True].save_dir, out, pairs, e)
-
-
-SPECS = [("btcvae", 11), ("betaB", 12), ("factor", 13)]
-
-
-def test_sweep_scores_equal_lone_runs(tmp_path):
-    from disvae.evaluate import evaluation_seed
-    from disvae.sweep import Sweep
-    from synthetic_factors import loader
-    with _n_samples(512):
-        members = [_member(kind, seed, tmp_path / ("m%d_%s" % (k, kind))) for k, (kind, seed) in enumerate(SPECS)]
-        sweep = Sweep(members, seeds=[seed for _, seed in SPECS])
-        sweep(_loader(), epochs=EPOCHS, checkpoint_every=1, metrics_every=1, beta_vae_score=True)
-        sweep.evaluate(is_metrics=False, is_losses=False, is_beta_vae_score=True)
-        lones = []
-        for kind, seed in SPECS:
-            tr = _member(kind, seed, tmp_path / ("lone_" + kind))
-            torch.manual_seed(seed)
-            tr(_loader(), epochs=EPOCHS, checkpoint_every=1, metrics_every=1, beta_vae_score=True)
-            _evaluator(tr.model, tr.loss_f, tr.save_dir)(loader(_dataset(), 1000), is_losses=False,
-                                                         is_beta_vae_score=True,
-                                                         beta_vae_score_seed=evaluation_seed(seed, EPOCHS - 1))
-            lones.append(tr)
-    for m, lone, (kind, _) in zip(members, lones, SPECS):
-        _assert_same_state(_state(m), _state(lone), kind)
-        _assert_same_eval_files(m.save_dir, lone.save_dir, _epoch_names() + SCORE_FILES, kind)
-        last = [("beta_vae_score.log", "beta_vae_score-%d.log" % (EPOCHS - 1)),
-                ("beta_vae_score_helpers.pth", "beta_vae_score_helpers-%d.pth" % (EPOCHS - 1))]
-        _assert_same_eval_files(m.save_dir, m.save_dir, last, kind)
-
-
-def _resume_run(phase, save_dir):
-    """'full': EPOCHS epochs; 'first': 1 epoch; 'resume': load training-state-0.pt and train EPOCHS - 1 more.  All with
-    save_state=True, metrics_every=1 and beta_vae_score=True."""
-    from disvae.utils.modelIO import load_training_state
-    tr = _member("btcvae", 29, save_dir)
-    if phase == "resume":
-        load_training_state(tr, os.path.join(str(save_dir), "training-state-0.pt"))
-    torch.manual_seed(29)
-    epochs = {"full": EPOCHS, "first": 1, "resume": EPOCHS - 1}[phase]
-    with _n_samples(512):
-        tr(_loader(), epochs=epochs, checkpoint_every=1, save_state=True, metrics_every=1, beta_vae_score=True)
-    torch.cuda.synchronize()
-    return _state(tr)
-
-
-def test_resumed_run_writes_the_same_later_scores(tmp_path):
-    full = _resume_run("full", tmp_path / "a")
-    for phase in ("first", "resume"):
-        r = subprocess.run([sys.executable, os.path.abspath(__file__), phase, str(tmp_path / "b"),
-                            str(tmp_path / (phase + ".pt"))], capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, (phase, r.stdout[-2000:] + r.stderr[-4000:])
-    got = torch.load(tmp_path / "resume.pt", weights_only=False)
-    _assert_same_state(got, full, "resumed")
-    _assert_same_eval_files(tmp_path / "b", tmp_path / "a", _epoch_names(), "resume")
-
-
-if __name__ == "__main__":
-    sys.path[:0] = [os.path.join(ROOT, "disentangling-vae_b200"), HERE]
-    phase, save_dir, out = sys.argv[1], sys.argv[2], sys.argv[3]
-    torch.cuda.set_device(DEV)
-    torch.save(_resume_run(phase, save_dir), out)

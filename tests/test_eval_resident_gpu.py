@@ -90,18 +90,24 @@ def _read(path):
         return f.read()
 
 
-def _assert_same_helpers(a, b, what):
+def _assert_same_helpers(a, b, what, nan_equal=False):
     ha, hb = torch.load(a, weights_only=False), torch.load(b, weights_only=False)
     assert ha.keys() == hb.keys(), what
     for k in hb:
-        assert torch.equal(ha[k], hb[k]), (what, k)
+        x, y = ha[k], hb[k]
+        if nan_equal and torch.is_floating_point(y):
+            assert torch.equal(x.isnan(), y.isnan()), (what, k)
+            x, y = x[~x.isnan()], y[~y.isnan()]
+        assert torch.equal(x, y), (what, k)
 
 
-def _assert_same_eval_files(dir_a, dir_b, names, what):
+def _assert_same_eval_files(dir_a, dir_b, names, what, nan_equal=False):
+    """Logs byte for byte and helper tensors bit for bit; with `nan_equal`, NaN where the other file has NaN (the
+    unused slots of SAP's "coef") and bit for bit elsewhere."""
     for fa, fb in names:
         pa, pb = os.path.join(dir_a, fa), os.path.join(dir_b, fb)
         if fa.endswith(".pth"):
-            _assert_same_helpers(pa, pb, (what, fa, fb))
+            _assert_same_helpers(pa, pb, (what, fa, fb), nan_equal)
         else:
             assert _read(pa) == _read(pb), (what, fa, fb, _read(pa), _read(pb))
 

@@ -9,7 +9,7 @@ import torch
 
 import sap_reference as R
 from disvae import evaluate
-from test_factor_score_cpu import _bare_sweep, _device_loader, _evaluator, _Grid, _trainer, no_gpu  # noqa: F401
+from score_stubs import _evaluator, _Grid, no_gpu  # noqa: F401
 
 
 # (dataset, latent_dim, settings, message) of every refusal
@@ -46,43 +46,6 @@ def test_evaluator_refusals_before_gpu_work(tmp_path, no_gpu, case):
         with pytest.raises(ValueError, match=msg):
             evaluate.sap_score(torch.zeros(len(ds), latent_dim), ds.lat_sizes, **settings)
     assert not list(tmp_path.iterdir())
-
-
-def test_trainer_refusals_before_gpu_work(tmp_path, no_gpu):
-    tr = _trainer(tmp_path)
-    good = _device_loader(_Grid([100, 100]))
-    with pytest.raises(ValueError, match="sap_score=True needs metrics_every > 0"):
-        tr(good, epochs=1, sap_score=True)
-    for ds, msg in ((_Grid([100, 100], n=10001), "has 10001 items, not the 10000"),
-                    (_Grid([1] * 3, n=10000), "has 10000 items, not the 1 of the full grid"),
-                    (_Grid([2, 5000]), "more than the kernel's limit of 256 values")):
-        with pytest.raises(ValueError, match=msg):
-            tr(_device_loader(ds), epochs=1, metrics_every=1, sap_score=True)
-    assert tr.loss_f.n_train_steps == 0 and tr._data_loader is None and good.epoch == 3
-
-
-def test_trainer_refuses_sap_score_under_distributed(tmp_path, no_gpu, monkeypatch):
-    monkeypatch.setattr(evaluate, "is_distributed", lambda: True)
-    tr = _trainer(tmp_path)
-    with pytest.raises(ValueError, match="not supported under torch.distributed"):
-        tr(_device_loader(_Grid([100, 100])), epochs=1, metrics_every=1, sap_score=True)
-    with pytest.raises(ValueError, match="sap_score=True needs metrics_every > 0"):
-        tr(_device_loader(_Grid([100, 100])), epochs=1, sap_score=True)
-    sw = _bare_sweep([_trainer(tmp_path, "a")])
-    with pytest.raises(ValueError, match="not supported under torch.distributed"):
-        sw(_device_loader(_Grid([100, 100])), epochs=1, metrics_every=1, sap_score=True)
-
-
-def test_sweep_refusals_before_gpu_work(tmp_path, no_gpu):
-    sw = _bare_sweep([_trainer(tmp_path, "a"), _trainer(tmp_path, "b")])
-    with pytest.raises(ValueError, match="sap_score=True needs metrics_every > 0"):
-        sw(_device_loader(_Grid([100, 100])), epochs=1, sap_score=True)
-    with pytest.raises(ValueError, match="has 10001 items, not the 10000"):
-        sw(_device_loader(_Grid([100, 100], n=10001)), epochs=1, metrics_every=1, sap_score=True)
-    assert sw.loader is None and not sw._device_loaders
-    sw.loader = _device_loader(_Grid([100, 100], n=10001))
-    with pytest.raises(ValueError, match="has 10001 items, not the 10000"):
-        sw.evaluate(is_metrics=False, is_losses=False, is_sap_score=True)
 
 
 # ---- the host path with an fp64 stand-in for the kernel -----------------------------------------------------------

@@ -13,7 +13,8 @@
 //     (b = b' - W m afterwards); it keeps features far from zero from coupling the intercept to the weights.
 //   - Truncated Newton: preconditioned conjugate gradient on Hessian-vector products H v = v_W + sum_i q_i(v) x~_i^T
 //     (q_ir = p_ir (u_ir - sum_s p_is u_is), u_i = V x~_i; p(1-p) u for binary), with the Hessian's diagonal as the
-//     preconditioner, stopped at |r| <= min(0.5, sqrt(|g| / |g_0|)) |g|; then an Armijo backtracking line search.
+//     preconditioner, stopped at |r| <= min(0.5, sqrt(|g| / |g_0|)) |g|; then an Armijo backtracking line search,
+//     except that a full step promising a decrease below 1e-12 |f| (beneath f's rounding) is taken whole.
 //   - For nc > 2 f is flat along "add a constant to every b_r", so every gradient, product and preconditioned
 //     residual has its b part projected onto sum_r b_r = 0, and the solution is reported with sum_r b_r = 0.
 //   - Converged when max_j |g_j| <= 1e-10 * max_j s_j, s_j = [j a weight] |theta_j| + sum_i |q_ir x~_id|: the scale of
@@ -38,6 +39,7 @@ constexpr int kFitMaxCG = 250;              // conjugate-gradient steps per Newt
 constexpr int kFitMaxHalvings = 40;
 constexpr double kFitTol = 1e-10;
 constexpr double kFitArmijo = 1e-4;
+constexpr double kFitFlat = 1e-12;          // a full step's promised decrease f cannot resolve, relative to |f|
 constexpr int kPairThreads = 256;
 
 __global__ void __launch_bounds__(kPairThreads)
@@ -387,6 +389,10 @@ logistic_fit_kernel(const double* __restrict__ x, int D, int num_train, int num_
     newton_direction(F, sqrt(dot(F, F.grad, F.grad)), gnorm0);
     const double slope = dot(F, F.grad, F.dir);
     if (!(slope < 0.0)) break;
+    // A full step that promises less than kFitFlat |f| of decrease is below what f's rounding can rank: f's noise
+    // would reject it and admit a needlessly short step instead, and the fit would stall just short of the gradient
+    // test (as on separable data with large margins).  Such a step is taken whole, and the gradient test decides.
+    const bool flat = -slope <= kFitFlat * fabs(f);
     bool moved = false;
     double step = 1.0;
     for (int h = 0; h <= kFitMaxHalvings; ++h, step *= 0.5) {
@@ -394,7 +400,7 @@ logistic_fit_kernel(const double* __restrict__ x, int D, int num_train, int num_
       __syncthreads();
       const double ft = objective(F, F.trial);
       // sufficient decrease, or a change of f below its rounding (where only the gradient test can decide)
-      if (ft - f <= kFitArmijo * step * slope + 1e-15 * fabs(f)) {
+      if (flat || ft - f <= kFitArmijo * step * slope + 1e-15 * fabs(f)) {
         for (int o = t; o < F.O; o += kFitThreads) F.theta[o] = F.trial[o];
         __syncthreads();
         f = ft;
@@ -461,7 +467,8 @@ extern "C" {
 
 int dv_pair_abs_diff_mean(const float* mu, int ld, int row_stride, int N, int D, const long long* rows_a,
                           const long long* rows_b, int V, int L, double* x, void* stream) {
-  if (N < 1 || D < 1 || V < 1 || L < 1 || (long long)V * D > 0x7fffffffLL) return DV_ERR_BAD_SHAPE;
+  if (N < 1 || D < 1 || V < 1 || L < 1 || (long long)V * D > 0x7fffffffLL || ld < 1 || row_stride < 1)
+    return DV_ERR_BAD_SHAPE;
   if (!mu || !rows_a || !rows_b || !x) return DV_ERR_BAD_ARG;
   if (misaligned(mu, 4) || misaligned(rows_a, 8) || misaligned(rows_b, 8) || misaligned(x, 8)) return DV_ERR_BAD_ARG;
   const long long total = (long long)V * D;

@@ -5,10 +5,12 @@
 //   group g = rows[g][0 .. L-1],  s = mu[rows[g][0]][d] (the group's first row)
 //   r       = mean_l (mu[rows[g][l]][d] - s)
 //   var[d]  = sum_l ((mu[rows[g][l]][d] - s) - r)^2 / (L - 1)
-//   vote    = argmin over d with global_var[d] >= min_var of var[d] / global_var[d], lowest d on a tie
+//   vote    = argmin over d with global_var[d] >= min_var and var[d] / global_var[d] not NaN of that ratio, lowest d
+//             on a tie, -1 if no dim qualifies
 //
-// The two-pass form around s is the one dv_dip_fwd uses: near s the differences are exact in fp32, so a column far
-// from zero (means near 100, spread 0.01) loses no precision.
+// The two-pass form around s keeps a column far from zero (means near 100, spread 0.01) at full precision: the
+// differences from s are exact in fp32 near s.  Since s is a row of the group, |s - mean| is at most about sqrt(L)
+// times the group's spread, so the shift costs at most that factor in the rounding of r and of the squares.
 //
 // One CTA per (group, slice of dims).  Its 256 threads are `lanes` row lanes x `dt` dim lanes (dt a power of two, at
 // most 32, the dims fastest so a warp reads whole runs of a row); row lane j sums rows j, j + lanes, ... in order and a
@@ -89,13 +91,16 @@ fs_group_var_kernel(const float* __restrict__ mu, int ld, int rs, int D, const l
   }
   if (!argmin_out) return;
 
-  // argmin of var / global_var over the active dims; (value, index) order, so the lowest index wins a tie
+  // argmin of var / global_var over the active dims; (value, index) order, so the lowest index wins a tie.  A NaN
+  // ratio (a NaN variance, or inf / inf) does not qualify, as a NaN global variance does not: kept, it would compare
+  // false against everything and drop the true minimum wherever it met it in the butterfly.
   float best = 0.f;
   int bi = -1;
   for (int d = t; d < D; d += kFsThreads) {
     const float gv = global_var[d];
     if (!(gv >= min_var)) continue;
     const float q = sv[d] / gv;
+    if (isnan(q)) continue;
     if (bi < 0 || q < best) { best = q; bi = d; }
   }
 #pragma unroll
@@ -129,7 +134,7 @@ extern "C" {
 
 int dv_group_variance(const float* mu, int ld, int row_stride, int N, int D, const long long* rows, int V, int L,
                       const float* global_var, float min_var, float* var_out, int* argmin_out, void* stream) {
-  if (L < 2 || V < 1 || N < 1 || D < 1 || D > kFsMaxD) return DV_ERR_BAD_SHAPE;
+  if (L < 2 || V < 1 || N < 1 || D < 1 || D > kFsMaxD || ld < 1 || row_stride < 1) return DV_ERR_BAD_SHAPE;
   if (!mu || !rows || (!var_out && !argmin_out) || (argmin_out && !global_var)) return DV_ERR_BAD_ARG;
   if (misaligned(mu, 4) || misaligned(rows, 8) || misaligned(global_var, 4) || misaligned(var_out, 4) ||
       misaligned(argmin_out, 4))

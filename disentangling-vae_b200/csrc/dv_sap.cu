@@ -210,7 +210,8 @@ int dv_sap_score_matrix(const float* mu, int ld, int row_stride, int N, int D, c
                         const int* test_cls, const int* n_classes, const int* counts, int K, int class_stride,
                         double C, float* score, double* coef, int* iters, void* stream) {
   if (N < 1 || D < 1 || D > kSapMaxD || num_train < 1 || num_train > kSapMaxTrain || num_test < 1 || K < 1 ||
-      class_stride < 1 || class_stride > kSapMaxClasses || (long long)D * K > 0x7fffffffLL)
+      class_stride < 1 || class_stride > kSapMaxClasses || (long long)D * K > 0x7fffffffLL || ld < 1 ||
+      row_stride < 1)
     return DV_ERR_BAD_SHAPE;
   if (!mu || !train_rows || !test_rows || !train_cls || !test_cls || !n_classes || !counts || !score)
     return DV_ERR_BAD_ARG;

@@ -205,11 +205,16 @@ def group_variance(mu, rows, global_var=None, var_out=None, argmin_out=None):
     """`dv_group_variance` on `mu` [N, D] (any strides, a view of q_zCx included) and int64 `rows` [V, L]: the
     unbiased variance of every group into `var_out` [V, D], and / or into int32 `argmin_out` [V] the dim minimising
     var / global_var over the dims with global_var >= FACTOR_SCORE_MIN_VAR."""
-    N.require_cuda_f32(mu, global_var, var_out)
+    N.require_cuda_f32(mu)
     n, d = mu.shape
     V, L = rows.shape
     if rows.dtype != torch.int64 or not rows.is_contiguous():
         raise ValueError("group_variance: rows must be a contiguous int64 tensor")
+    for name, t, dtype, shape in (("var_out", var_out, torch.float32, (V, d)),
+                                  ("argmin_out", argmin_out, torch.int32, (V,)),
+                                  ("global_var", global_var, torch.float32, (d,))):
+        if t is not None and (t.dtype != dtype or not t.is_contiguous() or not t.is_cuda or tuple(t.shape) != shape):
+            raise ValueError("group_variance: %s must be a contiguous CUDA %s tensor of shape %s" % (name, dtype, shape))
     N.call("dv_group_variance", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(rows), V, L, N.ptr(global_var),
            FACTOR_SCORE_MIN_VAR, N.ptr(var_out), N.ptr(argmin_out), N.stream())
 

@@ -348,10 +348,12 @@ int dv_latent_entropy(const float* zs, const float* mean, const float* logvar, i
  * caller builds them), repeats allowed.
  *   var_out[g][d] = unbiased variance (ddof 1) of mu[rows[g][l]][d] over l, in the centred two-pass form around
  *                   the group's first row (optional, [V][D])
- *   argmin_out[g] = the d minimising var[g][d] / global_var[d] over the dims with global_var[d] >= min_var, the lowest
- *                   d on a tie; -1 if no dim qualifies (optional, [V]; needs global_var [D])
+ *   argmin_out[g] = the d minimising var[g][d] / global_var[d] over the dims that qualify: global_var[d] >= min_var
+ *                   and the ratio (fp32, IEEE division) not NaN.  The lowest d wins a tie; -1 if no dim qualifies
+ *                   (optional, [V]; needs global_var [D]).  A NaN variance (inf or NaN among the group's rows) thus
+ *                   never takes or blocks a vote; an infinite ratio qualifies and orders above every finite one.
  * One launch, no workspace.  Deterministic (fixed-order reductions, no floating-point atomics), graph-capturable.
- * DV_ERR_BAD_SHAPE: L < 2, V < 1, N < 1, D < 1 or D > 1024.
+ * DV_ERR_BAD_SHAPE: L < 2, V < 1, N < 1, D < 1, D > 1024, ld < 1 or row_stride < 1.
  * DV_ERR_BAD_ARG: mu or rows NULL, both outputs NULL, argmin_out without global_var, or a pointer misaligned (rows
  * 8 bytes, the others 4). */
 int dv_group_variance(const float* mu, int ld, int row_stride, int N, int D, const long long* rows, int V, int L,
@@ -376,8 +378,8 @@ int dv_group_variance(const float* mu, int ld, int row_stride, int N, int D, con
  *   iters int32 [D][K][class_stride] (optional): Newton steps of problem p, -1 if it did not converge; 0 beyond
  * Rows are in [0, N) and labels within their ranges (not checked: the caller builds them).  One launch of D*K CTAs, no
  * workspace.  Deterministic (fixed-order reductions, no floating-point atomics), graph-capturable.
- * DV_ERR_BAD_SHAPE: N < 1, D < 1, D > 1024, num_train < 1, num_train > 32768, num_test < 1, K < 1, class_stride < 1
- * or class_stride > 256.
+ * DV_ERR_BAD_SHAPE: N < 1, D < 1, D > 1024, num_train < 1, num_train > 32768, num_test < 1, K < 1, class_stride < 1,
+ * class_stride > 256, ld < 1 or row_stride < 1.
  * DV_ERR_BAD_ARG: a required pointer NULL, C not finite and positive, or a pointer misaligned (rows and coef 8 bytes,
  * the others 4). */
 int dv_sap_score_matrix(const float* mu, int ld, int row_stride, int N, int D, const long long* train_rows,
@@ -391,7 +393,7 @@ int dv_sap_score_matrix(const float* mu, int ld, int row_stride, int N, int D, c
  * mu is read as dv_group_variance reads it (element (n, d) at n*row_stride + d*ld; q_zCx in place).  rows_a, rows_b:
  * int64 [V][L], every entry in [0, N) (not checked).  x: fp64 [V][D].  One launch, no workspace, deterministic,
  * graph-capturable.
- * DV_ERR_BAD_SHAPE: N < 1, D < 1, V < 1, L < 1 or V*D > INT_MAX.
+ * DV_ERR_BAD_SHAPE: N < 1, D < 1, V < 1, L < 1, V*D > INT_MAX, ld < 1 or row_stride < 1.
  * DV_ERR_BAD_ARG: a NULL pointer, or one misaligned (mu 4 bytes, the others 8). */
 int dv_pair_abs_diff_mean(const float* mu, int ld, int row_stride, int N, int D, const long long* rows_a,
                           const long long* rows_b, int V, int L, double* x, void* stream);
@@ -404,7 +406,8 @@ int dv_pair_abs_diff_mean(const float* mu, int ld, int row_stride, int N, int D,
  *   nc = 2: one binary model, 1/2 |w|^2 + sum_i log(1 + exp(-s_i (w.x_i + b))), s_i = +1 for class 1;
  *   nc = 1: no fit.
  * Solved in fp64 by truncated Newton (diagonally preconditioned conjugate gradient on Hessian-vector products over
- * features centred on their training mean, Armijo line search), to max |gradient| <= 1e-10 of the largest scale of
+ * features centred on their training mean, Armijo line search; a full step whose promised decrease is below 1e-12 |f|,
+ * which f's rounding cannot rank, is taken whole), to max |gradient| <= 1e-10 of the largest scale of
  * the gradient's parts (|weight| + sum_i |q_i x_i|).
  *   coef  fp64 [K][D + 1]: row c = (W_c, b_c) for c < nc (nc > 2) or row 0 = (w, b) (nc = 2); NaN elsewhere
  *   pred  int32 [num_train + num_eval]: argmax_c W_c x + b_c, the lowest c on a tie; class 1 if w.x + b > 0 for nc = 2;

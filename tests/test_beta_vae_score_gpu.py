@@ -190,8 +190,9 @@ def test_refusals_launch_nothing():
     rows = torch.zeros(16, 4, dtype=torch.int64, device=DEV)
     x = torch.full((16, 8), 7.0, dtype=torch.float64, device=DEV)
 
-    def pair(mu=mu.data_ptr(), N=100, D=8, a=rows.data_ptr(), b=rows.data_ptr(), V=16, Lp=4, x=x.data_ptr()):
-        return L.dv_pair_abs_diff_mean(mu, 1, 8, N, D, a, b, V, Lp, x, S)
+    def pair(mu=mu.data_ptr(), ld=1, rs=8, N=100, D=8, a=rows.data_ptr(), b=rows.data_ptr(), V=16, Lp=4,
+             x=x.data_ptr()):
+        return L.dv_pair_abs_diff_mean(mu, ld, rs, N, D, a, b, V, Lp, x, S)
 
     labels = torch.zeros(12, dtype=torch.int32, device=DEV)
     ncl = torch.tensor([1, 0], dtype=torch.int32, device=DEV)
@@ -212,7 +213,8 @@ def test_refusals_launch_nothing():
         torch.cuda.synchronize()
         assert rc == rc_want and L.dv_launch_count() == before, (fn.__name__, kw, rc)
 
-    for shape in (dict(N=0), dict(D=0), dict(V=0), dict(Lp=0), dict(V=2 ** 30, D=8)):
+    for shape in (dict(N=0), dict(D=0), dict(V=0), dict(Lp=0), dict(V=2 ** 30, D=8), dict(ld=0), dict(ld=-1),
+                  dict(rs=0), dict(rs=-8)):
         refused(pair, DV_ERR_BAD_SHAPE, **shape)
     for bad in (dict(mu=None), dict(a=None), dict(b=None), dict(x=None), dict(mu=mu.data_ptr() + 2),
                 dict(a=rows.data_ptr() + 4), dict(b=rows.data_ptr() + 4), dict(x=x.data_ptr() + 4)):

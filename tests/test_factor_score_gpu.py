@@ -154,9 +154,9 @@ def test_refusals_launch_nothing():
     arg = torch.full((4,), 7, dtype=torch.int32, device=DEV)
     S = torch.cuda.current_stream().cuda_stream
 
-    def args(mu=mu.data_ptr(), N=100, D=8, rows=rows.data_ptr(), V=4, Lr=8, gv=gv.data_ptr(), var=var.data_ptr(),
-             arg=arg.data_ptr()):
-        return (mu, 1, 8, N, D, rows, V, Lr, gv, 0.05, var, arg, S)
+    def args(mu=mu.data_ptr(), ld=1, rs=8, N=100, D=8, rows=rows.data_ptr(), V=4, Lr=8, gv=gv.data_ptr(),
+             var=var.data_ptr(), arg=arg.data_ptr()):
+        return (mu, ld, rs, N, D, rows, V, Lr, gv, 0.05, var, arg, S)
 
     def refused(rc_want, **kw):
         torch.cuda.synchronize()
@@ -165,7 +165,8 @@ def test_refusals_launch_nothing():
         torch.cuda.synchronize()
         assert rc == rc_want and L.dv_launch_count() == before, (kw, rc)
 
-    for shape in (dict(Lr=1), dict(Lr=0), dict(V=0), dict(N=0), dict(D=0), dict(D=1025)):
+    for shape in (dict(Lr=1), dict(Lr=0), dict(V=0), dict(N=0), dict(D=0), dict(D=1025), dict(ld=0), dict(ld=-1),
+                  dict(rs=0), dict(rs=-8)):
         refused(DV_ERR_BAD_SHAPE, **shape)
     for bad in (dict(mu=None), dict(rows=None), dict(var=None, arg=None), dict(gv=None), dict(mu=mu.data_ptr() + 2),
                 dict(rows=rows.data_ptr() + 4), dict(gv=gv.data_ptr() + 1), dict(var=var.data_ptr() + 2),

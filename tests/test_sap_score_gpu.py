@@ -190,10 +190,10 @@ def test_refusals_launch_nothing():
     iters = torch.full((8, 2, 4), 7, dtype=torch.int32, device=DEV)
     S = torch.cuda.current_stream().cuda_stream
 
-    def args(mu=mu.data_ptr(), N=100, D=8, tr=rows.data_ptr(), ntr=16, te=rows.data_ptr(), nte=16,
+    def args(mu=mu.data_ptr(), ld=1, rs=8, N=100, D=8, tr=rows.data_ptr(), ntr=16, te=rows.data_ptr(), nte=16,
              trc=cls.data_ptr(), tec=cls.data_ptr(), ncl=ncl.data_ptr(), cnt=cnt.data_ptr(), K=2, cs=4, C=0.01,
              score=score.data_ptr(), coef=coef.data_ptr(), iters=iters.data_ptr()):
-        return (mu, 1, 8, N, D, tr, ntr, te, nte, trc, tec, ncl, cnt, K, cs, C, score, coef, iters, S)
+        return (mu, ld, rs, N, D, tr, ntr, te, nte, trc, tec, ncl, cnt, K, cs, C, score, coef, iters, S)
 
     def refused(rc_want, **kw):
         torch.cuda.synchronize()
@@ -203,7 +203,7 @@ def test_refusals_launch_nothing():
         assert rc == rc_want and L.dv_launch_count() == before, (kw, rc)
 
     for shape in (dict(N=0), dict(D=0), dict(D=1025), dict(ntr=0), dict(ntr=32769), dict(nte=0), dict(K=0),
-                  dict(cs=0), dict(cs=257)):
+                  dict(cs=0), dict(cs=257), dict(ld=0), dict(ld=-1), dict(rs=0), dict(rs=-8)):
         refused(DV_ERR_BAD_SHAPE, **shape)
     for bad in (dict(mu=None), dict(tr=None), dict(te=None), dict(trc=None), dict(tec=None), dict(ncl=None),
                 dict(cnt=None), dict(score=None), dict(C=0.0), dict(C=-1.0), dict(C=float("nan")),

@@ -76,6 +76,8 @@ SIGNATURES = {
     "dv_pair_abs_diff_mean": (I, [P, I, I, I, I, P, P, I, I, P, P]),
     "dv_logistic_fit_workspace_bytes": (SZ, [I, I, I]),
     "dv_logistic_fit": (I, [P, I, I, I, P, P, I, P, P, P, P, SZ, P]),
+    "dv_dci_workspace_bytes": (SZ, [I, I, I, I, I]),
+    "dv_dci_fit": (I, [P, I, I, I, I, P, I, P, I, P, P, P, I, I, I, P, P, P, P, P, P, SZ, P]),
     "dv_permute_dims": (I, [P, P, ULL, P, P, I, I, P]),
     "dv_permute_dims_workspace_bytes": (SZ, [I, I]),
     "dv_permute_dims_rows": (I, [P, P, ULL, P, P, I, I, I, I, P, P]),

@@ -33,6 +33,10 @@ SAP_MAX_TRAIN = 32768                      # training rows staged in shared memo
 SAP_MAX_CLASSES = 256                      # and values of a scored factor
 BETA_VAE_MAX_DIM = 128                     # dv_logistic_fit's limits: latents,
 BETA_VAE_MAX_FACTORS = 32                  # and scored factors (classes)
+DCI_MAX_DIM = 1024                         # dv_dci_fit's limits: latents,
+DCI_MAX_TRAIN = 32768                      # training rows,
+DCI_MAX_CLASSES = 256                      # and values of a scored factor
+DCI_STAGES = 100                           # GradientBoostingClassifier()'s n_estimators
 EVAL_SEED_STRIDE = 0x9E3779B97F4A7C15      # odd 64-bit constant: consecutive epochs get unrelated seeds
 
 
@@ -521,6 +525,119 @@ def beta_vae_score(mu, lat_sizes, batch_size=64, num_train=10000, num_eval=5000,
     return score, helpers
 
 
+# ---- DCI score (Eastwood & Williams 2018; disentanglement_lib's dci.py with GradientBoostingClassifier()) ----------
+def check_dci_score(dataset, latent_dim, num_train=10000, num_test=5000):
+    """ValueError unless the DCI score can be computed over `dataset` for a `latent_dim` model with these settings: the
+    dataset has known factors (`lat_sizes`, `lat_names`), is their full grid and has at least 2 factors of more than
+    one value.  No GPU work.  Returns lat_sizes as a list of ints."""
+    return _check_dci_grid(_dataset_lat_sizes("DCI score", dataset), len(dataset), latent_dim, num_train, num_test)
+
+
+def _check_dci_grid(lat_sizes, n, latent_dim, num_train, num_test):
+    lat_sizes = _full_grid("DCI score", lat_sizes, n)
+    scored = sum(s > 1 for s in lat_sizes)
+    if scored < 2:
+        raise ValueError("DCI score: %s has %d factors of more than one value; completeness is an entropy over the "
+                         "factors and needs at least 2" % (lat_sizes, scored))
+    if max(lat_sizes) > DCI_MAX_CLASSES:
+        raise ValueError("DCI score: a factor of %s has more than the kernel's limit of %d values"
+                         % (lat_sizes, DCI_MAX_CLASSES))
+    if int(latent_dim) < 2:
+        raise ValueError("DCI score: latent_dim must be at least 2 (disentanglement is an entropy over the latents), "
+                         "got %d" % int(latent_dim))
+    if int(latent_dim) > DCI_MAX_DIM:
+        raise ValueError("DCI score: latent_dim %d is above the kernel's limit of %d" % (int(latent_dim), DCI_MAX_DIM))
+    if int(num_train) < 1:
+        raise ValueError("DCI score: num_train must be at least 1, got %d" % int(num_train))
+    if int(num_train) > DCI_MAX_TRAIN:
+        raise ValueError("DCI score: num_train %d is above the kernel's limit of %d" % (int(num_train), DCI_MAX_TRAIN))
+    if int(num_test) < 1:
+        raise ValueError("DCI score: num_test must be at least 1, got %d" % int(num_test))
+    return lat_sizes
+
+
+def dci_fit(mu, train_rows, test_rows, train_cls, n_classes, counts, stages=DCI_STAGES, trees=False):
+    """`dv_dci_fit` on `mu` [N, D] (any strides, a view of q_zCx included) and `sap_labels`' classes -> (importance
+    fp64 [D, K'], pred int32 [K', num_train + num_test] (class indices), trees), trees = None or (feature int32,
+    threshold fp64, value fp64), each [K', S, stages, 15]; see include/disvae_b200.h for the fit."""
+    N.require_cuda_f32(mu)
+    n, d = mu.shape
+    K, S = counts.shape
+    for name, t, dtype in (("train_rows", train_rows, torch.int64), ("test_rows", test_rows, torch.int64),
+                           ("train_cls", train_cls, torch.int32), ("n_classes", n_classes, torch.int32),
+                           ("counts", counts, torch.int32)):
+        if t.dtype != dtype or not t.is_contiguous() or not t.is_cuda:
+            raise ValueError("dci_fit: %s must be a contiguous CUDA %s tensor" % (name, dtype))
+    num_train, num_test = train_rows.numel(), test_rows.numel()
+    nbytes = N.lib().dv_dci_workspace_bytes(d, num_train, num_test, K, S)
+    ws = torch.empty(max(nbytes, 8) // 8, dtype=torch.float64, device=mu.device)
+    importance = torch.empty(d, K, dtype=torch.float64, device=mu.device)
+    pred = torch.empty(K, num_train + num_test, dtype=torch.int32, device=mu.device)
+    out = None
+    if trees:
+        shape = (K, S, int(stages), 15)
+        out = (torch.empty(shape, dtype=torch.int32, device=mu.device),
+               torch.empty(shape, dtype=torch.float64, device=mu.device),
+               torch.empty(shape, dtype=torch.float64, device=mu.device))
+    N.call("dv_dci_fit", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(train_rows), num_train, N.ptr(test_rows),
+           num_test, N.ptr(train_cls), N.ptr(n_classes), N.ptr(counts), K, S, int(stages), N.ptr(importance),
+           N.ptr(pred), *(N.ptr(t) for t in (out or (None, None, None))), N.ptr(ws), nbytes, N.stream())
+    return importance, pred, out
+
+
+def _entropy(p, base):
+    """scipy.stats.entropy(p, base=base) along axis 0 of a non-negative fp64 array."""
+    p = p / p.sum(0)
+    return -torch.where(p > 0, p * torch.log(p), torch.zeros_like(p)).sum(0) / math.log(base)
+
+
+def dci_from_importance(importance):
+    """(disentanglement, completeness) of an importance matrix R [D, K'] (D, K' >= 2), as dci.py computes them in
+    fp64: disentanglement = sum_d rho_d (1 - H_K'(R[d, :] + 1e-11)), completeness = sum_k rho_k (1 - H_D(R[:, k] +
+    1e-11)), rho the row (column) sums over the total, of a matrix of ones when R sums to 0."""
+    R = importance.double().cpu()
+    D, K = R.shape
+    per_code = 1.0 - _entropy(R.t() + 1e-11, K)
+    per_factor = 1.0 - _entropy(R + 1e-11, D)
+    W = torch.ones_like(R) if float(R.sum()) == 0.0 else R
+    return (float((per_code * (W.sum(1) / W.sum())).sum()), float((per_factor * (W.sum(0) / W.sum())).sum()))
+
+
+def dci_score(mu, lat_sizes, num_train=10000, num_test=5000, seed=0):
+    """DCI score of the encoder means `mu` [N, D] (CUDA fp32, dataset index order) of the full factor grid `lat_sizes`
+    -> ({"disentanglement", "completeness", "informativeness_train", "informativeness_test"}, helpers).  The draws
+    are SAP's: a device torch.Generator seeded with `seed`, `torch.randint(N, (num_train,))` for the training rows,
+    then `torch.randint(N, (num_test,))` for the test rows; the global generators are not touched.  For every scored
+    factor `dci_fit` grows GradientBoostingClassifier()'s 100 boosting stages on the training rows; a factor seen with
+    one value in training has no trees, zero importance and predicts that value.  The informativeness scores are the
+    mean accuracies over the factors (a test value unseen in training is never predicted right).
+    helpers: "importance_matrix" fp64 [D, K'], "factors" (the scored factor indices, ascending), "classes" int64
+    [K', S] (each factor's training values, ascending, -1 beyond), "train_accuracy" and "test_accuracy" fp64 [K']."""
+    lat_sizes = _check_dci_grid(lat_sizes, mu.shape[0], mu.shape[1], num_train, num_test)
+    N.require_cuda_f32(mu)
+    n = mu.shape[0]
+    num_train = int(num_train)
+    gen = torch.Generator(device=mu.device)
+    gen.manual_seed(int(seed))
+    train_rows = torch.randint(n, (num_train,), generator=gen, device=mu.device)
+    test_rows = torch.randint(n, (int(num_test),), generator=gen, device=mu.device)
+    factors, train_cls, test_cls, n_classes, counts, present = sap_labels(lat_sizes, train_rows, test_rows)
+    K, S = counts.shape
+    importance, pred, _ = dci_fit(mu, train_rows, test_rows, train_cls, n_classes, counts)
+    right = pred == torch.cat([train_cls, test_cls], 1)
+    train_acc = right[:, :num_train].double().mean(1).cpu()
+    test_acc = right[:, num_train:].double().mean(1).cpu()
+    importance, present = importance.cpu(), present.cpu()
+    disentanglement, completeness = dci_from_importance(importance)
+    classes = torch.sort(torch.where(present, torch.arange(S).expand(K, S), S), dim=1)[0]
+    helpers = {"importance_matrix": importance, "factors": torch.tensor(factors, dtype=torch.int64),
+               "classes": torch.where(classes < S, classes, -1), "train_accuracy": train_acc,
+               "test_accuracy": test_acc}
+    score = {"disentanglement": disentanglement, "completeness": completeness,
+             "informativeness_train": float(train_acc.mean()), "informativeness_test": float(test_acc.mean())}
+    return score, helpers
+
+
 # ---- the scores the Evaluator, training and sweeps write ----------------------------------------------------------
 class Score(NamedTuple):
     """A disentanglement score the Evaluator writes beside MIG / AAM.  `flag` names its switches: the Evaluator's
@@ -646,6 +763,14 @@ class Evaluator:
         see `beta_vae_score` for the definition and the order of the draws."""
         return self._score(check_beta_vae_score, beta_vae_score, dataloader, seed, batch_size=batch_size,
                            num_train=num_train, num_eval=num_eval)
+
+    def compute_dci_score(self, dataloader, num_train=10000, num_test=5000, seed=0):
+        """DCI score (Eastwood & Williams 2018) of the model's encoder means over `dataloader` (the dataset in index
+        order: DataLoader(shuffle=False) or DeviceLoader.in_order) -> {"disentanglement", "completeness",
+        "informativeness_train", "informativeness_test"}; see `dci_score` for the definition and the order of the
+        draws.  The Evaluator's __call__, training and sweeps do not write this score; score a sweep's members with
+        `Evaluator(member.model, ...).compute_dci_score(sweep.loader.in_order(1000), seed=...)`."""
+        return self._score(check_dci_score, dci_score, dataloader, seed, num_train=num_train, num_test=num_test)
 
     def _score(self, check, compute, dataloader, seed, **settings):
         """`compute(encoder means, lat_sizes, seed=seed, **settings)`'s score, after `check(dataset, latent_dim,

@@ -423,6 +423,63 @@ int dv_logistic_fit(const double* x, int D, int num_train, int num_eval, const i
                     int K, double* coef, int* pred, int* iters, void* workspace, size_t workspace_bytes,
                     void* stream);
 
+/* ---- disentanglement metrics: DCI score (Eastwood & Williams 2018; disentanglement_lib's dci.py) -----------
+ * dv_dci_fit: for every scored factor k < K, the gradient-boosted trees of sklearn's GradientBoostingClassifier() at
+ * its defaults (log loss, `stages` boosting stages of learning rate 0.1, one depth-3 friedman_mse regression tree per
+ * column per stage) fitted to the training rows' classes, their feature importances, and the predicted classes of the
+ * training and test rows.
+ * Inputs: mu is read as dv_group_variance reads it (element (n, d) at n*row_stride + d*ld; q_zCx in place), finite
+ * values assumed.  train_rows int64 [num_train] and test_rows int64 [num_test], every entry in [0, N) (not checked).
+ * train_cls int32 [K][num_train] (classes 0 .. nc-1, every class present), n_classes int32 [K] (nc, clamped to
+ * [0, class_stride]) and counts int32 [K][class_stride] (training rows of each class), as dv_sap_score_matrix takes
+ * them from the same labelling.  Training values x are the fp32 means; a row goes left at a node when
+ * (double)x <= threshold.
+ * The fit of a factor with nc classes (cols = nc columns for nc > 2, 1 for nc = 2, none for nc <= 1):
+ *   initial raw scores from the priors p_c = counts[c] / num_train clipped to [FLT_EPSILON, 1 - FLT_EPSILON]:
+ *     log(p_c / gmean(p)) per column for nc > 2, logit(p_1) for nc = 2;
+ *   each stage takes the residuals at its starting scores, r_c = [y = c] - softmax(raw)_c (nc > 2) or
+ *     r = [y = 1] - sigmoid(raw) (nc = 2), and grows one tree per column on them:
+ *     a node is a leaf at depth 3, below 2 rows, at impurity sum (r - mean)^2 / n <= DBL_EPSILON (sklearn's
+ *     sum r^2 / n - (sum r / n)^2, in the centred form: a node of equal residuals has impurity 0 up to rounding far
+ *     below DBL_EPSILON, where the difference of two sums leaves noise of that size), or without a
+ *     split candidate; a candidate lies between consecutive sorted values of the node with x_b > x_a + 1e-7 (fp64)
+ *     and has threshold x_a/2 + x_b/2 in fp64 (x_a if that equals x_b); the split maximises the friedman_mse proxy
+ *     (n_r S_l - n_l S_r)^2 / (n_l n_r), with S_l and S_r the sums of the residuals rounded to int64 fixed point at
+ *     2^-40, added exactly and converted with one rounding each (so one partition always has one proxy); an exact tie
+ *     goes to the lowest latent, then the lowest threshold;
+ *     a leaf's value is sum r / sum p (1 - p) over its rows with p = [y = c] - r, times (nc - 1) / nc for nc > 2, and
+ *     0 when |sum p (1 - p)| < 1e-150; every training and test row then takes raw += 0.1 * value, the product and
+ *     the sum each rounded (no fused multiply-add).
+ *   Impurities and leaf values are fp64 sums in a fixed order.
+ * Outputs:
+ *   importance fp64 [D][K]: column k is sklearn's feature_importances_ in absolute value: per tree, every internal
+ *              node adds (n imp - n_l imp_l - n_r imp_r) / num_train to its latent; the mean over the factor's trees
+ *              of more than one node, divided by its sum.  Zeros when there is no such tree (nc <= 1 included) or the
+ *              sum is 0.
+ *   pred       int32 [K][num_train + num_test]: the class of every training row, then of every test row: argmax of the
+ *              raw scores (the lowest column on a tie) for nc > 2, 1 iff raw >= 0 for nc = 2, 0 for nc <= 1.
+ *   tree_feature int32, tree_threshold fp64, tree_value fp64 [K][class_stride][stages][15] (each optional, NULL for
+ *              none): the 15 heap-ordered nodes (children of node h: 2h + 1, 2h + 2) of the tree of column c at each
+ *              stage: feature = the latent of an internal node, -1 for a leaf, -2 for a node the tree does not have
+ *              (and every node of a column the factor does not have); threshold of an internal node, value of a leaf,
+ *              NaN elsewhere.
+ * workspace: dv_dci_workspace_bytes(D, num_train, num_test, K, class_stride) bytes, 8-byte aligned, contents
+ * irrelevant.  4 + 2 * stages launches (prep and sort, init, a residual and a tree launch per stage, importance,
+ * predict), no host synchronisation, graph-capturable.  Deterministic (fixed-order reductions, no floating-point
+ * atomics).  stages = 0 predicts from the priors.
+ * DV_ERR_BAD_SHAPE: N < 1, D < 1, D > 1024, num_train < 1, num_train > 32768, num_test < 1, K < 1, class_stride < 1,
+ * class_stride > 256, stages < 0, ld < 1, row_stride < 1, or K*(num_train + num_test), num_train + num_test or
+ * K*class_stride*stages*15 above INT_MAX.
+ * DV_ERR_BAD_ARG: a required pointer NULL (all but the three tree outputs), or a pointer misaligned (rows, importance,
+ * tree_threshold, tree_value and workspace 8 bytes, the others 4).
+ * DV_ERR_WORKSPACE: workspace NULL or smaller than the query. */
+size_t dv_dci_workspace_bytes(int D, int num_train, int num_test, int K, int class_stride);  /* 0: unsupported */
+int dv_dci_fit(const float* mu, int ld, int row_stride, int N, int D, const long long* train_rows, int num_train,
+               const long long* test_rows, int num_test, const int* train_cls, const int* n_classes,
+               const int* counts, int K, int class_stride, int stages, double* importance, int* pred,
+               int* tree_feature, double* tree_threshold, double* tree_value, void* workspace,
+               size_t workspace_bytes, void* stream);
+
 /* ---- FactorVAE pieces ---------------------------------------------------------------------
  * dv_permute_dims replaces _permute_dims (losses.py:483-508): out[b][d] = z[perm[d][b]][d].
  * perms != NULL: int64 [D][B] (the reference's CPU randperm stream, trap T7).  perms == NULL:

@@ -37,6 +37,10 @@ DCI_MAX_DIM = 1024                         # dv_dci_fit's limits: latents,
 DCI_MAX_TRAIN = 32768                      # training rows,
 DCI_MAX_CLASSES = 256                      # and values of a scored factor
 DCI_STAGES = 100                           # GradientBoostingClassifier()'s n_estimators
+MODULARITY_MAX_DIM = 128                   # dv_explicitness_fit's limits: latents,
+MODULARITY_MAX_TRAIN = 32768               # training rows,
+MODULARITY_MAX_CLASSES = 256               # and values of a scored factor
+MODULARITY_BINS = 20                       # disentanglement_lib's num_bins of the mutual information
 EVAL_SEED_STRIDE = 0x9E3779B97F4A7C15      # odd 64-bit constant: consecutive epochs get unrelated seeds
 
 
@@ -638,6 +642,154 @@ def dci_score(mu, lat_sizes, num_train=10000, num_test=5000, seed=0):
     return score, helpers
 
 
+# ---- modularity and explicitness (Ridgeway & Zemel 2018; disentanglement_lib's modularity_explicitness.py) --------
+def check_modularity_explicitness(dataset, latent_dim, num_train=10000, num_test=5000):
+    """ValueError unless modularity and explicitness can be computed over `dataset` for a `latent_dim` model with these
+    settings: the dataset has known factors (`lat_sizes`, `lat_names`), is their full grid and has at least 2 factors
+    of more than one value.  No GPU work.  Returns lat_sizes as a list of ints."""
+    return _check_modularity_grid(_dataset_lat_sizes("modularity score", dataset), len(dataset), latent_dim, num_train,
+                                  num_test)
+
+
+def _check_modularity_grid(lat_sizes, n, latent_dim, num_train, num_test):
+    lat_sizes = _full_grid("modularity score", lat_sizes, n)
+    scored = sum(s > 1 for s in lat_sizes)
+    if scored < 2:
+        raise ValueError("modularity score: %s has %d factors of more than one value; modularity divides by the "
+                         "factors less one and needs at least 2" % (lat_sizes, scored))
+    if max(lat_sizes) > MODULARITY_MAX_CLASSES:
+        raise ValueError("modularity score: a factor of %s has more than the kernel's limit of %d values"
+                         % (lat_sizes, MODULARITY_MAX_CLASSES))
+    if not 1 <= int(latent_dim) <= MODULARITY_MAX_DIM:
+        raise ValueError("modularity score: latent_dim must be in [1, %d], got %d" % (MODULARITY_MAX_DIM,
+                                                                                      int(latent_dim)))
+    if not 1 <= int(num_train) <= MODULARITY_MAX_TRAIN:
+        raise ValueError("modularity score: num_train must be in [1, %d], got %d" % (MODULARITY_MAX_TRAIN,
+                                                                                     int(num_train)))
+    if int(num_test) < 1:
+        raise ValueError("modularity score: num_test must be at least 1, got %d" % int(num_test))
+    return lat_sizes
+
+
+def _require_labels(fn, tensors):
+    for name, t, dtype in tensors:
+        if t.dtype != dtype or not t.is_contiguous() or not t.is_cuda:
+            raise ValueError("%s: %s must be a contiguous CUDA %s tensor" % (fn, name, dtype))
+
+
+def discrete_mutual_info(mu, train_rows, train_cls, n_classes, class_stride):
+    """`dv_discrete_mutual_info` on `mu` [N, D] (any strides, a view of q_zCx included) and `sap_labels`' training
+    classes -> (mi fp64 [D, K'], edges fp32 [D, 21]): sklearn's mutual_info_score of every factor's classes with every
+    latent's 20-bin histogram discretisation over the training rows; see include/disvae_b200.h for the rules."""
+    N.require_cuda_f32(mu)
+    n, d = mu.shape
+    _require_labels("discrete_mutual_info", (("train_rows", train_rows, torch.int64),
+                                             ("train_cls", train_cls, torch.int32),
+                                             ("n_classes", n_classes, torch.int32)))
+    K = n_classes.numel()
+    mi = torch.empty(d, K, dtype=torch.float64, device=mu.device)
+    edges = torch.empty(d, MODULARITY_BINS + 1, dtype=torch.float32, device=mu.device)
+    N.call("dv_discrete_mutual_info", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(train_rows),
+           train_rows.numel(), N.ptr(train_cls), N.ptr(n_classes), K, int(class_stride), N.ptr(mi), N.ptr(edges),
+           N.stream())
+    return mi, edges
+
+
+def explicitness_fit(mu, train_rows, test_rows, train_cls, test_cls, n_classes, class_stride, proba=False):
+    """`dv_explicitness_fit` on `mu` [N, D] (any strides) and `sap_labels`' classes -> (coef fp64 [K', S, D + 1], auc
+    fp64 [2, K', S] (training, test), iters int32 [K'], mean fp64 [D], std fp64 [D], proba): LogisticRegression(C=1)
+    of every factor on the standardised latents and the ROC AUC of each class column; proba is None or fp64
+    [K', S, num_train + num_test].  See include/disvae_b200.h for the rules."""
+    N.require_cuda_f32(mu)
+    n, d = mu.shape
+    _require_labels("explicitness_fit", (("train_rows", train_rows, torch.int64), ("test_rows", test_rows, torch.int64),
+                                         ("train_cls", train_cls, torch.int32), ("test_cls", test_cls, torch.int32),
+                                         ("n_classes", n_classes, torch.int32)))
+    K, S = n_classes.numel(), int(class_stride)
+    num_train, num_test = train_rows.numel(), test_rows.numel()
+    nbytes = N.lib().dv_explicitness_workspace_bytes(d, num_train, num_test, K, S)
+    ws = torch.empty(max(nbytes, 8) // 8, dtype=torch.float64, device=mu.device)
+    f64 = dict(dtype=torch.float64, device=mu.device)
+    coef, auc = torch.empty(K, S, d + 1, **f64), torch.empty(2, K, S, **f64)
+    iters = torch.empty(K, dtype=torch.int32, device=mu.device)
+    mean, std = torch.empty(d, **f64), torch.empty(d, **f64)
+    out = torch.empty(K, S, num_train + num_test, **f64) if proba else None
+    N.call("dv_explicitness_fit", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(train_rows), num_train,
+           N.ptr(test_rows), num_test, N.ptr(train_cls), N.ptr(test_cls), N.ptr(n_classes), K, S, N.ptr(coef),
+           N.ptr(auc), N.ptr(iters), N.ptr(mean), N.ptr(std), N.ptr(out), N.ptr(ws), nbytes, N.stream())
+    return coef, auc, iters, mean, std, out
+
+
+def modularity_from_mutual_info(mi):
+    """(modularity score, per-latent scores [D]) of a mutual-information matrix [D, K'] (K' >= 2), as
+    modularity_explicitness.py's modularity() computes them in fp64: with m = max_k mi^2, a latent scores
+    1 - (sum_k mi^2 - m) / (m (K' - 1)), or 0 where m = 0; the score is the mean over the latents."""
+    sq = mi.double().cpu() ** 2
+    m = sq.max(1)[0]
+    delta = (sq.sum(1) - m) / (m * (sq.shape[1] - 1.0))
+    per_latent = torch.where(m == 0, torch.zeros_like(m), 1.0 - delta)
+    return float(per_latent.mean()), per_latent
+
+
+def _explicitness_of(auc):
+    """Mean AUC over the defined columns of every factor [K', S] -> [K'] (NaN for a factor without one)."""
+    defined = ~torch.isnan(auc)
+    count = defined.sum(1)
+    total = torch.where(defined, auc, torch.zeros_like(auc)).sum(1)
+    return torch.where(count > 0, total / count.clamp(min=1), torch.full_like(total, float("nan")))
+
+
+def modularity_explicitness(mu, lat_sizes, num_train=10000, num_test=5000, seed=0):
+    """Modularity and explicitness of the encoder means `mu` [N, D] (CUDA fp32, dataset index order) of the full factor
+    grid `lat_sizes` -> ({"modularity_score", "explicitness_score_train", "explicitness_score_test"}, helpers).  The
+    draws are SAP's: a device torch.Generator seeded with `seed`, `torch.randint(N, (num_train,))` for the training
+    rows, then `torch.randint(N, (num_test,))` for the test rows; the global generators are not touched.
+    Modularity is `modularity_from_mutual_info` of `discrete_mutual_info` over the training rows.  Explicitness:
+    `explicitness_fit` fits LogisticRegression(C=1) per scored factor on the standardised latents; a factor's value on
+    a set is the mean ROC AUC over its class columns that have positives and negatives there, NaN for a factor of one
+    training class or without such a column; each score is the mean over the factors with a value (NaN, with a
+    RuntimeWarning, when none has one).
+    helpers: "mutual_information" fp64 [D, K'], "bin_edges" fp32 [D, 21], "modularity_per_latent" fp64 [D],
+    "factors" (the scored factor indices, ascending), "classes" int64 [K', S] (each factor's training values,
+    ascending, -1 beyond), "feature_mean" and "feature_std" fp64 [D], "coef" fp64 [K', S, D + 1] (model rows in
+    standardised features, NaN beyond), "train_auc" and "test_auc" fp64 [K', S] (NaN where undefined),
+    "explicitness_train" and "explicitness_test" fp64 [K'], "solver_iterations" int32 [K'] (Newton steps, -1 for a
+    fit that did not converge, which also raises a RuntimeWarning)."""
+    lat_sizes = _check_modularity_grid(lat_sizes, mu.shape[0], mu.shape[1], num_train, num_test)
+    N.require_cuda_f32(mu)
+    n = mu.shape[0]
+    gen = torch.Generator(device=mu.device)
+    gen.manual_seed(int(seed))
+    train_rows = torch.randint(n, (int(num_train),), generator=gen, device=mu.device)
+    test_rows = torch.randint(n, (int(num_test),), generator=gen, device=mu.device)
+    factors, train_cls, test_cls, n_classes, counts, present = sap_labels(lat_sizes, train_rows, test_rows)
+    K, S = counts.shape
+    mi, edges = discrete_mutual_info(mu, train_rows, train_cls, n_classes, S)
+    coef, auc, iters, mean, std, _ = explicitness_fit(mu, train_rows, test_rows, train_cls, test_cls, n_classes, S)
+    mi, edges, coef, auc, iters = mi.cpu(), edges.cpu(), coef.cpu(), auc.cpu(), iters.cpu()
+    mean, std, present = mean.cpu(), std.cpu(), present.cpu()
+    modularity, per_latent = modularity_from_mutual_info(mi)
+    failed = int((iters < 0).sum())
+    if failed:
+        warnings.warn("modularity score: %d of the logistic-regression fits did not converge in the solver's step "
+                      "limit; see helpers['solver_iterations'] (-1)" % failed, RuntimeWarning)
+    explicit = [_explicitness_of(auc[s]) for s in (0, 1)]
+    score = {"modularity_score": modularity}
+    for name, e in zip(("explicitness_score_train", "explicitness_score_test"), explicit):
+        valued = e[~torch.isnan(e)]
+        if valued.numel() == 0:
+            warnings.warn("modularity score: no factor has an explicitness value on the %s rows; %s is NaN"
+                          % (name.split("_")[-1], name), RuntimeWarning)
+        score[name] = float(valued.mean()) if valued.numel() else float("nan")
+    classes = torch.sort(torch.where(present, torch.arange(S).expand(K, S), S), dim=1)[0]
+    helpers = {"mutual_information": mi, "bin_edges": edges, "modularity_per_latent": per_latent,
+               "factors": torch.tensor(factors, dtype=torch.int64), "classes": torch.where(classes < S, classes, -1),
+               "feature_mean": mean, "feature_std": std, "coef": coef, "train_auc": auc[0].clone(),
+               "test_auc": auc[1].clone(), "explicitness_train": explicit[0], "explicitness_test": explicit[1],
+               "solver_iterations": iters}
+    return score, helpers
+
+
 # ---- the scores the Evaluator, training and sweeps write ----------------------------------------------------------
 class Score(NamedTuple):
     """A disentanglement score the Evaluator writes beside MIG / AAM.  `flag` names its switches: the Evaluator's
@@ -771,6 +923,16 @@ class Evaluator:
         draws.  The Evaluator's __call__, training and sweeps do not write this score; score a sweep's members with
         `Evaluator(member.model, ...).compute_dci_score(sweep.loader.in_order(1000), seed=...)`."""
         return self._score(check_dci_score, dci_score, dataloader, seed, num_train=num_train, num_test=num_test)
+
+    def compute_modularity_explicitness(self, dataloader, num_train=10000, num_test=5000, seed=0):
+        """Modularity and explicitness (Ridgeway & Zemel 2018) of the model's encoder means over `dataloader` (the
+        dataset in index order: DataLoader(shuffle=False) or DeviceLoader.in_order) -> {"modularity_score",
+        "explicitness_score_train", "explicitness_score_test"}; see `modularity_explicitness` for the definition and
+        the order of the draws.  The Evaluator's __call__, training and sweeps do not write this score; score a sweep's
+        members with `Evaluator(member.model, ...).compute_modularity_explicitness(sweep.loader.in_order(1000),
+        seed=...)`."""
+        return self._score(check_modularity_explicitness, modularity_explicitness, dataloader, seed,
+                           num_train=num_train, num_test=num_test)
 
     def _score(self, check, compute, dataloader, seed, **settings):
         """`compute(encoder means, lat_sizes, seed=seed, **settings)`'s score, after `check(dataset, latent_dim,

@@ -480,6 +480,69 @@ int dv_dci_fit(const float* mu, int ld, int row_stride, int N, int D, const long
                int* tree_feature, double* tree_threshold, double* tree_value, void* workspace,
                size_t workspace_bytes, void* stream);
 
+/* ---- disentanglement metrics: modularity and explicitness (Ridgeway & Zemel 2018; modularity_explicitness.py) ---
+ * Inputs of both entry points: mu is read as dv_group_variance reads it (element (n, d) at n*row_stride + d*ld; q_zCx in
+ * place), finite values assumed.  train_rows int64 [num_train] and test_rows int64 [num_test], every entry in [0, N);
+ * train_cls int32 [K][num_train] (classes 0 .. nc-1, every class present), test_cls int32 [K][num_test] (-1 for a value
+ * no training row has) and n_classes int32 [K] (nc, clamped to [0, class_stride]), as dv_sap_score_matrix takes them
+ * from the same labelling.  Rows and labels are not checked: the caller builds them.
+ *
+ * dv_discrete_mutual_info: for every latent d, np.digitize(x, np.histogram(x, 20)[1][:-1]) of its fp32 training
+ * column x, and sklearn's mutual_info_score(train_cls[k], bins) with every factor k.
+ *   edges: lo, hi = min, max of x (lo - 0.5, hi + 0.5 in fp32 when equal); step = (hi - lo) / 20 in fp32;
+ *          edge_j = j * step + lo in fp32 without contraction (j < 20), edge_20 = hi (numpy's linspace of a float32
+ *          column).  A row's bin is the number of edge_0 .. edge_19 at or below it.  Where numpy refuses the range
+ *          ("Too many bins for data range": edges not strictly increasing, at ranges of a few ulps) the same rule bins
+ *          the column.
+ *   mi    fp64 [D][K]: sum over the non-zero cells (c rows of class a_tot, bin b_tot) of sklearn's terms
+ *         c/n (log c - log n) + c/n (-log(a_tot b_tot) + log n + log n), each rounded without contraction and set to 0
+ *         when below DBL_EPSILON in magnitude, the bins of a class in order and then the classes in order; clipped at
+ *         0; 0 when the latent occupies one bin or nc <= 1.  Natural log.
+ *   edges fp32 [D][21] (optional, NULL for none).
+ * One launch of D CTAs, contingency counts in integer shared memory, no workspace; deterministic, graph-capturable.
+ * DV_ERR_BAD_SHAPE: N < 1, D < 1, D > 1024, num_train < 1, num_train > 32768, K < 1, class_stride < 1,
+ * class_stride > 256, ld < 1, row_stride < 1, or K*num_train > INT_MAX.
+ * DV_ERR_BAD_ARG: a required pointer NULL (all but edges), or a pointer misaligned (rows and mi 8 bytes, the others 4).
+ *
+ * dv_explicitness_fit: for every factor k, LogisticRegression(C=1) on the standardised latents and the ROC AUC of every
+ * class column of its probabilities, on the training rows and on the test rows.
+ *   standardisation: mean_d and std_d (ddof 0) of latent d over the training rows in fp64 from the fp32 values,
+ *          fixed-order sums; std_d = 0 becomes 1 (StandardScaler's rule); features (x - mean) / std in fp64.
+ *   fit:   dv_logistic_fit's solver and conventions on factor k's training labels (multinomial for nc > 2, binary for
+ *          nc = 2, none for nc <= 1).
+ *   probabilities: nc > 2: p_c = exp(z_c - max z) / sum_s exp(z_s - max z), the sum in class order; nc = 2:
+ *          p_1 = 1 / (1 + exp(-z)), p_0 = 1 - p_1 (sklearn's predict_proba); z = W x + b.
+ *   AUC of column c on a set: positives the set's rows of class c, negatives every other row of the set (test rows of
+ *          class -1 included): (2 #{p_pos > p_neg} + #{p_pos = p_neg}) / (2 n_pos n_neg), pair counts exact in int64 and
+ *          one fp64 division; NaN without positives or negatives, beyond the factor's columns (nc for nc > 2, 2 for
+ *          nc = 2) and for nc <= 1.
+ * Outputs:
+ *   coef  fp64 [K][class_stride][D + 1]: row r = (W_r, b_r) in standardised features (as dv_logistic_fit's coef, one
+ *         row for nc = 2), NaN beyond the factor's model rows
+ *   auc   fp64 [2][K][class_stride]: the training set, then the test set
+ *   iters int32 [K]: Newton steps, -1 if 100 did not converge; 0 for nc <= 1
+ *   mean, std fp64 [D]
+ *   proba fp64 [K][class_stride][num_train + num_test] (optional, NULL for none): p of column c on the training rows,
+ *         then the test rows; NaN beyond the factor's columns
+ * workspace: dv_explicitness_workspace_bytes(D, num_train, num_test, K, class_stride) bytes, 8-byte aligned, contents
+ * irrelevant.  Three launches (standardise: D CTAs; fit: K CTAs, one fit each; AUC: 2 K class_stride CTAs), no host
+ * synchronisation, graph-capturable.  Deterministic (fixed-order reductions, no floating-point atomics).
+ * DV_ERR_BAD_SHAPE: N < 1, D < 1, D > 128, num_train < 1, num_train > 32768, num_test < 1, K < 1, class_stride < 1,
+ * class_stride > 256, ld < 1, row_stride < 1, or num_train + num_test, K*(num_train + num_test) or 2 K class_stride
+ * above INT_MAX.
+ * DV_ERR_BAD_ARG: a required pointer NULL (all but proba), or a pointer misaligned (rows, coef, auc, mean, std, proba
+ * and workspace 8 bytes, the others 4).
+ * DV_ERR_WORKSPACE: workspace NULL or smaller than the query. */
+int dv_discrete_mutual_info(const float* mu, int ld, int row_stride, int N, int D, const long long* train_rows,
+                            int num_train, const int* train_cls, const int* n_classes, int K, int class_stride,
+                            double* mi, float* edges, void* stream);
+size_t dv_explicitness_workspace_bytes(int D, int num_train, int num_test, int K, int class_stride);  /* 0: unsupported */
+int dv_explicitness_fit(const float* mu, int ld, int row_stride, int N, int D, const long long* train_rows,
+                        int num_train, const long long* test_rows, int num_test, const int* train_cls,
+                        const int* test_cls, const int* n_classes, int K, int class_stride, double* coef,
+                        double* auc, int* iters, double* mean, double* std, double* proba, void* workspace,
+                        size_t workspace_bytes, void* stream);
+
 /* ---- FactorVAE pieces ---------------------------------------------------------------------
  * dv_permute_dims replaces _permute_dims (losses.py:483-508): out[b][d] = z[perm[d][b]][d].
  * perms != NULL: int64 [D][B] (the reference's CPU randperm stream, trap T7).  perms == NULL:

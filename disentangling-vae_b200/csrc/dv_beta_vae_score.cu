@@ -76,8 +76,6 @@ logistic_fit_kernel(const double* __restrict__ x, int D, int num_train, int num_
   }
 }
 
-bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
-
 bool fit_shape_ok(int num_train, int D, int K) {
   return num_train >= 1 && D >= 1 && D <= kFitMaxD && K >= 1 && K <= kFitMaxClasses;
 }

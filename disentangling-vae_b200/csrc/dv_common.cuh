@@ -38,6 +38,23 @@ inline int set_max_dynamic_smem(Kernel kernel, int bytes, bool* done) {
   return DV_OK;
 }
 
+// True when p is not a multiple of `a` bytes (a power of two).  NULL passes: optional operands are checked for
+// presence elsewhere.
+inline bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
+
+// A workspace cut into consecutive segments of sizes[s] bytes, each starting on a 256-byte boundary: the offsets into
+// off[] -> the total bytes.
+inline size_t align_up(size_t b) { return (b + 255) & ~size_t(255); }
+template <int kSegs>
+inline size_t carve_workspace(const size_t (&sizes)[kSegs], size_t (&off)[kSegs]) {
+  size_t total = 0;
+  for (int s = 0; s < kSegs; ++s) {
+    off[s] = total;
+    total += align_up(sizes[s]);
+  }
+  return total;
+}
+
 // First 1024-byte aligned address at or after p (TMA destinations with the 128-byte swizzle need it).
 __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
@@ -46,11 +63,30 @@ __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
 __device__ __forceinline__ float4 ldg4(const float* p) {
   return __ldg(reinterpret_cast<const float4*>(p));
 }
-__device__ __forceinline__ float warp_sum(float v) {
+
+// The fixed-order sums behind the "bit-identical run to run" results: over a warp by the butterfly (xor 16, 8, 4, 2,
+// 1), over a block of kWarps warps by the warps' sums added in order 0 .. kWarps - 1 (red: kWarps shared slots).
+// Every thread ends with the same bits.
+template <typename T>
+__device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+template <int kWarps, typename T>
+__device__ T block_sum(T v, T* red) {
+  v = warp_sum(v);
+  __syncthreads();
+  if ((threadIdx.x & (kWarp - 1)) == 0) red[threadIdx.x / kWarp] = v;
+  __syncthreads();
+  T s = 0;
+  for (int w = 0; w < kWarps; ++w) s += red[w];
+  return s;
+}
+
+// The classes of scored factor k: n_classes[k] clamped to [0, S].
+__device__ __forceinline__ int class_count(const int* n_classes, int k, int S) { return min(max(n_classes[k], 0), S); }
+
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));

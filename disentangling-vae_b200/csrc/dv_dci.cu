@@ -61,18 +61,13 @@ struct DciWs {
   double* cnt;      // [K][S] trees of more than one node
 };
 
-size_t align_up(size_t b) { return (b + 255) & ~size_t(255); }
-
 // Offsets of the workspace segments from `base` (NULL for the size only) -> total bytes.
 size_t dci_layout(int D, int n, int m, int K, int S, char* base, DciWs* w) {
   const size_t KS = (size_t)K * S;
   const size_t sizes[9] = {(size_t)D * n * 4, (size_t)D * m * 4, (size_t)D * n * 4, (size_t)D * n * 4,
                            KS * ((size_t)n + m) * 8, KS * n * 8, KS * n * 8, KS * D * 8, KS * 8};
-  size_t off[9], total = 0;
-  for (int s = 0; s < 9; ++s) {
-    off[s] = total;
-    total += align_up(sizes[s]);
-  }
+  size_t off[9];
+  const size_t total = carve_workspace(sizes, off);
   if (w) {
     w->xt = reinterpret_cast<float*>(base + off[0]);
     w->xe = reinterpret_cast<float*>(base + off[1]);
@@ -93,9 +88,6 @@ int pow2_at_least(int n) {
   return p;
 }
 
-__device__ __forceinline__ int dci_classes(const int* n_classes, int k, int S) {
-  return min(max(n_classes[k], 0), S);
-}
 __device__ __forceinline__ int dci_columns(int nc) { return nc > 2 ? nc : (nc == 2 ? 1 : 0); }
 
 __device__ __forceinline__ unsigned order_key(float v) {
@@ -161,7 +153,7 @@ dci_init_kernel(const int* __restrict__ n_classes, const int* __restrict__ count
   const long long ks = (long long)k * S + c;
   for (int d = t; d < D; d += kDciThreads) w.acc[ks * D + d] = 0.0;
   if (t == 0) w.cnt[ks] = 0.0;
-  const int nc = dci_classes(n_classes, k, S);
+  const int nc = class_count(n_classes, k, S);
   if (c >= dci_columns(nc)) return;
   double v;
   if (nc == 2) {
@@ -182,7 +174,7 @@ dci_residual_kernel(const int* __restrict__ train_cls, const int* __restrict__ n
   const long long g = (long long)blockIdx.x * kDciThreads + threadIdx.x;
   if (g >= (long long)K * n) return;
   const int k = (int)(g / n), i = (int)(g % n);
-  const int nc = dci_classes(n_classes, k, S);
+  const int nc = class_count(n_classes, k, S);
   if (nc < 2) return;
   const int y = train_cls[g];
   const long long N2 = (long long)n + m;
@@ -206,17 +198,6 @@ dci_residual_kernel(const int* __restrict__ train_cls, const int* __restrict__ n
     r[(long long)c * n] = v;
     q[(long long)c * n] = __double2ll_rn(v * kDciFix);
   }
-}
-
-__device__ __forceinline__ double warp_sum_dd(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ long long warp_sum_ll(long long v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
 }
 
 struct DciTreeArgs {
@@ -248,7 +229,7 @@ dci_tree_kernel(DciTreeArgs a, DciWs w) {
   const int n = a.n, m = a.m, D = a.D;
   const long long ks = (long long)k * a.S + c;
   const long long tree0 = (ks * a.stages + a.stage) * kDciNodes;
-  const int nc = dci_classes(a.n_classes, k, a.S);
+  const int nc = class_count(a.n_classes, k, a.S);
   if (t < kDciNodes) {
     feat[t] = kDciAbsent;
     thr[t] = CUDART_NAN;
@@ -310,8 +291,8 @@ dci_tree_kernel(DciTreeArgs a, DciWs w) {
 #pragma unroll
         for (int s = 0; s < kDciSplitMax; ++s) {
 #pragma unroll
-          for (int u = 0; u < 3; ++u) acc[s][u] = warp_sum_dd(acc[s][u]);
-          accq[s] = warp_sum_ll(accq[s]);
+          for (int u = 0; u < 3; ++u) acc[s][u] = warp_sum(acc[s][u]);
+          accq[s] = warp_sum(accq[s]);
         }
         if (lane == 0) {
 #pragma unroll
@@ -564,7 +545,7 @@ dci_importance_kernel(const int* __restrict__ n_classes, int K, int S, int D, Dc
   __shared__ double mean[kDciMaxD];
   __shared__ double norm;
   const int t = threadIdx.x, k = blockIdx.x;
-  const int cols = dci_columns(dci_classes(n_classes, k, S));
+  const int cols = dci_columns(class_count(n_classes, k, S));
   double trees = 0.0;
   for (int c = 0; c < cols; ++c) trees += w.cnt[(long long)k * S + c];
   for (int d = t; d < D; d += kDciThreads) {
@@ -589,7 +570,7 @@ dci_predict_kernel(const int* __restrict__ n_classes, int K, int S, int n, int m
   if (g >= (long long)K * N2) return;
   const int k = (int)(g / N2);
   const long long i = g % N2;
-  const int nc = dci_classes(n_classes, k, S);
+  const int nc = class_count(n_classes, k, S);
   const double* raw = w.raw + (long long)k * S * N2 + i;
   int best = 0;
   if (nc == 2) {
@@ -603,8 +584,6 @@ dci_predict_kernel(const int* __restrict__ n_classes, int K, int S, int n, int m
   }
   pred[g] = best;
 }
-
-bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
 
 bool dci_shape_ok(int D, int n, int m, int K, int S) {
   return D >= 1 && D <= kDciMaxD && n >= 1 && n <= kDciMaxTrain && m >= 1 && K >= 1 && S >= 1 &&

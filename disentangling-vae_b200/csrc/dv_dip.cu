@@ -265,8 +265,6 @@ dip_bwd_kernel(const float* __restrict__ mu, const float* __restrict__ logvar, i
   }
 }
 
-bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
-
 bool bad_dims(int B, int D) { return B < 1 || B > kDipMaxB || D < 1 || D > 1024; }
 
 int dip_check(const float* mu, const float* logvar, int ld, int rs, int B, int D, int dip_type, const void* ws) {

@@ -226,7 +226,7 @@ int dv_permute_dims_rows(const float* z, const long long* perms, unsigned long l
                                                                              row0, nrows);
     rc = check_launch();
   } else {
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 7)) return DV_ERR_BAD_ARG;
+    if (!workspace || misaligned(workspace, 8)) return DV_ERR_BAD_ARG;
     unsigned long long* buf[2] = {static_cast<unsigned long long*>(workspace),
                                   static_cast<unsigned long long*>(workspace) + (size_t)B * D};
     const int dims = std::min(D, 65535);
@@ -254,10 +254,10 @@ size_t dv_index_permutation_workspace_bytes(int N) {
 int dv_index_permutation(int N, unsigned long long seed, unsigned long long* offset_dev, long long* out_idx,
                          void* workspace, void* stream) {
   if (N < 1) return DV_ERR_BAD_SHAPE;
-  if (!offset_dev || !out_idx || (reinterpret_cast<uintptr_t>(out_idx) & 7)) return DV_ERR_BAD_ARG;
+  if (!offset_dev || !out_idx || misaligned(out_idx, 8)) return DV_ERR_BAD_ARG;
   int passes = 0;
   for (long long w = kPermMaxB; w < N; w *= 2) ++passes;
-  if (passes > 0 && (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 7))) return DV_ERR_BAD_ARG;
+  if (passes > 0 && (!workspace || misaligned(workspace, 8))) return DV_ERR_BAD_ARG;
   // The key buffers ping-pong between out_idx (N x 8 bytes, like the keys) and the workspace; the tile pass writes to
   // the one that makes the last merge pass land in out_idx, where the index column is then extracted in place.
   unsigned long long* out_keys = reinterpret_cast<unsigned long long*>(out_idx);

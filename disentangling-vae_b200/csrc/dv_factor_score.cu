@@ -123,8 +123,6 @@ fs_group_var_kernel(const float* __restrict__ mu, int ld, int rs, int D, const l
   }
 }
 
-bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
-
 }  // namespace
 }  // namespace dv
 

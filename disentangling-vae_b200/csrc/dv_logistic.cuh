@@ -36,27 +36,13 @@ struct Fit {
   double* red;          // shared: kFitWarps
 };
 
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 __device__ __forceinline__ double warp_max_d(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
 
-// Sum (or max) over the block; every thread gets the same bits.
-__device__ double block_sum(double v, double* red) {
-  v = warp_sum_d(v);
-  __syncthreads();
-  if ((threadIdx.x & (kWarp - 1)) == 0) red[threadIdx.x / kWarp] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < kFitWarps; ++w) s += red[w];
-  return s;
-}
+// Max over the block; every thread gets the same bits.
 __device__ double block_max(double v, double* red) {
   v = warp_max_d(v);
   __syncthreads();
@@ -70,7 +56,7 @@ __device__ double block_max(double v, double* red) {
 __device__ double dot(const Fit& F, const double* a, const double* b) {
   double s = 0.0;
   for (int o = threadIdx.x; o < F.O; o += kFitThreads) s = fma(a[o], b[o], s);
-  return block_sum(s, F.red);
+  return block_sum<kFitWarps>(s, F.red);
 }
 
 __device__ __forceinline__ double xc(const Fit& F, int i, int d) {
@@ -168,7 +154,7 @@ __device__ double objective(const Fit& F, const double* V) {
   double reg = 0.0;
   for (int o = threadIdx.x; o < F.O; o += kFitThreads)
     if (o % F.Dp != F.D) reg = fma(V[o], V[o], reg);
-  return 0.5 * block_sum(reg, F.red) + block_sum(acc, F.red);
+  return 0.5 * block_sum<kFitWarps>(reg, F.red) + block_sum<kFitWarps>(acc, F.red);
 }
 
 // grad and scale at theta, from the Q of the last `objective(theta)`.

@@ -37,8 +37,6 @@ constexpr int kAucThreads = 512;
 constexpr int kAucWarps = kAucThreads / kWarp;
 constexpr int kAucTile = 4096;                // positives sorted in shared memory at a time
 
-__device__ __forceinline__ int mod_classes(const int* n_classes, int k, int S) { return min(max(n_classes[k], 0), S); }
-
 // ---- mutual information --------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kMiThreads)
 discrete_mi_kernel(const float* __restrict__ mu, int ld, int rs, const long long* __restrict__ train_rows, int n,
@@ -108,7 +106,7 @@ discrete_mi_kernel(const float* __restrict__ mu, int ld, int rs, const long long
   }
   const double dn = (double)n, ln = log(dn);
   for (int k = 0; k < K; ++k) {
-    const int nc = mod_classes(n_classes, k, S);
+    const int nc = class_count(n_classes, k, S);
     for (int j = t; j < nc * kMiBins; j += kMiThreads) cnt[j] = 0;
     __syncthreads();
     const int* cls = train_cls + (long long)k * n;
@@ -152,18 +150,13 @@ struct ModWs {
   size_t fit_stride;
 };
 
-size_t align_up(size_t b) { return (b + 255) & ~size_t(255); }
-
 // Offsets of the workspace segments from `base` (NULL for the size only) -> total bytes.
 size_t mod_layout(int D, int n, int m, int K, int S, char* base, ModWs* w) {
   const size_t rows = (size_t)n + m;
   const size_t fit_bytes = align_up(fit_workspace_doubles(n, D, S) * sizeof(double));
   const size_t sizes[3] = {rows * D * 8, (size_t)K * fit_bytes, (size_t)K * S * rows * 8};
-  size_t off[3], total = 0;
-  for (int s = 0; s < 3; ++s) {
-    off[s] = total;
-    total += align_up(sizes[s]);
-  }
+  size_t off[3];
+  const size_t total = carve_workspace(sizes, off);
   if (w) {
     w->feat = reinterpret_cast<double*>(base + off[0]);
     w->fit = reinterpret_cast<double*>(base + off[1]);
@@ -171,19 +164,6 @@ size_t mod_layout(int D, int n, int m, int K, int S, char* base, ModWs* w) {
     w->fit_stride = fit_bytes / sizeof(double);
   }
   return total;
-}
-
-// Sum over the block in a fixed order (lanes by the butterfly, then the warps in order); every thread gets the bits.
-template <int kWarps>
-__device__ double block_sum_fixed(double v, double* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & (kWarp - 1)) == 0) red[threadIdx.x / kWarp] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < kWarps; ++w) s += red[w];
-  return s;
 }
 
 __global__ void __launch_bounds__(kStdThreads)
@@ -195,13 +175,13 @@ standardise_kernel(const float* __restrict__ mu, int ld, int rs, int D, const lo
   const long long col = (long long)d * ld;
   double s = 0.0;
   for (int i = t; i < n; i += kStdThreads) s += (double)mu[train_rows[i] * (long long)rs + col];
-  const double mean = block_sum_fixed<kStdWarps>(s, red) / n;
+  const double mean = block_sum<kStdWarps>(s, red) / n;
   s = 0.0;
   for (int i = t; i < n; i += kStdThreads) {
     const double e = __dsub_rn((double)mu[train_rows[i] * (long long)rs + col], mean);
     s = __dadd_rn(s, __dmul_rn(e, e));
   }
-  double sd = sqrt(block_sum_fixed<kStdWarps>(s, red) / n);
+  double sd = sqrt(block_sum<kStdWarps>(s, red) / n);
   if (sd == 0.0) sd = 1.0;                                     // StandardScaler's rule for a constant feature
   if (t == 0) {
     mean_out[d] = mean;
@@ -218,7 +198,7 @@ explicitness_fit_kernel(int D, int n, int m, const int* __restrict__ train_cls, 
                         int S, double* __restrict__ coef, int* __restrict__ iters, double* __restrict__ proba,
                         ModWs w) {
   const int t = threadIdx.x, k = blockIdx.x;
-  const int nc = mod_classes(n_classes, k, S);
+  const int nc = class_count(n_classes, k, S);
   const int Dp = D + 1;
   const long long rows = (long long)n + m;
   double* ck = coef + (long long)k * S * Dp;
@@ -260,18 +240,6 @@ __device__ __forceinline__ unsigned long long prob_key(double v) {
   return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
 }
 
-__device__ long long block_sum_ll(long long v, long long* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & (kWarp - 1)) == 0) red[threadIdx.x / kWarp] = v;
-  __syncthreads();
-  long long s = 0;
-  for (int w = 0; w < kAucWarps; ++w) s += red[w];
-  __syncthreads();
-  return s;
-}
-
 __global__ void __launch_bounds__(kAucThreads)
 auc_kernel(int n, int m, int K, const int* __restrict__ train_cls, const int* __restrict__ test_cls,
            const int* __restrict__ n_classes, int S, const double* __restrict__ proba, double* __restrict__ auc,
@@ -281,7 +249,7 @@ auc_kernel(int n, int m, int K, const int* __restrict__ train_cls, const int* __
   __shared__ int wcount[kAucWarps];
   const int t = threadIdx.x, lane = t & (kWarp - 1), warp = t / kWarp;
   const int set = blockIdx.x & 1, c = (blockIdx.x >> 1) % S, k = (blockIdx.x >> 1) / S;
-  const int nc = mod_classes(n_classes, k, S);
+  const int nc = class_count(n_classes, k, S);
   const int cols = nc > 2 ? nc : (nc == 2 ? 2 : 0);
   double* out = auc + ((long long)set * K + k) * S + c;
   if (c >= cols) {
@@ -295,7 +263,8 @@ auc_kernel(int n, int m, int K, const int* __restrict__ train_cls, const int* __
 
   long long np_ = 0;
   for (int i = t; i < len; i += kAucThreads) np_ += lab[i] == c ? 1 : 0;
-  const long long n_pos = block_sum_ll(np_, red), n_neg = (long long)len - n_pos;
+  const long long n_pos = block_sum<kAucWarps>(np_, red), n_neg = (long long)len - n_pos;
+  __syncthreads();
   if (n_pos == 0 || n_neg == 0) {
     if (t == 0) *out = CUDART_NAN;
     return;
@@ -360,12 +329,12 @@ auc_kernel(int n, int m, int K, const int* __restrict__ train_cls, const int* __
     }
     __syncthreads();
   }
-  gt = block_sum_ll(gt, red);
-  eq = block_sum_ll(eq, red);
+  gt = block_sum<kAucWarps>(gt, red);
+  __syncthreads();
+  eq = block_sum<kAucWarps>(eq, red);
+  __syncthreads();
   if (t == 0) *out = (double)(2 * gt + eq) / (2.0 * (double)n_pos * (double)n_neg);
 }
-
-bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
 
 bool mod_shape_ok(int D, int n, int m, int K, int S) {
   return D >= 1 && D <= kModMaxD && n >= 1 && n <= kModMaxTrain && m >= 1 && K >= 1 && S >= 1 &&

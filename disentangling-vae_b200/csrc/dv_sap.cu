@@ -40,12 +40,6 @@ constexpr int kSapFixedSmem = kSapMaxClasses * 8 + kSapMaxClasses * 16 + kSapWar
 
 size_t sap_smem_bytes(int num_train) { return (size_t)kSapFixedSmem + (size_t)num_train * 5; }
 
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 struct SapEval {
   double f, gw, gb, hww, hwb, hbb, scale;
 };
@@ -73,13 +67,13 @@ __device__ __forceinline__ SapEval sap_eval(const float* x, const uint8_t* lab, 
     }
   }
   SapEval e;
-  e.f = 0.5 * (w * w + b * b) + warp_sum_d(f);
-  e.gw = w - 2.0 * warp_sum_d(gx);
-  e.gb = b - 2.0 * warp_sum_d(g1);
-  e.hww = 1.0 + 2.0 * warp_sum_d(hxx);
-  e.hwb = 2.0 * warp_sum_d(hx);
-  e.hbb = 1.0 + 2.0 * warp_sum_d(h1);
-  e.scale = fabs(w) + fabs(b) + 2.0 * warp_sum_d(sc);
+  e.f = 0.5 * (w * w + b * b) + warp_sum(f);
+  e.gw = w - 2.0 * warp_sum(gx);
+  e.gb = b - 2.0 * warp_sum(g1);
+  e.hww = 1.0 + 2.0 * warp_sum(hxx);
+  e.hwb = 2.0 * warp_sum(hx);
+  e.hbb = 1.0 + 2.0 * warp_sum(h1);
+  e.scale = fabs(w) + fabs(b) + 2.0 * warp_sum(sc);
   return e;
 }
 
@@ -137,7 +131,7 @@ sap_kernel(const float* __restrict__ mu, int ld, int rs, int D, const long long*
   uint8_t* lab = reinterpret_cast<uint8_t*>(x + n_train);
   const int t = threadIdx.x, lane = t & (kWarp - 1), warp = t / kWarp;
   const int cell = blockIdx.x, d = cell / K, k = cell % K;
-  const int nc = min(max(n_classes[k], 0), cs);
+  const int nc = class_count(n_classes, k, cs);
   const long long col = (long long)d * ld;
 
   for (int i = t; i < n_train; i += kSapThreads) {
@@ -185,8 +179,7 @@ sap_kernel(const float* __restrict__ mu, int ld, int rs, int D, const long long*
     }
     correct += pred == test_cls[(long long)k * n_test + j];
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) correct += __shfl_xor_sync(0xffffffffu, correct, o);
+  correct = warp_sum(correct);
   if (lane == 0) wcount[warp] = correct;
   __syncthreads();
   if (t == 0) {
@@ -195,8 +188,6 @@ sap_kernel(const float* __restrict__ mu, int ld, int rs, int D, const long long*
     score[cell] = (float)((double)total / (double)n_test);
   }
 }
-
-bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
 
 }  // namespace
 }  // namespace dv

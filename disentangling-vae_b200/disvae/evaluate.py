@@ -163,6 +163,31 @@ def _full_grid(label, lat_sizes, n):
     return lat_sizes
 
 
+# ---- what every wrapper of a score kernel checks and passes -------------------------------------------------------
+def _mu_args(mu):
+    """`mu` [N, D] (CUDA fp32, any strides, a view of q_zCx included) as the score kernels take it: (ptr, ld,
+    row_stride, N, D), with latent d of row i at ptr[i * row_stride + d * ld]."""
+    N.require_cuda_f32(mu)
+    n, d = mu.shape
+    return N.ptr(mu), mu.stride(1), mu.stride(0), n, d
+
+
+def _require_operands(fn, optional=False, **operands):
+    """ValueError `{fn}: {name} must be a contiguous CUDA {dtype} tensor[ of shape {shape}]` unless every operand
+    name=(tensor, dtype[, shape]) is one; with `optional`, a None tensor passes."""
+    for name, (t, dtype, *shape) in operands.items():
+        if t is None and optional:
+            continue
+        if t.dtype != dtype or not t.is_contiguous() or not t.is_cuda or (shape and tuple(t.shape) != shape[0]):
+            raise ValueError("%s: %s must be a contiguous CUDA %s tensor%s"
+                             % (fn, name, dtype, " of shape %s" % (shape[0],) if shape else ""))
+
+
+def _f64_workspace(nbytes, device):
+    """A kernel workspace of at least `nbytes` bytes (8-byte aligned, never empty)."""
+    return torch.empty(max(nbytes, 8) // 8, dtype=torch.float64, device=device)
+
+
 # ---- FactorVAE score (Kim & Mnih 2018, section 4; the conventions of disentanglement_lib's factor_vae.py) ----------
 def check_factor_score(dataset, latent_dim, batch_size=64, num_train=10000, num_eval=5000,
                        num_variance_estimate=10000):
@@ -213,18 +238,15 @@ def group_variance(mu, rows, global_var=None, var_out=None, argmin_out=None):
     """`dv_group_variance` on `mu` [N, D] (any strides, a view of q_zCx included) and int64 `rows` [V, L]: the
     unbiased variance of every group into `var_out` [V, D], and / or into int32 `argmin_out` [V] the dim minimising
     var / global_var over the dims with global_var >= FACTOR_SCORE_MIN_VAR."""
-    N.require_cuda_f32(mu)
-    n, d = mu.shape
+    mu_args, d = _mu_args(mu), mu.shape[1]
     V, L = rows.shape
     if rows.dtype != torch.int64 or not rows.is_contiguous():
         raise ValueError("group_variance: rows must be a contiguous int64 tensor")
-    for name, t, dtype, shape in (("var_out", var_out, torch.float32, (V, d)),
-                                  ("argmin_out", argmin_out, torch.int32, (V,)),
-                                  ("global_var", global_var, torch.float32, (d,))):
-        if t is not None and (t.dtype != dtype or not t.is_contiguous() or not t.is_cuda or tuple(t.shape) != shape):
-            raise ValueError("group_variance: %s must be a contiguous CUDA %s tensor of shape %s" % (name, dtype, shape))
-    N.call("dv_group_variance", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(rows), V, L, N.ptr(global_var),
-           FACTOR_SCORE_MIN_VAR, N.ptr(var_out), N.ptr(argmin_out), N.stream())
+    _require_operands("group_variance", var_out=(var_out, torch.float32, (V, d)),
+                      argmin_out=(argmin_out, torch.int32, (V,)), global_var=(global_var, torch.float32, (d,)),
+                      optional=True)
+    N.call("dv_group_variance", *mu_args, N.ptr(rows), V, L, N.ptr(global_var), FACTOR_SCORE_MIN_VAR, N.ptr(var_out),
+           N.ptr(argmin_out), N.stream())
 
 
 def factor_vae_score(mu, lat_sizes, batch_size=64, num_train=10000, num_eval=5000, num_variance_estimate=10000,
@@ -337,23 +359,39 @@ def sap_labels(lat_sizes, train_rows, test_rows):
             torch.stack(counts).int(), present)
 
 
+def _sap_draws(mu, lat_sizes, num_train, num_test, seed):
+    """The rows of the SAP, DCI, modularity and explicitness scores of `mu` [N, D] (CUDA fp32) -> (train_rows,
+    test_rows) + `sap_labels`' tuple.  They come from a device torch.Generator seeded with `seed`: `torch.randint(N,
+    (num_train,))`, then `torch.randint(N, (num_test,))`; the global generators are not touched."""
+    N.require_cuda_f32(mu)
+    gen = torch.Generator(device=mu.device)
+    gen.manual_seed(int(seed))
+    train_rows = torch.randint(mu.shape[0], (int(num_train),), generator=gen, device=mu.device)
+    test_rows = torch.randint(mu.shape[0], (int(num_test),), generator=gen, device=mu.device)
+    return (train_rows, test_rows) + sap_labels(lat_sizes, train_rows, test_rows)
+
+
+def _classes_table(present):
+    """`sap_labels`' `present` [K', S] (host) as the helpers' "classes" int64 [K', S]: the values seen, -1 beyond."""
+    K, S = present.shape
+    classes = torch.sort(torch.where(present, torch.arange(S).expand(K, S), S), dim=1)[0]   # the values seen, then S
+    return torch.where(classes < S, classes, -1)
+
+
 def sap_score_matrix(mu, train_rows, test_rows, train_cls, test_cls, n_classes, counts, C, coef=None, iters=None):
     """`dv_sap_score_matrix` on `mu` [N, D] (any strides, a view of q_zCx included) -> the fp32 score [D, K'] of
     `sap_labels`' classes; optionally the fitted lines into fp64 `coef` [D, K', S, 2] and the Newton steps into int32
     `iters` [D, K', S]."""
-    N.require_cuda_f32(mu)
-    n, d = mu.shape
+    mu_args, d = _mu_args(mu), mu.shape[1]
     K, S = counts.shape
-    for name, t, dtype in (("train_rows", train_rows, torch.int64), ("test_rows", test_rows, torch.int64),
-                           ("train_cls", train_cls, torch.int32), ("test_cls", test_cls, torch.int32),
-                           ("n_classes", n_classes, torch.int32), ("counts", counts, torch.int32),
-                           ("coef", coef, torch.float64), ("iters", iters, torch.int32)):
-        if t is not None and (t.dtype != dtype or not t.is_contiguous() or not t.is_cuda):
-            raise ValueError("sap_score_matrix: %s must be a contiguous CUDA %s tensor" % (name, dtype))
+    _require_operands("sap_score_matrix", train_rows=(train_rows, torch.int64), test_rows=(test_rows, torch.int64),
+                      train_cls=(train_cls, torch.int32), test_cls=(test_cls, torch.int32),
+                      n_classes=(n_classes, torch.int32), counts=(counts, torch.int32), coef=(coef, torch.float64),
+                      iters=(iters, torch.int32), optional=True)
     score = torch.empty(d, K, dtype=torch.float32, device=mu.device)
-    N.call("dv_sap_score_matrix", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(train_rows), train_rows.numel(),
-           N.ptr(test_rows), test_rows.numel(), N.ptr(train_cls), N.ptr(test_cls), N.ptr(n_classes), N.ptr(counts), K,
-           S, float(C), N.ptr(score), N.ptr(coef), N.ptr(iters), N.stream())
+    N.call("dv_sap_score_matrix", *mu_args, N.ptr(train_rows), train_rows.numel(), N.ptr(test_rows), test_rows.numel(),
+           N.ptr(train_cls), N.ptr(test_cls), N.ptr(n_classes), N.ptr(counts), K, S, float(C), N.ptr(score),
+           N.ptr(coef), N.ptr(iters), N.stream())
     return score
 
 
@@ -366,22 +404,17 @@ def sap_from_matrix(score_matrix):
 
 def sap_score(mu, lat_sizes, num_train=10000, num_test=5000, C=0.01, seed=0):
     """SAP score of the encoder means `mu` [N, D] (CUDA fp32, dataset index order) of the full factor grid `lat_sizes`
-    -> ({"SAP"}, helpers).  The draws come from a device torch.Generator seeded with `seed`: `torch.randint(N,
-    (num_train,))` for the training rows, then `torch.randint(N, (num_test,))` for the test rows; the global generators
-    are not touched.  For every latent and scored factor `dv_sap_score_matrix` fits LinearSVC(C,
-    class_weight="balanced") exactly and scores it on the test rows; SAP is `sap_from_matrix` of that table.
+    -> ({"SAP"}, helpers).  The rows and their classes are `_sap_draws`' (seeded with `seed`).  For every latent and
+    scored factor `dv_sap_score_matrix` fits LinearSVC(C, class_weight="balanced") exactly and scores it on the test
+    rows; SAP is `sap_from_matrix` of that table.
     helpers: "score_matrix" fp32 [D, K'], "factors" (the scored factor indices, ascending), "classes" int64 [K', S]
     (each factor's training values, ascending, -1 beyond), "coef" fp64 [D, K', S, 2] (w, b of each problem: class c's
     one-vs-rest problem in slot c, the two-class problem in slot 0, NaN beyond) and "solver_iterations" int32
     [D, K', S] (Newton steps, -1 for a fit that did not converge, which also raises a RuntimeWarning)."""
     lat_sizes = _check_sap_grid(lat_sizes, mu.shape[0], mu.shape[1], num_train, num_test, C)
-    N.require_cuda_f32(mu)
-    n, D = mu.shape
-    gen = torch.Generator(device=mu.device)
-    gen.manual_seed(int(seed))
-    train_rows = torch.randint(n, (int(num_train),), generator=gen, device=mu.device)
-    test_rows = torch.randint(n, (int(num_test),), generator=gen, device=mu.device)
-    factors, train_cls, test_cls, n_classes, counts, present = sap_labels(lat_sizes, train_rows, test_rows)
+    D = mu.shape[1]
+    train_rows, test_rows, factors, train_cls, test_cls, n_classes, counts, present = _sap_draws(
+        mu, lat_sizes, num_train, num_test, seed)
     K, S = counts.shape
     coef = torch.empty(D, K, S, 2, dtype=torch.float64, device=mu.device)
     iters = torch.empty(D, K, S, dtype=torch.int32, device=mu.device)
@@ -391,10 +424,8 @@ def sap_score(mu, lat_sizes, num_train=10000, num_test=5000, C=0.01, seed=0):
     if failed:
         warnings.warn("SAP score: %d of the linear-SVM fits did not converge in the solver's step limit; see "
                       "helpers['solver_iterations'] (-1)" % failed, RuntimeWarning)
-    values = torch.arange(S).expand(K, S)
-    classes = torch.sort(torch.where(present, values, S), dim=1)[0]           # the values seen, ascending, then S
     helpers = {"score_matrix": matrix, "factors": torch.tensor(factors, dtype=torch.int64),
-               "classes": torch.where(classes < S, classes, -1), "coef": coef, "solver_iterations": iters}
+               "classes": _classes_table(present), "coef": coef, "solver_iterations": iters}
     return {"SAP": sap_from_matrix(matrix)}, helpers
 
 
@@ -451,15 +482,13 @@ def beta_vae_points(lat_sizes, count, batch_size, generator):
 def pair_abs_diff_mean(mu, rows_a, rows_b):
     """`dv_pair_abs_diff_mean` on `mu` [N, D] (any strides, a view of q_zCx included) and int64 `rows_a`, `rows_b`
     [V, L] -> fp64 x [V, D], x[v, d] = mean over l of |mu[rows_a[v, l], d] - mu[rows_b[v, l], d]|, added in order."""
-    N.require_cuda_f32(mu)
-    n, d = mu.shape
+    mu_args, d = _mu_args(mu), mu.shape[1]
     V, L = rows_a.shape
     for name, t in (("rows_a", rows_a), ("rows_b", rows_b)):
         if t.dtype != torch.int64 or not t.is_contiguous() or t.shape != (V, L):
             raise ValueError("pair_abs_diff_mean: %s must be a contiguous int64 tensor of shape %s" % (name, (V, L)))
     x = torch.empty(V, d, dtype=torch.float64, device=mu.device)
-    N.call("dv_pair_abs_diff_mean", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(rows_a), N.ptr(rows_b), V, L,
-           N.ptr(x), N.stream())
+    N.call("dv_pair_abs_diff_mean", *mu_args, N.ptr(rows_a), N.ptr(rows_b), V, L, N.ptr(x), N.stream())
     return x
 
 
@@ -468,13 +497,10 @@ def logistic_fit(x, labels, n_classes, K, num_train):
     `labels` [num_train] and the class count in int32 `n_classes` [1] on the device -> (coef fp64 [K, D + 1], pred
     int32 [V], iters int32 [1]); see include/disvae_b200.h for the objective and the layout of coef."""
     V, D = x.shape
-    for name, t, dtype in (("x", x, torch.float64), ("labels", labels, torch.int32),
-                           ("n_classes", n_classes, torch.int32)):
-        if t.dtype != dtype or not t.is_contiguous() or not t.is_cuda:
-            raise ValueError("logistic_fit: %s must be a contiguous CUDA %s tensor" % (name, dtype))
-    L = N.lib()
-    nbytes = L.dv_logistic_fit_workspace_bytes(int(num_train), D, int(K))
-    ws = torch.empty(max(nbytes, 8) // 8, dtype=torch.float64, device=x.device)
+    _require_operands("logistic_fit", x=(x, torch.float64), labels=(labels, torch.int32),
+                      n_classes=(n_classes, torch.int32))
+    nbytes = N.lib().dv_logistic_fit_workspace_bytes(int(num_train), D, int(K))
+    ws = _f64_workspace(nbytes, x.device)
     coef = torch.empty(int(K), D + 1, dtype=torch.float64, device=x.device)
     pred = torch.empty(V, dtype=torch.int32, device=x.device)
     iters = torch.empty(1, dtype=torch.int32, device=x.device)
@@ -564,17 +590,14 @@ def dci_fit(mu, train_rows, test_rows, train_cls, n_classes, counts, stages=DCI_
     """`dv_dci_fit` on `mu` [N, D] (any strides, a view of q_zCx included) and `sap_labels`' classes -> (importance
     fp64 [D, K'], pred int32 [K', num_train + num_test] (class indices), trees), trees = None or (feature int32,
     threshold fp64, value fp64), each [K', S, stages, 15]; see include/disvae_b200.h for the fit."""
-    N.require_cuda_f32(mu)
-    n, d = mu.shape
+    mu_args, d = _mu_args(mu), mu.shape[1]
     K, S = counts.shape
-    for name, t, dtype in (("train_rows", train_rows, torch.int64), ("test_rows", test_rows, torch.int64),
-                           ("train_cls", train_cls, torch.int32), ("n_classes", n_classes, torch.int32),
-                           ("counts", counts, torch.int32)):
-        if t.dtype != dtype or not t.is_contiguous() or not t.is_cuda:
-            raise ValueError("dci_fit: %s must be a contiguous CUDA %s tensor" % (name, dtype))
+    _require_operands("dci_fit", train_rows=(train_rows, torch.int64), test_rows=(test_rows, torch.int64),
+                      train_cls=(train_cls, torch.int32), n_classes=(n_classes, torch.int32),
+                      counts=(counts, torch.int32))
     num_train, num_test = train_rows.numel(), test_rows.numel()
     nbytes = N.lib().dv_dci_workspace_bytes(d, num_train, num_test, K, S)
-    ws = torch.empty(max(nbytes, 8) // 8, dtype=torch.float64, device=mu.device)
+    ws = _f64_workspace(nbytes, mu.device)
     importance = torch.empty(d, K, dtype=torch.float64, device=mu.device)
     pred = torch.empty(K, num_train + num_test, dtype=torch.int32, device=mu.device)
     out = None
@@ -583,9 +606,9 @@ def dci_fit(mu, train_rows, test_rows, train_cls, n_classes, counts, stages=DCI_
         out = (torch.empty(shape, dtype=torch.int32, device=mu.device),
                torch.empty(shape, dtype=torch.float64, device=mu.device),
                torch.empty(shape, dtype=torch.float64, device=mu.device))
-    N.call("dv_dci_fit", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(train_rows), num_train, N.ptr(test_rows),
-           num_test, N.ptr(train_cls), N.ptr(n_classes), N.ptr(counts), K, S, int(stages), N.ptr(importance),
-           N.ptr(pred), *(N.ptr(t) for t in (out or (None, None, None))), N.ptr(ws), nbytes, N.stream())
+    N.call("dv_dci_fit", *mu_args, N.ptr(train_rows), num_train, N.ptr(test_rows), num_test, N.ptr(train_cls),
+           N.ptr(n_classes), N.ptr(counts), K, S, int(stages), N.ptr(importance), N.ptr(pred),
+           *(N.ptr(t) for t in (out or (None, None, None))), N.ptr(ws), nbytes, N.stream())
     return importance, pred, out
 
 
@@ -609,34 +632,25 @@ def dci_from_importance(importance):
 
 def dci_score(mu, lat_sizes, num_train=10000, num_test=5000, seed=0):
     """DCI score of the encoder means `mu` [N, D] (CUDA fp32, dataset index order) of the full factor grid `lat_sizes`
-    -> ({"disentanglement", "completeness", "informativeness_train", "informativeness_test"}, helpers).  The draws
-    are SAP's: a device torch.Generator seeded with `seed`, `torch.randint(N, (num_train,))` for the training rows,
-    then `torch.randint(N, (num_test,))` for the test rows; the global generators are not touched.  For every scored
-    factor `dci_fit` grows GradientBoostingClassifier()'s 100 boosting stages on the training rows; a factor seen with
-    one value in training has no trees, zero importance and predicts that value.  The informativeness scores are the
-    mean accuracies over the factors (a test value unseen in training is never predicted right).
+    -> ({"disentanglement", "completeness", "informativeness_train", "informativeness_test"}, helpers).  The rows and
+    their classes are `_sap_draws`' (seeded with `seed`), as SAP's are.  For every scored factor `dci_fit` grows
+    GradientBoostingClassifier()'s 100 boosting stages on the training rows; a factor seen with one value in training
+    has no trees, zero importance and predicts that value.  The informativeness scores are the mean accuracies over the
+    factors (a test value unseen in training is never predicted right).
     helpers: "importance_matrix" fp64 [D, K'], "factors" (the scored factor indices, ascending), "classes" int64
     [K', S] (each factor's training values, ascending, -1 beyond), "train_accuracy" and "test_accuracy" fp64 [K']."""
     lat_sizes = _check_dci_grid(lat_sizes, mu.shape[0], mu.shape[1], num_train, num_test)
-    N.require_cuda_f32(mu)
-    n = mu.shape[0]
     num_train = int(num_train)
-    gen = torch.Generator(device=mu.device)
-    gen.manual_seed(int(seed))
-    train_rows = torch.randint(n, (num_train,), generator=gen, device=mu.device)
-    test_rows = torch.randint(n, (int(num_test),), generator=gen, device=mu.device)
-    factors, train_cls, test_cls, n_classes, counts, present = sap_labels(lat_sizes, train_rows, test_rows)
-    K, S = counts.shape
+    train_rows, test_rows, factors, train_cls, test_cls, n_classes, counts, present = _sap_draws(
+        mu, lat_sizes, num_train, num_test, seed)
     importance, pred, _ = dci_fit(mu, train_rows, test_rows, train_cls, n_classes, counts)
     right = pred == torch.cat([train_cls, test_cls], 1)
     train_acc = right[:, :num_train].double().mean(1).cpu()
     test_acc = right[:, num_train:].double().mean(1).cpu()
     importance, present = importance.cpu(), present.cpu()
     disentanglement, completeness = dci_from_importance(importance)
-    classes = torch.sort(torch.where(present, torch.arange(S).expand(K, S), S), dim=1)[0]
     helpers = {"importance_matrix": importance, "factors": torch.tensor(factors, dtype=torch.int64),
-               "classes": torch.where(classes < S, classes, -1), "train_accuracy": train_acc,
-               "test_accuracy": test_acc}
+               "classes": _classes_table(present), "train_accuracy": train_acc, "test_accuracy": test_acc}
     score = {"disentanglement": disentanglement, "completeness": completeness,
              "informativeness_train": float(train_acc.mean()), "informativeness_test": float(test_acc.mean())}
     return score, helpers
@@ -671,27 +685,18 @@ def _check_modularity_grid(lat_sizes, n, latent_dim, num_train, num_test):
     return lat_sizes
 
 
-def _require_labels(fn, tensors):
-    for name, t, dtype in tensors:
-        if t.dtype != dtype or not t.is_contiguous() or not t.is_cuda:
-            raise ValueError("%s: %s must be a contiguous CUDA %s tensor" % (fn, name, dtype))
-
-
 def discrete_mutual_info(mu, train_rows, train_cls, n_classes, class_stride):
     """`dv_discrete_mutual_info` on `mu` [N, D] (any strides, a view of q_zCx included) and `sap_labels`' training
     classes -> (mi fp64 [D, K'], edges fp32 [D, 21]): sklearn's mutual_info_score of every factor's classes with every
     latent's 20-bin histogram discretisation over the training rows; see include/disvae_b200.h for the rules."""
-    N.require_cuda_f32(mu)
-    n, d = mu.shape
-    _require_labels("discrete_mutual_info", (("train_rows", train_rows, torch.int64),
-                                             ("train_cls", train_cls, torch.int32),
-                                             ("n_classes", n_classes, torch.int32)))
+    mu_args, d = _mu_args(mu), mu.shape[1]
+    _require_operands("discrete_mutual_info", train_rows=(train_rows, torch.int64), train_cls=(train_cls, torch.int32),
+                      n_classes=(n_classes, torch.int32))
     K = n_classes.numel()
     mi = torch.empty(d, K, dtype=torch.float64, device=mu.device)
     edges = torch.empty(d, MODULARITY_BINS + 1, dtype=torch.float32, device=mu.device)
-    N.call("dv_discrete_mutual_info", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(train_rows),
-           train_rows.numel(), N.ptr(train_cls), N.ptr(n_classes), K, int(class_stride), N.ptr(mi), N.ptr(edges),
-           N.stream())
+    N.call("dv_discrete_mutual_info", *mu_args, N.ptr(train_rows), train_rows.numel(), N.ptr(train_cls),
+           N.ptr(n_classes), K, int(class_stride), N.ptr(mi), N.ptr(edges), N.stream())
     return mi, edges
 
 
@@ -700,23 +705,22 @@ def explicitness_fit(mu, train_rows, test_rows, train_cls, test_cls, n_classes, 
     fp64 [2, K', S] (training, test), iters int32 [K'], mean fp64 [D], std fp64 [D], proba): LogisticRegression(C=1)
     of every factor on the standardised latents and the ROC AUC of each class column; proba is None or fp64
     [K', S, num_train + num_test].  See include/disvae_b200.h for the rules."""
-    N.require_cuda_f32(mu)
-    n, d = mu.shape
-    _require_labels("explicitness_fit", (("train_rows", train_rows, torch.int64), ("test_rows", test_rows, torch.int64),
-                                         ("train_cls", train_cls, torch.int32), ("test_cls", test_cls, torch.int32),
-                                         ("n_classes", n_classes, torch.int32)))
+    mu_args, d = _mu_args(mu), mu.shape[1]
+    _require_operands("explicitness_fit", train_rows=(train_rows, torch.int64), test_rows=(test_rows, torch.int64),
+                      train_cls=(train_cls, torch.int32), test_cls=(test_cls, torch.int32),
+                      n_classes=(n_classes, torch.int32))
     K, S = n_classes.numel(), int(class_stride)
     num_train, num_test = train_rows.numel(), test_rows.numel()
     nbytes = N.lib().dv_explicitness_workspace_bytes(d, num_train, num_test, K, S)
-    ws = torch.empty(max(nbytes, 8) // 8, dtype=torch.float64, device=mu.device)
+    ws = _f64_workspace(nbytes, mu.device)
     f64 = dict(dtype=torch.float64, device=mu.device)
     coef, auc = torch.empty(K, S, d + 1, **f64), torch.empty(2, K, S, **f64)
     iters = torch.empty(K, dtype=torch.int32, device=mu.device)
     mean, std = torch.empty(d, **f64), torch.empty(d, **f64)
     out = torch.empty(K, S, num_train + num_test, **f64) if proba else None
-    N.call("dv_explicitness_fit", N.ptr(mu), mu.stride(1), mu.stride(0), n, d, N.ptr(train_rows), num_train,
-           N.ptr(test_rows), num_test, N.ptr(train_cls), N.ptr(test_cls), N.ptr(n_classes), K, S, N.ptr(coef),
-           N.ptr(auc), N.ptr(iters), N.ptr(mean), N.ptr(std), N.ptr(out), N.ptr(ws), nbytes, N.stream())
+    N.call("dv_explicitness_fit", *mu_args, N.ptr(train_rows), num_train, N.ptr(test_rows), num_test, N.ptr(train_cls),
+           N.ptr(test_cls), N.ptr(n_classes), K, S, N.ptr(coef), N.ptr(auc), N.ptr(iters), N.ptr(mean), N.ptr(std),
+           N.ptr(out), N.ptr(ws), nbytes, N.stream())
     return coef, auc, iters, mean, std, out
 
 
@@ -742,13 +746,12 @@ def _explicitness_of(auc):
 def modularity_explicitness(mu, lat_sizes, num_train=10000, num_test=5000, seed=0):
     """Modularity and explicitness of the encoder means `mu` [N, D] (CUDA fp32, dataset index order) of the full factor
     grid `lat_sizes` -> ({"modularity_score", "explicitness_score_train", "explicitness_score_test"}, helpers).  The
-    draws are SAP's: a device torch.Generator seeded with `seed`, `torch.randint(N, (num_train,))` for the training
-    rows, then `torch.randint(N, (num_test,))` for the test rows; the global generators are not touched.
-    Modularity is `modularity_from_mutual_info` of `discrete_mutual_info` over the training rows.  Explicitness:
-    `explicitness_fit` fits LogisticRegression(C=1) per scored factor on the standardised latents; a factor's value on
-    a set is the mean ROC AUC over its class columns that have positives and negatives there, NaN for a factor of one
-    training class or without such a column; each score is the mean over the factors with a value (NaN, with a
-    RuntimeWarning, when none has one).
+    rows and their classes are `_sap_draws`' (seeded with `seed`), as SAP's are.  Modularity is
+    `modularity_from_mutual_info` of `discrete_mutual_info` over the training rows.  Explicitness: `explicitness_fit`
+    fits LogisticRegression(C=1) per scored factor on the standardised latents; a factor's value on a set is the mean
+    ROC AUC over its class columns that have positives and negatives there, NaN for a factor of one training class or
+    without such a column; each score is the mean over the factors with a value (NaN, with a RuntimeWarning, when none
+    has one).
     helpers: "mutual_information" fp64 [D, K'], "bin_edges" fp32 [D, 21], "modularity_per_latent" fp64 [D],
     "factors" (the scored factor indices, ascending), "classes" int64 [K', S] (each factor's training values,
     ascending, -1 beyond), "feature_mean" and "feature_std" fp64 [D], "coef" fp64 [K', S, D + 1] (model rows in
@@ -756,14 +759,9 @@ def modularity_explicitness(mu, lat_sizes, num_train=10000, num_test=5000, seed=
     "explicitness_train" and "explicitness_test" fp64 [K'], "solver_iterations" int32 [K'] (Newton steps, -1 for a
     fit that did not converge, which also raises a RuntimeWarning)."""
     lat_sizes = _check_modularity_grid(lat_sizes, mu.shape[0], mu.shape[1], num_train, num_test)
-    N.require_cuda_f32(mu)
-    n = mu.shape[0]
-    gen = torch.Generator(device=mu.device)
-    gen.manual_seed(int(seed))
-    train_rows = torch.randint(n, (int(num_train),), generator=gen, device=mu.device)
-    test_rows = torch.randint(n, (int(num_test),), generator=gen, device=mu.device)
-    factors, train_cls, test_cls, n_classes, counts, present = sap_labels(lat_sizes, train_rows, test_rows)
-    K, S = counts.shape
+    train_rows, test_rows, factors, train_cls, test_cls, n_classes, counts, present = _sap_draws(
+        mu, lat_sizes, num_train, num_test, seed)
+    S = counts.shape[1]
     mi, edges = discrete_mutual_info(mu, train_rows, train_cls, n_classes, S)
     coef, auc, iters, mean, std, _ = explicitness_fit(mu, train_rows, test_rows, train_cls, test_cls, n_classes, S)
     mi, edges, coef, auc, iters = mi.cpu(), edges.cpu(), coef.cpu(), auc.cpu(), iters.cpu()
@@ -781,9 +779,8 @@ def modularity_explicitness(mu, lat_sizes, num_train=10000, num_test=5000, seed=
             warnings.warn("modularity score: no factor has an explicitness value on the %s rows; %s is NaN"
                           % (name.split("_")[-1], name), RuntimeWarning)
         score[name] = float(valued.mean()) if valued.numel() else float("nan")
-    classes = torch.sort(torch.where(present, torch.arange(S).expand(K, S), S), dim=1)[0]
     helpers = {"mutual_information": mi, "bin_edges": edges, "modularity_per_latent": per_latent,
-               "factors": torch.tensor(factors, dtype=torch.int64), "classes": torch.where(classes < S, classes, -1),
+               "factors": torch.tensor(factors, dtype=torch.int64), "classes": _classes_table(present),
                "feature_mean": mean, "feature_std": std, "coef": coef, "train_auc": auc[0].clone(),
                "test_auc": auc[1].clone(), "explicitness_train": explicit[0], "explicitness_test": explicit[1],
                "solver_iterations": iters}

@@ -13,28 +13,13 @@ import pytest
 import torch
 
 import beta_vae_reference as R
+from score_kernels import DEV, DV_ERR_BAD_ARG, DV_ERR_BAD_SHAPE, DV_ERR_WORKSPACE, _layout, grid_values
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda", 0)
-DV_ERR_BAD_SHAPE, DV_ERR_BAD_ARG, DV_ERR_WORKSPACE = -1, -2, -3
 COEF_RTOL = 1e-7          # |(W, b) - fp64 (W, b)|_inf against the fp64 solution's |(W, b)|_inf
 KKT_TOL = 1e-8            # |gradient of the fp64 objective at the GPU's (W, b)|_inf against its largest part
 MARGIN = 1e-7             # rows whose top two decisions are closer than this (relatively) may go either way
 DSPRITES = [1, 3, 6, 40, 32, 32]
-
-
-def _layout(x, layout):
-    """`x` [N, D] as the kernel reads it: a contiguous copy, or the mean half of an interleaved [N, D, 2] buffer."""
-    if layout == "contig":
-        return x.contiguous()
-    q = torch.full(x.shape + (2,), float("nan"), device=x.device)
-    q[..., 0] = x
-    return q.unbind(-1)[0]
-
-
-def _values(lat_sizes):
-    n = int(np.prod(lat_sizes))
-    return torch.from_numpy(np.stack(np.unravel_index(np.arange(n), lat_sizes), 1)).double()
 
 
 def _points(lat_sizes, num_train, num_eval, L, seed):
@@ -107,7 +92,7 @@ def _dsprites_features(seed):
     follow the scored factors."""
     from disvae.evaluate import pair_abs_diff_mean
     g = torch.Generator().manual_seed(seed)
-    v = _values(DSPRITES)
+    v = grid_values(DSPRITES).double()
     noise = torch.randn(v.size(0), 10, generator=g, dtype=torch.float64)
     mu = noise.clone()
     mu[:, :5] = v[:, 1:] / torch.tensor(DSPRITES[1:]) + 0.2 * noise[:, :5]
@@ -254,7 +239,7 @@ def test_constant_code_scores_the_majority_class_share():
 @pytest.mark.parametrize("layout", ["q_zCx", "contig"])
 def test_aligned_code_scores_one(layout):
     from disvae.evaluate import beta_vae_score
-    v = _values(DSPRITES)
+    v = grid_values(DSPRITES).double()
     g = torch.Generator().manual_seed(9)
     mu = torch.cat([v[:, 1:] / (torch.tensor(DSPRITES[1:]) - 1), torch.randn(v.size(0), 2, generator=g,
                                                                             dtype=torch.float64)], 1)

@@ -12,10 +12,10 @@ import pytest
 import torch
 
 import dci_reference as R
-from test_score_paths_gpu import DEV, LAYOUTS, Buf, _call, _lib, place_mu
+from score_kernels import (DEV, DV_ERR_BAD_ARG, DV_ERR_BAD_SHAPE, DV_ERR_WORKSPACE, LAYOUTS, Buf, _call, _Code, _code,
+                           _Factors, _graph_replays, _lib, _rows, grid_values, place_mu)
 
 pytestmark = pytest.mark.gpu
-DV_ERR_BAD_SHAPE, DV_ERR_BAD_ARG, DV_ERR_WORKSPACE = -1, -2, -3
 VALUE_RTOL = 1e-12        # leaf values, against max(1, |fp64 value|)
 IMPORTANCE_TOL = 1e-12    # importances sum to 1
 
@@ -93,27 +93,6 @@ class DciCase:
         return imp, pred, tf, tt, tv
 
 
-def _rows(n, num, seed, where=None):
-    g = torch.Generator().manual_seed(seed)
-    rows = torch.randint(n, (num,), generator=g)
-    return rows if where is None else where[rows % len(where)]
-
-
-def _values(lat_sizes):
-    n = int(np.prod(lat_sizes))
-    return torch.from_numpy(np.stack(np.unravel_index(np.arange(n), lat_sizes), 1)).float()
-
-
-def _code(lat_sizes, D, seed, noise=0.3):
-    """Latent d follows factor d (scaled to [0, 1)) plus noise; the latents past the factors are noise."""
-    g = torch.Generator().manual_seed(seed)
-    v = _values(lat_sizes)
-    x = torch.randn(v.size(0), D, generator=g)
-    K = min(D, len(lat_sizes))
-    x[:, :K] = v[:, :K] / torch.tensor(lat_sizes[:K]).float() + noise * x[:, :K]
-    return x
-
-
 # ---- kernel against the restatement -------------------------------------------------------------------------------
 @pytest.mark.parametrize("layout", LAYOUTS)
 def test_class_counts_1_2_3_40_every_layout(layout):
@@ -157,7 +136,7 @@ def test_repeated_near_equal_constant_and_duplicated_latents():
     never a candidate) and of 2e-7, latent 2 constant, latent 3 a copy of latent 5 (the lowest latent wins the tie),
     latent 4 noise."""
     lat = [6, 5, 4]
-    v = _values(lat)
+    v = grid_values(lat).float()
     n = v.size(0)
     g = torch.Generator().manual_seed(9)
     base = torch.round((v[:, 0] / 2 + 0.5 * torch.randn(n, generator=g)) * 4) / 4
@@ -176,7 +155,7 @@ def test_equal_residuals_make_leaves():
     """A binary factor that latent 0 separates: after the root split every row of a child has the same residual,
     so the children are leaves by the impurity rule, above depth 3 and with many rows."""
     lat = [2, 3]
-    v = _values(lat)
+    v = grid_values(lat).float()
     x = torch.stack([v[:, 0] * 2 - 1, torch.randn(6, generator=torch.Generator().manual_seed(12))], 1)
     case = DciCase(x, lat, _rows(6, 3000, 13), _rows(6, 500, 14), stages=3)
     imp, pred, tf, tt, tv = case.check()
@@ -225,7 +204,6 @@ def test_workspace_and_refusals_launch_nothing():
 
 
 def test_graph_replay_equals_eager():
-    from test_score_paths_gpu import _graph_replays
     lat = [3, 6]
     case = DciCase(_code(lat, 5, 18), lat, _rows(18, 2000, 19), _rows(18, 300, 20), stages=3)
     case.run()
@@ -300,39 +278,6 @@ def test_isolation_from_rng_and_other_scores(tmp_path):
             ev(loader(ds, 1000), is_metrics=True, is_losses=False, is_factor_score=True, is_sap_score=True,
                is_beta_vae_score=True)
     _assert_same_eval_files(tmp_path / "a", tmp_path / "b", files, "with vs without a DCI score", nan_equal=True)
-
-
-class _Code(torch.nn.Module):
-    """An encoder whose means are a fixed linear map of the factor values the synthetic images carry."""
-
-    def __init__(self, M):
-        super().__init__()
-        self.latent_dim = M.shape[1]
-        self.register_buffer("M", M)
-
-    def encoder(self, x):
-        v = x.view(x.size(0), -1)[:, :self.M.shape[0]]
-        return v @ self.M, torch.zeros(x.size(0), self.latent_dim, device=x.device)
-
-    def reparameterize(self, mean, logvar):
-        return mean
-
-
-class _Factors(torch.utils.data.Dataset):
-    """The full grid of `lat_sizes`; an item's 'image' holds its factor values (plus small noise) in its first pixels."""
-
-    def __init__(self, lat_sizes, noise, seed):
-        self.lat_sizes, self.lat_names = np.array(lat_sizes), tuple("f%d" % k for k in range(len(lat_sizes)))
-        v = _values(lat_sizes) / torch.tensor(lat_sizes).float()
-        g = torch.Generator().manual_seed(seed)
-        self.imgs = torch.zeros(v.size(0), 1, 8, 8)
-        self.imgs.view(v.size(0), -1)[:, :len(lat_sizes)] = v + noise * torch.randn(v.shape, generator=g)
-
-    def __len__(self):
-        return len(self.imgs)
-
-    def __getitem__(self, i):
-        return self.imgs[i], 0
 
 
 def test_known_answer_aligned_and_rotated_codes(tmp_path):

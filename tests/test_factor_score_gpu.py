@@ -12,19 +12,10 @@ import numpy as np
 import pytest
 import torch
 
+from score_kernels import DEV, DV_ERR_BAD_ARG, DV_ERR_BAD_SHAPE, _layout, grid_values
+
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda", 0)
-DV_ERR_BAD_SHAPE, DV_ERR_BAD_ARG = -1, -2
 AMBIGUOUS = 1e-5                          # two ratios closer than this (relatively) may be ordered either way in fp32
-
-
-def _layout(x, layout):
-    """`x` [N, D] as the kernel reads it: a contiguous copy, or the mean half of an interleaved [N, D, 2] buffer."""
-    if layout == "contig":
-        return x.contiguous()
-    q = torch.full(x.shape + (2,), float("nan"), device=x.device)
-    q[..., 0] = x
-    return q.unbind(-1)[0]
 
 
 def _variances(mu, rows):
@@ -181,14 +172,9 @@ def test_refusals_launch_nothing():
 LAT = [3, 4, 5, 6]
 
 
-def _factor_values(lat_sizes):
-    n = int(np.prod(lat_sizes))
-    return torch.from_numpy(np.stack(np.unravel_index(np.arange(n), lat_sizes), axis=-1)).double()
-
-
 def _aligned_mu(lat_sizes, g):
     """Dim k = factor k's value scaled to variance > 0.05, a last dim of variance 0.0004, small noise on the rest."""
-    v = _factor_values(lat_sizes)
+    v = grid_values(lat_sizes).double()
     mu = torch.cat([v / v.std(0) * 0.5, 0.02 * torch.randn(v.size(0), 1, generator=g, dtype=torch.float64)], 1)
     return mu.float().to(DEV)
 
@@ -224,7 +210,7 @@ class _Images(torch.utils.data.Dataset):
     lat_sizes = np.array(LAT)
 
     def __init__(self):
-        v = _factor_values(LAT).float()
+        v = grid_values(LAT).float()
         self.imgs = torch.zeros(v.size(0), 1, 32, 32)
         self.imgs[:, 0, 0, :len(LAT)] = v
 

@@ -18,11 +18,10 @@ import torch
 
 import beta_vae_reference as BR
 import modularity_reference as R
-from test_dci_score_gpu import _Code, _Factors, _code, _rows, _values
-from test_score_paths_gpu import DEV, LAYOUTS, Buf, _call, _graph_replays, _lib, place_mu
+from score_kernels import (DEV, DV_ERR_BAD_ARG, DV_ERR_BAD_SHAPE, DV_ERR_WORKSPACE, LAYOUTS, Buf, _call, _Code, _code,
+                           _Factors, _graph_replays, _lib, _rows, grid_values, place_mu)
 
 pytestmark = pytest.mark.gpu
-DV_ERR_BAD_SHAPE, DV_ERR_BAD_ARG, DV_ERR_WORKSPACE = -1, -2, -3
 MI_TOL = 1e-12
 STD_RTOL = 1e-12         # the kernel's fixed-order fp64 sums against numpy's pairwise ones
 COEF_RTOL, KKT_TOL = 1e-7, 1e-8
@@ -175,7 +174,7 @@ def test_constant_duplicated_edge_valued_and_refused_latents():
     """Latent 0 constant (std 1, one bin), latent 1 a copy of latent 4, latent 2 on the edges of its own histogram,
     latent 3 a range of a few ulps (numpy refuses it; the same edges bin it), latent 4 informative."""
     lat = [6, 5, 4]
-    v = _values(lat)
+    v = grid_values(lat).float()
     n = v.size(0)
     g = torch.Generator().manual_seed(12)
     x4 = v[:, 1] + 0.4 * torch.randn(n, generator=g)
@@ -197,7 +196,7 @@ def test_tied_probabilities_and_unseen_test_values():
     """One latent on a coarse grid, so rows share their probabilities (ties across positives and negatives, in
     column 0 of a binary factor as well); no training row has value 5 of the 6-value factor, which test rows have."""
     lat = [2, 6, 3]
-    v = _values(lat)
+    v = grid_values(lat).float()
     x = torch.round(v[:, :1] + 0.7 * torch.randn(v.size(0), 1, generator=torch.Generator().manual_seed(15)))
     case = ModCase(x, lat, _rows(v.size(0), 40, 16, where=torch.nonzero(v[:, 1] < 5)[:, 0]),
                    _rows(v.size(0), 2000, 17))

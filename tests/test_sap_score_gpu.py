@@ -12,22 +12,12 @@ import pytest
 import torch
 
 import sap_reference as R
+from score_kernels import DEV, DV_ERR_BAD_ARG, DV_ERR_BAD_SHAPE, _layout, grid_values
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda", 0)
-DV_ERR_BAD_SHAPE, DV_ERR_BAD_ARG = -1, -2
 COEF_RTOL = 1e-7          # |(w, b) - fp64 (w, b)|_inf against the fp64 solution's |(w, b)|_inf
 KKT_TOL = 1e-8            # |gradient of the fp64 objective at the GPU's (w, b)|_inf against its scale
 MARGIN = 1e-7             # test rows whose top two decisions are closer than this (relatively) may go either way
-
-
-def _layout(x, layout):
-    """`x` [N, D] as the kernel reads it: a contiguous copy, or the mean half of an interleaved [N, D, 2] buffer."""
-    if layout == "contig":
-        return x.contiguous()
-    q = torch.full(x.shape + (2,), float("nan"), device=x.device)
-    q[..., 0] = x
-    return q.unbind(-1)[0]
 
 
 def _run_kernel(mu, lat_sizes, train_rows, test_rows, C=0.01):
@@ -85,15 +75,10 @@ def _rows(n, num, g):
     return torch.randint(n, (num,), generator=g).to(DEV)
 
 
-def _values(lat_sizes):
-    n = int(np.prod(lat_sizes))
-    return torch.from_numpy(np.stack(np.unravel_index(np.arange(n), lat_sizes), 1)).double()
-
-
 def test_kernel_dsprites_shape():
     lat = [1, 3, 6, 40, 32, 32]
     g = torch.Generator().manual_seed(1)
-    v = _values(lat)
+    v = grid_values(lat).double()
     n = v.size(0)
     noise = torch.randn(n, 10, generator=g, dtype=torch.float64)
     x = noise.clone()
@@ -104,7 +89,7 @@ def test_kernel_dsprites_shape():
 def test_kernel_binary_factors():
     lat = [2, 2, 2, 3]
     g = torch.Generator().manual_seed(2)
-    v = _values(lat)
+    v = grid_values(lat).double()
     x = torch.cat([2 * v[:, :3] - 1 + 0.7 * torch.randn(v.size(0), 3, generator=g, dtype=torch.float64),
                    torch.randn(v.size(0), 3, generator=g, dtype=torch.float64)], 1)
     _check_against_fp64(x.float().to(DEV), lat, _rows(v.size(0), 4000, g), _rows(v.size(0), 2000, g))
@@ -126,7 +111,7 @@ def test_kernel_factor_with_one_class_in_training():
 def test_kernel_constant_and_near_constant_columns():
     lat = [4, 6]
     g = torch.Generator().manual_seed(4)
-    v = _values(lat)
+    v = grid_values(lat).double()
     n = v.size(0)
     x = torch.stack([torch.full((n,), 0.5, dtype=torch.float64),
                      0.5 + 1e-6 * torch.randn(n, generator=g, dtype=torch.float64),
@@ -139,7 +124,7 @@ def test_kernel_column_far_from_zero():
     """Means near 100 with a spread of 0.01, the spread carrying the factors."""
     lat = [5, 3]
     g = torch.Generator().manual_seed(5)
-    v = _values(lat)
+    v = grid_values(lat).double()
     n = v.size(0)
     spread = torch.cat([v / torch.tensor([5.0, 3.0]) + 0.3 * torch.randn(n, 2, generator=g, dtype=torch.float64),
                         torch.randn(n, 1, generator=g, dtype=torch.float64)], 1)
@@ -158,7 +143,7 @@ def test_kernel_dim_limit():
 def test_kernel_class_limit():
     lat = [256]
     g = torch.Generator().manual_seed(7)
-    v = _values(lat)
+    v = grid_values(lat).double()
     x = torch.cat([v / 256 + 0.05 * torch.randn(256, 1, generator=g, dtype=torch.float64),
                    torch.randn(256, 2, generator=g, dtype=torch.float64)], 1)
     train = _rows(256, 10000, g)
@@ -233,7 +218,7 @@ def test_aligned_binary_factors_score_one():
     from disvae.evaluate import sap_score
     lat = [2, 2, 2]
     g = torch.Generator().manual_seed(9)
-    v = _values(lat)
+    v = grid_values(lat).double()
     x = torch.cat([2 * v - 1, torch.randn(v.size(0), 1, generator=g, dtype=torch.float64)], 1).float().to(DEV)
     for layout in ("q_zCx", "contig"):
         score, helpers = sap_score(_layout(x, layout), lat, seed=4)

@@ -46,6 +46,7 @@ import torch
 
 import beta_vae_reference as BR
 import sap_reference as SR
+from score_kernels import DEV, DV_ERR_WORKSPACE, LAYOUTS, Buf, _bits, _call, _graph_replays, _lib, _same, place_mu
 
 U = 2.0 ** -24               # fp32 unit roundoff
 TINY = 2.0 ** -149
@@ -55,14 +56,8 @@ SAP_WARPS = 16               # kSapThreads / kWarp
 SAP_MAX_TRAIN = 32768
 FIT_THREADS = 512            # kFitThreads
 MIN_VAR = 0.05               # FACTOR_SCORE_MIN_VAR
-OFFB = 16                    # every operand starts 16 bytes into its allocation
-GUARDB = 1024                # bytes of sentinel after it
-SENT32 = 0x7FBADBAD          # NaN as fp32
-SENT64 = 0x7FFBADBADBADBADB  # NaN as fp64
-DV_OK, DV_ERR_BAD_SHAPE, DV_ERR_BAD_ARG, DV_ERR_WORKSPACE = 0, -1, -2, -3
 SAP_COEF_RTOL, SAP_KKT_TOL, SAP_MARGIN = 1e-7, 1e-8, 1e-7      # as test_sap_score_gpu.py
 FIT_COEF_RTOL, FIT_KKT_TOL, FIT_MARGIN = 1e-7, 1e-8, 1e-7      # as test_beta_vae_score_gpu.py
-LAYOUTS = ["contiguous", "q_zCx", "padded", "colmajor"]
 
 
 def _cdiv(a, b):
@@ -245,98 +240,6 @@ def _minimise(f, z0):
     from scipy.optimize import minimize
     r = minimize(f, z0, method="BFGS", options=dict(gtol=1e-12, maxiter=10000))
     return minimize(f, r.x, method="Nelder-Mead", options=dict(xatol=1e-13, fatol=1e-16, maxiter=20000)).x
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# guarded device buffers and raw calls
-# ---------------------------------------------------------------------------------------------------------------------
-DEV = torch.device("cuda", 0)
-
-
-class Buf:
-    """n elements of `dtype` 16 bytes into a device allocation, sentinel words before and after them."""
-
-    def __init__(self, n, dtype, fill=None):
-        self.es = torch.empty(0, dtype=dtype).element_size()
-        self.n = n
-        self.raw = torch.empty(OFFB + n * self.es + GUARDB, dtype=torch.uint8, device=DEV)
-        self._words().fill_(SENT32 if self.es == 4 else SENT64)
-        self.body = self.raw[OFFB:OFFB + n * self.es].view(dtype)
-        if fill is not None:
-            if torch.is_tensor(fill):
-                self.body.copy_(fill.reshape(-1))
-            else:
-                self.body.fill_(fill)
-
-    def _words(self):
-        return self.raw.view(torch.int32 if self.es == 4 else torch.int64)
-
-    @property
-    def ptr(self):
-        return self.raw.data_ptr() + OFFB
-
-    def intact(self):
-        w, k = self._words(), OFFB // self.es
-        s = SENT32 if self.es == 4 else SENT64
-        return bool((w[:k] == s).all()) and bool((w[k + self.n:] == s).all())
-
-
-def layout_strides(layout, N, D):
-    return {"contiguous": (1, D), "q_zCx": (2, 2 * D), "padded": (3, 3 * D + 5), "colmajor": (N, 1)}[layout]
-
-
-def place_mu(x, layout):
-    """fp32 x [N, D] at element (n, d) = n rs + d ld of a guarded NaN-filled buffer -> (Buf, ld, rs)."""
-    N, D = x.shape
-    ld, rs = layout_strides(layout, N, D)
-    buf = Buf((N - 1) * rs + (D - 1) * ld + 1, torch.float32, float("nan"))
-    idx = torch.arange(N, device=DEV)[:, None] * rs + torch.arange(D, device=DEV)[None, :] * ld
-    buf.body[idx.reshape(-1)] = x.to(DEV, torch.float32).reshape(-1)
-    return buf, ld, rs
-
-
-def _lib():
-    from disvae import _native as N
-    return N.lib(), N.stream()
-
-
-def _call(launches, name, *args):
-    L, _ = _lib()
-    torch.cuda.synchronize()
-    before = L.dv_launch_count()
-    rc = getattr(L, name)(*args)
-    torch.cuda.synchronize()
-    assert rc == DV_OK, (name, rc)
-    assert L.dv_launch_count() - before == launches, name
-
-
-def _bits(t):
-    t = t.contiguous()
-    return t.view(torch.int32) if t.element_size() == 4 else t.view(torch.int64)
-
-
-def _same(a, b, tag):
-    assert torch.equal(_bits(a), _bits(b)), tag + ": differs bit for bit"
-
-
-def _graph_replays(run, outs, tag):
-    """Capture `run()` (one raw call on the current stream) in a CUDA graph, clear `outs`, replay, and compare the
-    replay's bits with the eager ones."""
-    eager = [o.body.clone() for o in outs]
-    g = torch.cuda.CUDAGraph()
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        with torch.cuda.graph(g, stream=s):
-            run()
-    torch.cuda.current_stream().wait_stream(s)
-    for o in outs:
-        o.body.view(torch.uint8).fill_(0xA5)
-    g.replay()
-    torch.cuda.synchronize()
-    for e, o in zip(eager, outs):
-        _same(e, o.body, tag + " graph replay")
-        assert o.intact(), tag + " graph replay wrote past an output"
 
 
 def _report(tag, **w):

@@ -41,6 +41,15 @@ MODULARITY_MAX_DIM = 128                   # dv_explicitness_fit's limits: laten
 MODULARITY_MAX_TRAIN = 32768               # training rows,
 MODULARITY_MAX_CLASSES = 256               # and values of a scored factor
 MODULARITY_BINS = 20                       # disentanglement_lib's num_bins of the mutual information
+UDR_MAX_DIM = 128                          # dv_udr_fit's limits: latents of a model,
+UDR_MAX_COLUMNS = 4096                     # models x latents,
+UDR_MAX_POINTS = 16384                     # and points
+UDR_CORRELATIONS = {"lasso": 0, "spearman": 1}   # UDR_L and UDR_S: dv_udr_fit's modes
+UDR_LASSO_ALPHA = 0.1                      # udr.py's Lasso(alpha=0.1)
+UDR_KL_THRESHOLD = 0.01                    # a latent is informative when its mean KL is above this
+UDR_ENCODE_BATCH = 1000                    # points per encoder call
+UDR_FILENAME = "udr.log"
+UDR_HELPERS_FILE = "udr_helpers.pth"
 EVAL_SEED_STRIDE = 0x9E3779B97F4A7C15      # odd 64-bit constant: consecutive epochs get unrelated seeds
 
 
@@ -785,6 +794,163 @@ def modularity_explicitness(mu, lat_sizes, num_train=10000, num_test=5000, seed=
                "test_auc": auc[1].clone(), "explicitness_train": explicit[0], "explicitness_test": explicit[1],
                "solver_iterations": iters}
     return score, helpers
+
+
+# ---- UDR (Duan et al. 2020; disentanglement_lib's udr.py, compute_udr_sklearn) ------------------------------------
+def udr_filenames(epoch=None):
+    """(`udr.log`, `udr_helpers.pth`), or after training epoch `epoch` (`udr-{epoch}.log`, `udr_helpers-{epoch}.pth`)."""
+    if epoch is None:
+        return UDR_FILENAME, UDR_HELPERS_FILE
+    return "udr-{}.log".format(epoch), "udr_helpers-{}.pth".format(epoch)
+
+
+def check_udr(num_models, latent_dims, img_sizes=None, num_points=1000, correlation="lasso", groups=None):
+    """ValueError unless UDR can score `num_models` models of latents `latent_dims` (one per model) taking images of
+    `img_sizes` (one per model, or None) over `num_points` points with these settings: at least 2 models of one
+    latent_dim D and one image shape, 1 <= D <= UDR_MAX_DIM, K D <= UDR_MAX_COLUMNS, 2 <= num_points <=
+    UDR_MAX_POINTS, `correlation` one of UDR_CORRELATIONS, and `groups` (None: one group of every model) a partition of
+    range(num_models) into groups of at least 2.  No GPU work.  Returns the groups as lists of ints."""
+    K = int(num_models)
+    if K < 2:
+        raise ValueError("UDR: needs at least 2 models, got %d" % K)
+    dims = [int(d) for d in latent_dims]
+    if len(set(dims)) > 1:
+        raise ValueError("UDR: the models have different latent_dim %s; UDR compares latents of one size" % dims)
+    if img_sizes is not None and len({tuple(s) for s in img_sizes}) > 1:
+        raise ValueError("UDR: the models take different image shapes %s; they must encode the same images"
+                         % [tuple(s) for s in img_sizes])
+    D = dims[0]
+    if not 1 <= D <= UDR_MAX_DIM:
+        raise ValueError("UDR: latent_dim must be in [1, %d], got %d" % (UDR_MAX_DIM, D))
+    if K * D > UDR_MAX_COLUMNS:
+        raise ValueError("UDR: %d models of %d latents are %d columns, above the kernel's limit of %d"
+                         % (K, D, K * D, UDR_MAX_COLUMNS))
+    if not 2 <= int(num_points) <= UDR_MAX_POINTS:
+        raise ValueError("UDR: num_points must be in [2, %d], got %d" % (UDR_MAX_POINTS, int(num_points)))
+    if correlation not in UDR_CORRELATIONS:
+        raise ValueError("UDR: correlation must be one of %s, got %r" % (list(UDR_CORRELATIONS), correlation))
+    if groups is None:
+        return [list(range(K))]
+    groups = [[int(k) for k in g] for g in groups]
+    members = sorted(k for g in groups for k in g)
+    if members != list(range(K)):
+        raise ValueError("UDR: groups %s are not a partition of the models 0 .. %d" % (groups, K - 1))
+    for g in groups:
+        if len(g) < 2:
+            raise ValueError("UDR: group %s has fewer than 2 models; a model's score is a median over the others of "
+                             "its group" % g)
+    return groups
+
+
+def udr_fit(mu, logvar, correlation="lasso"):
+    """`dv_udr_fit` on the encoder outputs `mu`, `logvar` (contiguous CUDA fp32 [K, n, D], the same points for every
+    model) -> (raw fp64 [K, K, D, D], pair fp64 [K, K], kl fp64 [K, D], iters int32 [K, K]); see
+    include/disvae_b200.h for the rules."""
+    K, n, D = mu.shape
+    _require_operands("udr_fit", mu=(mu, torch.float32), logvar=(logvar, torch.float32, (K, n, D)))
+    check_udr(K, [D] * K, num_points=n, correlation=correlation)
+    nbytes = N.lib().dv_udr_workspace_bytes(K, n, D)
+    ws = _f64_workspace(nbytes, mu.device)
+    f64 = dict(dtype=torch.float64, device=mu.device)
+    raw, pair, kl = torch.empty(K, K, D, D, **f64), torch.empty(K, K, **f64), torch.empty(K, D, **f64)
+    iters = torch.empty(K, K, dtype=torch.int32, device=mu.device)
+    N.call("dv_udr_fit", N.ptr(mu), N.ptr(logvar), K, n, D, UDR_CORRELATIONS[correlation], UDR_LASSO_ALPHA,
+           UDR_KL_THRESHOLD, N.ptr(raw), N.ptr(pair), N.ptr(kl), N.ptr(iters), N.ptr(ws), nbytes, N.stream())
+    return raw, pair, kl, iters
+
+
+def _median(values):
+    """np.median of a 1-d fp64 tensor: the middle value, or the mean of the two middle values for an even count."""
+    v = torch.sort(values)[0]
+    m = v.numel()
+    return float((v[(m - 1) // 2] + v[m // 2]) / 2)
+
+
+def udr_from_pairs(pair, groups):
+    """Every model's UDR from the pair scores [K, K] (pair[i, j]: i's latents the inputs, j's the targets): model k
+    scores the median over the others j of its group of pair[j, k]."""
+    scores = [0.0] * pair.shape[0]
+    for g in groups:
+        for k in g:
+            scores[k] = _median(torch.stack([pair[j, k] for j in g if j != k]))
+    return scores
+
+
+def udr_score(mu, logvar, correlation="lasso", groups=None):
+    """UDR of K models from their encoder outputs `mu`, `logvar` (contiguous CUDA fp32 [K, n, D] over the same points)
+    -> ({"model_scores": [K] floats}, helpers).  `udr_fit` computes every ordered pair's score; `udr_from_pairs` takes
+    each model's median within its group (`groups`, a partition of range(K); None: one group of every model).
+    helpers: "pairwise" fp64 [K, K] (NaN on the diagonal), "raw_correlations" fp64 [K, K, D, D] (before the filter),
+    "kl" fp64 [K, D], "informative" bool [K, D], "groups" (lists of model indices) and "solver_iterations" int32
+    [K, K] (the Lasso's largest sweep count of each pair, -1 for a pair with a fit that did not converge, which also
+    raises a RuntimeWarning; 0 for Spearman)."""
+    K, n, D = mu.shape
+    groups = check_udr(K, [D] * K, num_points=n, correlation=correlation, groups=groups)
+    raw, pair, kl, iters = (t.cpu() for t in udr_fit(mu, logvar, correlation))
+    failed = int((iters < 0).sum())
+    if failed:
+        warnings.warn("UDR: %d of the pairs have a Lasso fit that did not converge in the solver's sweep limit; see "
+                      "helpers['solver_iterations'] (-1)" % failed, RuntimeWarning)
+    helpers = {"pairwise": pair, "raw_correlations": raw, "kl": kl, "informative": kl > UDR_KL_THRESHOLD,
+               "groups": groups, "solver_iterations": iters}
+    return {"model_scores": udr_from_pairs(pair, groups)}, helpers
+
+
+def udr_points(loader, num_points, seed):
+    """The dataset rows UDR encodes: `torch.randint(len(dataset), (num_points,))` from a torch.Generator on
+    `loader.device` seeded with `seed`; the global generators are not touched."""
+    gen = torch.Generator(device=loader.device)
+    gen.manual_seed(int(seed) & 0xFFFFFFFFFFFFFFFF)
+    return torch.randint(loader.n, (int(num_points),), generator=gen, device=loader.device)
+
+
+def udr(models, loader, num_points=1000, seed=0, correlation="lasso", groups=None):
+    """UDR (Duan et al. 2020) of the trained `models` (any models with the same latent_dim and image shape, on
+    `loader`'s device) over `loader` (a disvae.data.DeviceLoader) -> ({"model_scores": [K]}, helpers).  Every model
+    encodes the same `num_points` rows (`udr_points`, seeded with `seed`), gathered from the loader's resident data, in
+    eval mode (so the code is the encoder mean); each model's train / eval mode is kept.  No labels are read.  See
+    `udr_score` for the score; helpers also hold "rows" int64 [num_points]."""
+    from disvae import ops
+    from disvae.data import DeviceLoader
+    models = list(models)
+    if not isinstance(loader, DeviceLoader):
+        raise ValueError("UDR: expected a disvae.data.DeviceLoader, got %s" % type(loader).__name__)
+    groups = check_udr(len(models), [m.latent_dim for m in models], [m.img_size for m in models], num_points,
+                       correlation, groups)
+    if tuple(models[0].img_size) != tuple(loader.data.shape[1:]):
+        raise ValueError("UDR: the loader holds %s images, the models take %s"
+                         % (tuple(loader.data.shape[1:]), tuple(models[0].img_size)))
+    rows = udr_points(loader, num_points, seed)
+    K, n, D = len(models), int(num_points), int(models[0].latent_dim)
+    mu = torch.empty(K, n, D, dtype=torch.float32, device=loader.device)
+    logvar = torch.empty_like(mu)
+    with torch.no_grad():
+        for k, model in enumerate(models):
+            was_training = model.training
+            model.eval()
+            try:
+                for a in range(0, n, UDR_ENCODE_BATCH):
+                    x = ops.gather_u8_to_f32(loader.data, rows[a:a + UDR_ENCODE_BATCH])
+                    mu[k, a:a + x.shape[0]], logvar[k, a:a + x.shape[0]] = model.encoder(x)
+            finally:
+                model.train(was_training)
+    scores, helpers = udr_score(mu, logvar, correlation, groups)
+    helpers["rows"] = rows.cpu()
+    return scores, helpers
+
+
+def write_udr(models, loader, save_dirs, seed, epoch=None, loggers=None, num_points=1000, correlation="lasso",
+              groups=None):
+    """`udr(models, loader, ...)` into every model's save_dir: `udr_filenames(epoch)`, the log {"UDR": its score} and
+    the helpers with "member" = its index; each model's logger of `loggers` (or None) records its score."""
+    scores, helpers = udr(models, loader, num_points=num_points, seed=seed, correlation=correlation, groups=groups)
+    log_name, helpers_name = udr_filenames(epoch)
+    for k, save_dir in enumerate(save_dirs):
+        if loggers is not None:
+            loggers[k].info("UDR: {}".format(scores["model_scores"][k]))
+        save_metadata({"UDR": scores["model_scores"][k]}, save_dir, filename=log_name)
+        torch.save(dict(helpers, member=k), os.path.join(save_dir, helpers_name))
+    return scores, helpers
 
 
 # ---- the scores the Evaluator, training and sweeps write ----------------------------------------------------------

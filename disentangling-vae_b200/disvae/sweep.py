@@ -14,6 +14,9 @@ Member k's result is bit-identical to a lone `Trainer` run with the same setting
 `torch.manual_seed(seeds[k])`: the members share no scratch buffer, workspace or side stream (`ops.owner`), and their
 Philox keys come from `seeds` (`philox_keys`) rather than from `torch.initial_seed()` at first use.
 
+`Sweep.udr` (and `udr_every`) ranks the members against each other with the UDR score, which needs no known factors
+of variation (`disvae.evaluate.udr`).
+
 Limits: one process, one GPU, the CUDA-graph path.  Members must not have taken a training step yet (call the same
 Sweep again to continue, or, in a new process, give every member the training state it saved with `save_state=True`
 through `load_training_state`).  They must share the device and the input image shape, and
@@ -31,8 +34,8 @@ import torch
 
 from disvae import ops
 from disvae.data import DeviceLoader, device_loader_for
-from disvae.evaluate import (Evaluator, check_epoch_scores, check_resident_metrics, evaluation_rng, evaluation_seed,
-                             score_evaluator_args, select_scores, write_epoch_metrics)
+from disvae.evaluate import (Evaluator, check_epoch_scores, check_resident_metrics, check_udr, evaluation_rng,
+                             evaluation_seed, score_evaluator_args, select_scores, write_epoch_metrics, write_udr)
 from disvae.fused import FusedAdam
 from disvae.models.losses import permutation_key
 from disvae.models.vae import noise_key
@@ -48,11 +51,24 @@ def philox_keys(seed):
     return noise_key(seed), permutation_key(seed)
 
 
-class Sweep:
-    """Sweep(members, seeds): train the Trainers `members` together; `seeds[k]` plays the role of member k's
-    `torch.manual_seed` for the draws made during training (reparameterisation noise, FactorVAE permutations)."""
+def check_udr_every(udr_every):
+    if isinstance(udr_every, bool) or not isinstance(udr_every, int) or udr_every < 0:
+        raise ValueError("udr_every must be a non-negative integer (0: no UDR), got %r" % (udr_every,))
 
-    def __init__(self, members, seeds):
+
+class Sweep:
+    """Sweep(members, seeds, udr_every=0): train the Trainers `members` together; `seeds[k]` plays the role of member
+    k's `torch.manual_seed` for the draws made during training (reparameterisation noise, FactorVAE permutations).
+    `udr_every` > 0 (the attribute of that name, which may be changed between calls) ranks the members with the UDR
+    score during training: every call writes each member's `udr-{epoch}.log` and `udr_helpers-{epoch}.pth` after
+    epochs 0, e, 2e, ... and its last, what `udr` writes after that epoch (UDR over all members, seeded with
+    `evaluation_seed(loader.seed, epoch)`), independently of `metrics_every` and without known factors."""
+
+    udr_every = 0
+
+    def __init__(self, members, seeds, udr_every=0):
+        check_udr_every(udr_every)
+        self.udr_every = udr_every
         self.members, self.seeds = list(members), list(seeds)
         if not self.members:
             raise ValueError("Sweep: no members")
@@ -92,6 +108,8 @@ class Sweep:
         if len(devs) > 1:
             raise ValueError("Sweep: members are on different devices %s; a sweep runs on one GPU" % sorted(map(str, devs)))
         self.device = devs.pop()
+        if udr_every:
+            self._check_udr()
         for k, m in enumerate(self.members):
             opts = [("optimizer", m.optimizer)]
             if hasattr(m.loss_f, "call_optimize"):
@@ -140,12 +158,17 @@ class Sweep:
         each member's training state into its own save_dir; members that loaded one continue from it.
         `metrics_every` writes each member's `metrics-{epoch}.log` as `Trainer.__call__` does, one member after
         another on the caller's stream, over the one resident copy; `factor_score=True`, `sap_score=True` and
-        `beta_vae_score=True` add each member's FactorVAE, SAP and beta-VAE scores of those epochs."""
+        `beta_vae_score=True` add each member's FactorVAE, SAP and beta-VAE scores of those epochs.  With
+        `self.udr_every` > 0 the members' UDR files of those epochs are written too (see the class)."""
         scores = select_scores(locals())
         first, loader_state = self._resume()
         if loader_state is not None:
             check_loader_state(loader_state, data_loader, device_data=True)
         check_metrics_every(metrics_every)
+        udr_every = self.udr_every
+        check_udr_every(udr_every)
+        if udr_every:
+            self._check_udr()
         if metrics_every:
             check_resident_metrics(data_loader, metrics_batch_size, device_data=True)
         for m in self.members:
@@ -159,7 +182,7 @@ class Sweep:
         start = default_timer()
         with torch.cuda.device(self.device):
             self._run(loader, first, epochs, checkpoint_every, save_state, start, metrics_every, metrics_batch_size,
-                      scores)
+                      scores, udr_every)
 
     def evaluate(self, is_metrics=True, is_losses=True, batch_size=1000, is_factor_score=False, is_sap_score=False,
                  is_beta_vae_score=False):
@@ -170,7 +193,7 @@ class Sweep:
         `is_factor_score=True` also writes `factor_vae_score.log` and `factor_vae_score_helpers.pth`, seeded as the score
         after its latest epoch (`disvae.evaluate.evaluation_seed`), `is_sap_score=True` `sap_score.log` and
         `sap_score_helpers.pth`, and `is_beta_vae_score=True` `beta_vae_score.log` and `beta_vae_score_helpers.pth`,
-        seeded the same way."""
+        seeded the same way.  The UDR files of the members come from `udr`."""
         scores = select_scores(locals(), "is_")
         if self.loader is None:
             raise ValueError("Sweep.evaluate: the sweep has no loader yet; train it first (sweep(loader, ...))")
@@ -189,6 +212,26 @@ class Sweep:
                     Evaluator(m.model, m.loss_f, device=self.device, logger=m.logger, save_dir=m.save_dir,
                               is_progress_bar=m.is_progress_bar)(self.loader.in_order(batch_size), is_metrics=is_metrics,
                                                                  is_losses=is_losses, **score_args)
+
+    def udr(self, num_points=1000, seed=None, correlation="lasso", groups=None):
+        """UDR (Duan et al. 2020) of the members over the loader of the latest call -> (scores, helpers) of
+        `disvae.evaluate.udr`; member k's score is `scores["model_scores"][k]`.  Every member's save_dir gets `udr.log`
+        ({"UDR": its score}) and `udr_helpers.pth` (the helpers with "member" = k and the drawn "rows").  The points
+        are drawn with `seed`, by default `evaluation_seed(loader.seed, latest epoch)`, which depends on neither the
+        order of the members nor their seeds.  `groups` partitions the member indices (None: one group of all)."""
+        if self.loader is None:
+            raise ValueError("Sweep.udr: the sweep has no loader yet; train it first (sweep(loader, ...))")
+        groups = self._check_udr(num_points, correlation, groups)
+        if seed is None:
+            seed = evaluation_seed(self.loader.seed, self.members[0]._next_epoch - 1)
+        with torch.cuda.device(self.device):
+            return write_udr([m.model for m in self.members], self.loader, [m.save_dir for m in self.members], seed,
+                             loggers=[m.logger for m in self.members], num_points=num_points,
+                             correlation=correlation, groups=groups)
+
+    def _check_udr(self, num_points=1000, correlation="lasso", groups=None):
+        return check_udr(len(self.members), [m.model.latent_dim for m in self.members],
+                         [m.model.img_size for m in self.members], num_points, correlation, groups)
 
     def _resume(self):
         """(first epoch, saved loader state) of the members' loaded training states, (0, None) if none has one.
@@ -216,7 +259,7 @@ class Sweep:
             yield
 
     def _run(self, loader, first, epochs, checkpoint_every, save_state, start, metrics_every, metrics_batch_size,
-             scores):
+             scores, udr_every=0):
         members = self.members
         main = torch.cuda.current_stream(self.device)
         if self.streams is None:
@@ -273,6 +316,11 @@ class Sweep:
                         main.wait_event(ev)
                     for m in members:                              # the next gather, on `main`, waits for these
                         write_epoch_metrics(m.model, loader, epoch, metrics_batch_size, m.save_dir, m.logger, scores)
+                if udr_every and (epoch % udr_every == 0 or epoch == last):
+                    for ev in done:                                # every member has ended the epoch
+                        main.wait_event(ev)
+                    write_udr([m.model for m in members], loader, [m.save_dir for m in members],
+                              evaluation_seed(loader.seed, epoch), epoch, [m.logger for m in members])
         finally:
             for ev in done:
                 if ev is not None:

@@ -543,6 +543,42 @@ int dv_explicitness_fit(const float* mu, int ld, int row_stride, int N, int D, c
                         double* auc, int* iters, double* mean, double* std, double* proba, void* workspace,
                         size_t workspace_bytes, void* stream);
 
+/* ---- disentanglement metrics: UDR (Duan et al. 2020; disentanglement_lib's udr.py, compute_udr_sklearn) ----------
+ * dv_udr_fit: the unsupervised disentanglement ranking of K models that encoded the same n points.
+ *   mu, logvar fp32 [K][n][D] contiguous (model k's encoder outputs of point p at (k n + p) D), finite values assumed.
+ *   kl:       kl[k][d] = mean over the points of 0.5 (mu^2 + exp(logvar) - logvar - 1) in fp64, added in order; latent d
+ *             of model k is informative when kl[k][d] > kl_threshold.
+ *   features: each informative column standardised in fp64 (mean, std with ddof 0, std 0 taken as 1); in Spearman mode
+ *             the column's average ranks (ties averaged, the sort on the fp32 values, -0 equal to +0) standardised the
+ *             same way.  A column that is not informative is 0.
+ *   P = Z Z^T / n over the K D feature columns (each entry one fp64 sum over the points in order, then one division);
+ *   block (i, j) of P is C_ij, block (i, i) is G_i.
+ *   raw [i][j][a][b] (a a latent of i, b a latent of j):
+ *     DV_UDR_LASSO    |w_a| of sklearn's Lasso(alpha) with fit_intercept regressing j's feature b on i's features, as
+ *                     min_w 1/2 (y^T y / n - 2 C_ij[:, b]^T w + w^T G_i w) + alpha |w|_1, solved by cyclic coordinate
+ *                     descent (coordinates in order, skipped where G_i[a][a] = 0) from w = 0 until sklearn's duality
+ *                     gap is at most 1e-12 y^T y / n, at most 10000 sweeps;
+ *     DV_UDR_SPEARMAN |P[i a][j b]|: the Spearman correlation, 0 for a constant column.
+ *     NaN for i = j.
+ *   pair [i][j]: over the rows a informative in i and the columns b informative in j, the mean over those columns of
+ *     max_a R^2 / sum_a R and the mean over those rows of max_b R^2 / sum_b R (0 for 0 / 0), averaged; 0 when i or j
+ *     has no informative latent; NaN for i = j.
+ *   iters [i][j]: the largest sweep count over the D targets of the pair, -1 when a fit reached the cap; 0 in Spearman
+ *     mode and for i = j.
+ * workspace: dv_udr_workspace_bytes(K, n, D) bytes (features K D n and P (K D)^2 fp64), 8-byte aligned, contents
+ * irrelevant.  Three launches (columns: K D CTAs; P: the upper-triangular 64 x 64 tiles; pairs: K^2 CTAs, one warp per
+ * target), no host synchronisation, graph-capturable.  Deterministic (fixed-order reductions, no floating-point
+ * atomics).
+ * DV_ERR_BAD_SHAPE: K < 2, D < 1, D > 128, K D > 4096, n < 2 or n > 16384.
+ * DV_ERR_BAD_ARG: a NULL pointer, mode not one of the two, alpha not finite and positive, kl_threshold not finite and
+ * non-negative, or a pointer misaligned (mu, logvar and iters 4 bytes, the others 8).
+ * DV_ERR_WORKSPACE: workspace NULL or smaller than the query. */
+enum { DV_UDR_LASSO = 0, DV_UDR_SPEARMAN = 1 };
+size_t dv_udr_workspace_bytes(int K, int n, int D);                          /* 0: unsupported */
+int dv_udr_fit(const float* mu, const float* logvar, int K, int n, int D, int mode, double alpha, double kl_threshold,
+               double* raw, double* pair, double* kl, int* iters, void* workspace, size_t workspace_bytes,
+               void* stream);
+
 /* ---- FactorVAE pieces ---------------------------------------------------------------------
  * dv_permute_dims replaces _permute_dims (losses.py:483-508): out[b][d] = z[perm[d][b]][d].
  * perms != NULL: int64 [D][B] (the reference's CPU randperm stream, trap T7).  perms == NULL:

@@ -87,6 +87,53 @@ __device__ T block_sum(T v, T* red) {
 // The classes of scored factor k: n_classes[k] clamped to [0, S].
 __device__ __forceinline__ int class_count(const int* n_classes, int k, int S) { return min(max(n_classes[k], 0), S); }
 
+// disentanglement_lib's 20-bin histogram discretisation of an fp32 column, np.digitize(x, np.histogram(x, 20)[1][:-1]).
+constexpr int kHistBins = 20;
+
+// Every thread's partial min `lo` and max `hi` of the column -> edge[0 .. 20] (shared) for the whole block: the column's
+// range (lo - 0.5, hi + 0.5 in fp32 when equal, as np.histogram widens it), then np.linspace(lo, hi, 21) in fp32 without
+// contraction: step = (hi - lo) / 20, edge_j = j * step + lo, the last edge hi.  wlo, whi: kWarps shared slots each.
+// Ends with a barrier.
+template <int kWarps>
+__device__ void histogram_edges(float lo, float hi, float* wlo, float* whi, float* edge) {
+  const int t = threadIdx.x;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+  }
+  if ((t & (kWarp - 1)) == 0) {
+    wlo[t / kWarp] = lo;
+    whi[t / kWarp] = hi;
+  }
+  __syncthreads();
+  if (t == 0) {
+    lo = wlo[0];
+    hi = whi[0];
+    for (int w = 1; w < kWarps; ++w) {
+      lo = fminf(lo, wlo[w]);
+      hi = fmaxf(hi, whi[w]);
+    }
+    if (lo == hi) {
+      lo = __fsub_rn(lo, 0.5f);
+      hi = __fadd_rn(hi, 0.5f);
+    }
+    const float step = __fdiv_rn(__fsub_rn(hi, lo), (float)kHistBins);
+    for (int j = 0; j < kHistBins; ++j) edge[j] = __fadd_rn(__fmul_rn((float)j, step), lo);
+    edge[kHistBins] = hi;
+  }
+  __syncthreads();
+}
+
+// np.digitize(v, edge[:-1]) - 1: the number of edge_0 .. edge_19 at or below v, less one (0 .. 19).  edge_0 = lo unless
+// the range overflows fp32, so every value of the column has at least one.
+__device__ __forceinline__ int histogram_bin(const float* edge, float v) {
+  int b = 0;
+#pragma unroll
+  for (int j = 0; j < kHistBins; ++j) b += edge[j] <= v ? 1 : 0;
+  return max(b, 1) - 1;
+}
+
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));

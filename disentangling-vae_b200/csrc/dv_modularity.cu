@@ -26,7 +26,7 @@ namespace {
 
 constexpr int kMiThreads = 512;
 constexpr int kMiWarps = kMiThreads / kWarp;
-constexpr int kMiBins = 20;                   // disentanglement_lib's num_bins
+constexpr int kMiBins = kHistBins;            // disentanglement_lib's num_bins
 constexpr int kMiMaxD = 1024;
 constexpr int kModMaxD = kFitMaxD;            // dv_explicitness_fit's latents
 constexpr int kModMaxClasses = 256;
@@ -49,7 +49,7 @@ discrete_mi_kernel(const float* __restrict__ mu, int ld, int rs, const long long
   __shared__ float wlo[kMiWarps], whi[kMiWarps];
   __shared__ float edge[kMiBins + 1];
   __shared__ int occupied;
-  const int t = threadIdx.x, lane = t & (kWarp - 1), warp = t / kWarp, d = blockIdx.x;
+  const int t = threadIdx.x, d = blockIdx.x;
   const long long col = (long long)d * ld;
 
   float lo = CUDART_INF_F, hi = -CUDART_INF_F;
@@ -58,45 +58,13 @@ discrete_mi_kernel(const float* __restrict__ mu, int ld, int rs, const long long
     lo = fminf(lo, v);
     hi = fmaxf(hi, v);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, o));
-    hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, o));
-  }
-  if (lane == 0) {
-    wlo[warp] = lo;
-    whi[warp] = hi;
-  }
   if (t < kMiBins) bcnt[t] = 0;
-  __syncthreads();
-  if (t == 0) {
-    lo = wlo[0];
-    hi = whi[0];
-    for (int w = 1; w < kMiWarps; ++w) {
-      lo = fminf(lo, wlo[w]);
-      hi = fmaxf(hi, whi[w]);
-    }
-    if (lo == hi) {                                            // np.histogram's range of a constant column
-      lo = __fsub_rn(lo, 0.5f);
-      hi = __fadd_rn(hi, 0.5f);
-    }
-    // np.linspace(lo, hi, 21) in fp32: step = (hi - lo) / 20, edge_j = j * step + lo, the last edge hi
-    const float step = __fdiv_rn(__fsub_rn(hi, lo), (float)kMiBins);
-    for (int j = 0; j < kMiBins; ++j) edge[j] = __fadd_rn(__fmul_rn((float)j, step), lo);
-    edge[kMiBins] = hi;
-    if (edges_out)
-      for (int j = 0; j <= kMiBins; ++j) edges_out[(long long)d * (kMiBins + 1) + j] = edge[j];
-  }
-  __syncthreads();
-  // np.digitize(x, edges[:-1]): the number of edge_0 .. edge_19 at or below x (1 .. 20), stored less one
+  histogram_edges<kMiWarps>(lo, hi, wlo, whi, edge);
+  if (edges_out && t <= kMiBins) edges_out[(long long)d * (kMiBins + 1) + t] = edge[t];
   for (int i = t; i < n; i += kMiThreads) {
-    const float v = mu[train_rows[i] * (long long)rs + col];
-    int b = 0;
-#pragma unroll
-    for (int j = 0; j < kMiBins; ++j) b += edge[j] <= v ? 1 : 0;
-    b = max(b, 1);                                             // edge_0 = lo unless the range overflows fp32
-    bin[i] = (uint8_t)(b - 1);
-    atomicAdd(&bcnt[b - 1], 1);
+    const int b = histogram_bin(edge, mu[train_rows[i] * (long long)rs + col]);
+    bin[i] = (uint8_t)b;
+    atomicAdd(&bcnt[b], 1);
   }
   __syncthreads();
   if (t == 0) {

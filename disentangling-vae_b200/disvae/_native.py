@@ -83,6 +83,8 @@ SIGNATURES = {
     "dv_explicitness_fit": (I, [P, I, I, I, I, P, I, P, I, P, P, P, I, I, P, P, P, P, P, P, P, SZ, P]),
     "dv_udr_workspace_bytes": (SZ, [I, I, I]),
     "dv_udr_fit": (I, [P, P, I, I, I, I, DBL, DBL, P, P, P, P, P, SZ, P]),
+    "dv_unsupervised_workspace_bytes": (SZ, [I, I]),
+    "dv_unsupervised_fit": (I, [P, P, I, I, I, I, P, I, P, P, P, P, P, P, P, P, SZ, P]),
     "dv_permute_dims": (I, [P, P, ULL, P, P, I, I, P]),
     "dv_permute_dims_workspace_bytes": (SZ, [I, I]),
     "dv_permute_dims_rows": (I, [P, P, ULL, P, P, I, I, I, I, P, P]),

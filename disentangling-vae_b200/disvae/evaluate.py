@@ -50,6 +50,12 @@ UDR_KL_THRESHOLD = 0.01                    # a latent is informative when its me
 UDR_ENCODE_BATCH = 1000                    # points per encoder call
 UDR_FILENAME = "udr.log"
 UDR_HELPERS_FILE = "udr_helpers.pth"
+UNSUPERVISED_MAX_DIM = 128                 # dv_unsupervised_fit's limits: latents (the Jacobi matrix in shared memory),
+UNSUPERVISED_MAX_POINTS = 32768            # and drawn points (dv_discrete_mutual_info's)
+UNSUPERVISED_REPRESENTATIONS = ("mean", "sampled")
+UNSUPERVISED_DBL_EPSILON = 2.0 ** -52
+UNSUPERVISED_FILENAME = "unsupervised_scores.log"
+UNSUPERVISED_HELPERS_FILE = "unsupervised_scores_helpers.pth"
 EVAL_SEED_STRIDE = 0x9E3779B97F4A7C15      # odd 64-bit constant: consecutive epochs get unrelated seeds
 
 
@@ -910,7 +916,6 @@ def udr(models, loader, num_points=1000, seed=0, correlation="lasso", groups=Non
     encodes the same `num_points` rows (`udr_points`, seeded with `seed`), gathered from the loader's resident data, in
     eval mode (so the code is the encoder mean); each model's train / eval mode is kept.  No labels are read.  See
     `udr_score` for the score; helpers also hold "rows" int64 [num_points]."""
-    from disvae import ops
     from disvae.data import DeviceLoader
     models = list(models)
     if not isinstance(loader, DeviceLoader):
@@ -921,7 +926,18 @@ def udr(models, loader, num_points=1000, seed=0, correlation="lasso", groups=Non
         raise ValueError("UDR: the loader holds %s images, the models take %s"
                          % (tuple(loader.data.shape[1:]), tuple(models[0].img_size)))
     rows = udr_points(loader, num_points, seed)
-    K, n, D = len(models), int(num_points), int(models[0].latent_dim)
+    mu, logvar = encode_resident_rows(models, loader, rows)
+    scores, helpers = udr_score(mu, logvar, correlation, groups)
+    helpers["rows"] = rows.cpu()
+    return scores, helpers
+
+
+def encode_resident_rows(models, loader, rows):
+    """The encoder outputs (mu, logvar), fp32 [K, n, D], of the K `models` (one latent_dim) on the dataset rows `rows`
+    (int64 [n] on the device), gathered from `loader`'s resident data (a DeviceLoader) UDR_ENCODE_BATCH at a time, in
+    eval mode (so the code is the encoder mean); each model's train / eval mode is kept."""
+    from disvae import ops
+    K, n, D = len(models), rows.numel(), int(models[0].latent_dim)
     mu = torch.empty(K, n, D, dtype=torch.float32, device=loader.device)
     logvar = torch.empty_like(mu)
     with torch.no_grad():
@@ -934,9 +950,7 @@ def udr(models, loader, num_points=1000, seed=0, correlation="lasso", groups=Non
                     mu[k, a:a + x.shape[0]], logvar[k, a:a + x.shape[0]] = model.encoder(x)
             finally:
                 model.train(was_training)
-    scores, helpers = udr_score(mu, logvar, correlation, groups)
-    helpers["rows"] = rows.cpu()
-    return scores, helpers
+    return mu, logvar
 
 
 def write_udr(models, loader, save_dirs, seed, epoch=None, loggers=None, num_points=1000, correlation="lasso",
@@ -950,6 +964,150 @@ def write_udr(models, loader, save_dirs, seed, epoch=None, loggers=None, num_poi
             loggers[k].info("UDR: {}".format(scores["model_scores"][k]))
         save_metadata({"UDR": scores["model_scores"][k]}, save_dir, filename=log_name)
         torch.save(dict(helpers, member=k), os.path.join(save_dir, helpers_name))
+    return scores, helpers
+
+
+# ---- unsupervised scores (disentanglement_lib's unsupervised_metrics.py; Locatello et al. 2019, section 5.1) --------
+def unsupervised_filenames(epoch=None):
+    """(`unsupervised_scores.log`, `unsupervised_scores_helpers.pth`), or after training epoch `epoch`
+    (`unsupervised_scores-{epoch}.log`, `unsupervised_scores_helpers-{epoch}.pth`)."""
+    if epoch is None:
+        return UNSUPERVISED_FILENAME, UNSUPERVISED_HELPERS_FILE
+    return "unsupervised_scores-{}.log".format(epoch), "unsupervised_scores_helpers-{}.pth".format(epoch)
+
+
+def check_unsupervised_scores(latent_dim, num_train=10000):
+    """ValueError unless the unsupervised scores can be computed for codes of `latent_dim` latents over `num_train`
+    drawn points: 2 <= latent_dim <= UNSUPERVISED_MAX_DIM (np.cov of one latent is 0-d and the mutual-information
+    score divides by D^2 - D) and 2 <= num_train <= UNSUPERVISED_MAX_POINTS.  Needs no known factors; no GPU work."""
+    D = int(latent_dim)
+    if not 2 <= D <= UNSUPERVISED_MAX_DIM:
+        raise ValueError("unsupervised scores: latent_dim must be in [2, %d], got %d" % (UNSUPERVISED_MAX_DIM, D))
+    if not 2 <= int(num_train) <= UNSUPERVISED_MAX_POINTS:
+        raise ValueError("unsupervised scores: num_train must be in [2, %d], got %d"
+                         % (UNSUPERVISED_MAX_POINTS, int(num_train)))
+
+
+def unsupervised_draws(n_items, num_train, latent_dim, seed, device):
+    """(rows int64 [num_train], eps fp32 [num_train, latent_dim]) on `device`, from one torch.Generator seeded with
+    `seed`: `torch.randint(n_items, (num_train,))` first, then `torch.randn(num_train, latent_dim)`.  The global
+    generators are not touched."""
+    gen = torch.Generator(device=device)
+    gen.manual_seed(int(seed) & 0xFFFFFFFFFFFFFFFF)
+    rows = torch.randint(int(n_items), (int(num_train),), generator=gen, device=device)
+    eps = torch.randn(int(num_train), int(latent_dim), generator=gen, device=device)
+    return rows, eps
+
+
+def unsupervised_fit(mu, logvar, rows, eps):
+    """`dv_unsupervised_fit` on `mu`, `logvar` [N, D] (CUDA fp32, the same strides, any of them: views of q_zCx
+    included), the drawn `rows` int64 [n] and `eps` fp32 [n, D] -> (cov fp64 [2, D, D], eig fp64 [2, 2, D], sweeps
+    int32 [2, 2], mi fp64 [2, D, D], edges fp32 [2, D, 21]), representation 0 the mean, 1 the sampled; see
+    include/disvae_b200.h for the rules."""
+    mu_args, d = _mu_args(mu), mu.shape[1]
+    N.require_cuda_f32(logvar)
+    if logvar.shape != mu.shape or logvar.stride() != mu.stride() or logvar.device != mu.device:
+        raise ValueError("unsupervised_fit: logvar must have mu's shape, strides and device")
+    n = rows.numel()
+    _require_operands("unsupervised_fit", rows=(rows, torch.int64, (n,)), eps=(eps, torch.float32, (n, d)))
+    check_unsupervised_scores(d, n)
+    nbytes = N.lib().dv_unsupervised_workspace_bytes(n, d)
+    ws = _f64_workspace(nbytes, mu.device)
+    f64 = dict(dtype=torch.float64, device=mu.device)
+    cov, eig, mi = torch.empty(2, d, d, **f64), torch.empty(2, 2, d, **f64), torch.empty(2, d, d, **f64)
+    sweeps = torch.empty(2, 2, dtype=torch.int32, device=mu.device)
+    edges = torch.empty(2, d, MODULARITY_BINS + 1, dtype=torch.float32, device=mu.device)
+    N.call("dv_unsupervised_fit", mu_args[0], N.ptr(logvar), *mu_args[1:], N.ptr(rows), n, N.ptr(eps), N.ptr(cov),
+           N.ptr(eig), N.ptr(sweeps), N.ptr(mi), N.ptr(edges), None, N.ptr(ws), nbytes, N.stream())
+    return cov, eig, sweeps, mi, edges
+
+
+def unsupervised_from_fit(cov, eig, mi):
+    """The four scores of each representation from `unsupervised_fit`'s cov, eig and mi (fp64, combined on the host
+    in fp64) -> {"mean": {...}, "sampled": {...}} under disentanglement_lib's keys:
+    gaussian_total_correlation = -1/2 sum log eig(R) (+inf, with a RuntimeWarning, when eig_min(R) <= D DBL_EPSILON
+    eig_max(R): linearly dependent latents); gaussian_wasserstein_correlation = 2 trace(C) - 2 sum sqrt(max(eig(S), 0));
+    its _norm = that / trace(C) (0 when trace(C) = 0); mutual_info_score = the sum of mi off its diagonal / (D^2 - D)."""
+    cov, eig, mi = cov.double().cpu(), eig.double().cpu(), mi.double().cpu()
+    D = cov.shape[-1]
+    scores = {}
+    for r, name in enumerate(UNSUPERVISED_REPRESENTATIONS):
+        lam_r, lam_s = eig[r, 0], eig[r, 1]
+        if lam_r[0] <= D * UNSUPERVISED_DBL_EPSILON * lam_r[-1]:
+            warnings.warn("unsupervised scores: the %s representation has linearly dependent latents (smallest "
+                          "correlation eigenvalue %.3g); its gaussian_total_correlation is +inf" % (name, lam_r[0]),
+                          RuntimeWarning)
+            tc = math.inf
+        else:
+            tc = float(-0.5 * torch.log(lam_r).sum())
+        trace = float(torch.diagonal(cov[r]).sum())
+        w = 2.0 * trace - 2.0 * float(torch.sqrt(lam_s.clamp(min=0)).sum())
+        off = mi[r] - torch.diag(torch.diagonal(mi[r]))
+        scores[name] = {"gaussian_total_correlation": tc, "gaussian_wasserstein_correlation": w,
+                        "gaussian_wasserstein_correlation_norm": w / trace if trace != 0 else 0.0,
+                        "mutual_info_score": float(off.sum() / (D * D - D))}
+    return scores
+
+
+def _unsupervised_of(mu, logvar, fit_rows, eps, rows):
+    """(scores, helpers) of `unsupervised_fit(mu, logvar, fit_rows, eps)`, `rows` the dataset rows drawn."""
+    cov, eig, sweeps, mi, edges = (t.cpu() for t in unsupervised_fit(mu, logvar, fit_rows, eps))
+    failed = int((sweeps < 0).sum())
+    if failed:
+        warnings.warn("unsupervised scores: %d of the eigensolves stopped at the sweep limit; see "
+                      "helpers['solver_sweeps'] (-1)" % failed, RuntimeWarning)
+    scores = unsupervised_from_fit(cov, eig, mi)
+    eye = torch.eye(mi.shape[-1], dtype=torch.bool)
+    helpers = {"rows": rows.cpu(), "cov": cov, "eigenvalues": eig,
+               "constant": torch.diagonal(cov, dim1=1, dim2=2) == 0,
+               "mutual_information": mi.masked_fill(eye, 0.0), "bin_edges": edges, "solver_sweeps": sweeps}
+    return scores, helpers
+
+
+def unsupervised_scores(mu, logvar, num_train=10000, seed=0):
+    """The unsupervised scores of Locatello et al. 2019 (disentanglement_lib's unsupervised_metrics.py) of the encoder
+    outputs `mu`, `logvar` [N, D] (CUDA fp32, the same strides, any of them; q_zCx views included) ->
+    ({"mean": {4 keys}, "sampled": {4 keys}}, helpers).  `unsupervised_draws` (seeded with `seed`) draws num_train rows
+    and the noise of the sampled representation mu + exp(logvar / 2) eps; `unsupervised_fit` computes each
+    representation's covariance, the eigenvalues of its correlation matrix R and of diag(c)^1/2 C diag(c)^1/2, and the
+    mutual information of every pair of latents; `unsupervised_from_fit` combines them.  No labels are read.
+    helpers: "rows" int64 [num_train], "cov" fp64 [2, D, D], "eigenvalues" fp64 [2, 2, D] (R then S, ascending),
+    "constant" bool [2, D] (latents of zero variance over the rows), "mutual_information" fp64 [2, D, D] (diagonal
+    zeroed), "bin_edges" fp32 [2, D, 21] and "solver_sweeps" int32 [2, 2] (Jacobi sweeps, -1 for an eigensolve that
+    reached the sweep limit, which also raises a RuntimeWarning); index 0 the mean representation, 1 the sampled."""
+    n_items, D = mu.shape
+    check_unsupervised_scores(D, num_train)
+    rows, eps = unsupervised_draws(n_items, num_train, D, seed, mu.device)
+    return _unsupervised_of(mu, logvar, rows, eps, rows)
+
+
+def resident_unsupervised_scores(model, loader, num_train=10000, seed=0):
+    """`unsupervised_scores` of `model` over the dataset of `loader` (a disvae.data.DeviceLoader), encoding only the
+    drawn rows: the rows and noise are `unsupervised_draws(len(dataset), num_train, latent_dim, seed)`, the rows
+    gathered from the resident data and encoded in eval mode (`encode_resident_rows`); the model keeps its train / eval
+    mode.  Equals `unsupervised_scores` of the whole dataset's encodings in index order (up to the rounding of the
+    encoder at another batch size)."""
+    from disvae.data import DeviceLoader
+    if not isinstance(loader, DeviceLoader):
+        raise ValueError("unsupervised scores: expected a disvae.data.DeviceLoader, got %s" % type(loader).__name__)
+    check_unsupervised_scores(model.latent_dim, num_train)
+    if tuple(model.img_size) != tuple(loader.data.shape[1:]):
+        raise ValueError("unsupervised scores: the loader holds %s images, the model takes %s"
+                         % (tuple(loader.data.shape[1:]), tuple(model.img_size)))
+    rows, eps = unsupervised_draws(loader.n, num_train, model.latent_dim, seed, loader.device)
+    mu, logvar = encode_resident_rows([model], loader, rows)
+    return _unsupervised_of(mu[0], logvar[0], torch.arange(rows.numel(), device=rows.device), eps, rows)
+
+
+def write_unsupervised_scores(model, loader, save_dir, seed, epoch=None, logger=None, num_train=10000):
+    """`resident_unsupervised_scores(model, loader, num_train, seed)` into `save_dir` as
+    `unsupervised_filenames(epoch)`; `logger` (or None) records the scores."""
+    scores, helpers = resident_unsupervised_scores(model, loader, num_train, seed)
+    log_name, helpers_name = unsupervised_filenames(epoch)
+    if logger is not None:
+        logger.info("Unsupervised scores: {}".format(scores))
+    save_metadata(scores, save_dir, filename=log_name)
+    torch.save(helpers, os.path.join(save_dir, helpers_name))
     return scores, helpers
 
 
@@ -1096,6 +1254,20 @@ class Evaluator:
         seed=...)`."""
         return self._score(check_modularity_explicitness, modularity_explicitness, dataloader, seed,
                            num_train=num_train, num_test=num_test)
+
+    def compute_unsupervised_scores(self, dataloader, num_train=10000, seed=0):
+        """The unsupervised scores (Locatello et al. 2019, section 5.1) of the model's mean and sampled representations
+        over `dataloader` (any dataset, with or without known factors, in index order: DataLoader(shuffle=False) or
+        DeviceLoader.in_order) -> {"mean": {...}, "sampled": {...}}; see `unsupervised_scores` for the definition and
+        the order of the draws.  The Evaluator's __call__ and training do not write these scores; a sweep writes them
+        with `unsupervised_every` or `Sweep.unsupervised_scores`."""
+        check_unsupervised_scores(self.model.latent_dim, num_train)
+        dataset = getattr(dataloader, "dataset", None)
+        if dataset is None or not hasattr(dataset, "__len__") or len(dataset) < 1:
+            raise ValueError("unsupervised scores: expected a loader over a non-empty dataset, got %s"
+                             % type(dataloader).__name__)
+        mean, logvar = self._compute_q_zCx(dataloader)[1]
+        return unsupervised_scores(mean, logvar, num_train=num_train, seed=seed)[0]
 
     def _score(self, check, compute, dataloader, seed, **settings):
         """`compute(encoder means, lat_sizes, seed=seed, **settings)`'s score, after `check(dataset, latent_dim,

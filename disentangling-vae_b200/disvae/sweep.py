@@ -15,7 +15,9 @@ Member k's result is bit-identical to a lone `Trainer` run with the same setting
 Philox keys come from `seeds` (`philox_keys`) rather than from `torch.initial_seed()` at first use.
 
 `Sweep.udr` (and `udr_every`) ranks the members against each other with the UDR score, which needs no known factors
-of variation (`disvae.evaluate.udr`).
+of variation (`disvae.evaluate.udr`).  `Sweep.unsupervised_scores` (and `unsupervised_every`) writes every member's
+unsupervised scores of its mean and sampled representations, which need none either
+(`disvae.evaluate.unsupervised_scores`).
 
 Limits: one process, one GPU, the CUDA-graph path.  Members must not have taken a training step yet (call the same
 Sweep again to continue, or, in a new process, give every member the training state it saved with `save_state=True`
@@ -34,8 +36,9 @@ import torch
 
 from disvae import ops
 from disvae.data import DeviceLoader, device_loader_for
-from disvae.evaluate import (Evaluator, check_epoch_scores, check_resident_metrics, check_udr, evaluation_rng,
-                             evaluation_seed, score_evaluator_args, select_scores, write_epoch_metrics, write_udr)
+from disvae.evaluate import (Evaluator, check_epoch_scores, check_resident_metrics, check_udr,
+                             check_unsupervised_scores, evaluation_rng, evaluation_seed, score_evaluator_args,
+                             select_scores, write_epoch_metrics, write_udr, write_unsupervised_scores)
 from disvae.fused import FusedAdam
 from disvae.models.losses import permutation_key
 from disvae.models.vae import noise_key
@@ -52,23 +55,39 @@ def philox_keys(seed):
 
 
 def check_udr_every(udr_every):
-    if isinstance(udr_every, bool) or not isinstance(udr_every, int) or udr_every < 0:
-        raise ValueError("udr_every must be a non-negative integer (0: no UDR), got %r" % (udr_every,))
+    _check_every("udr_every", udr_every, "UDR")
+
+
+def check_unsupervised_every(unsupervised_every):
+    _check_every("unsupervised_every", unsupervised_every, "unsupervised scores")
+
+
+def _check_every(name, every, what):
+    if isinstance(every, bool) or not isinstance(every, int) or every < 0:
+        raise ValueError("%s must be a non-negative integer (0: no %s), got %r" % (name, what, every))
 
 
 class Sweep:
-    """Sweep(members, seeds, udr_every=0): train the Trainers `members` together; `seeds[k]` plays the role of member
-    k's `torch.manual_seed` for the draws made during training (reparameterisation noise, FactorVAE permutations).
+    """Sweep(members, seeds, udr_every=0, unsupervised_every=0): train the Trainers `members` together; `seeds[k]`
+    plays the role of member k's `torch.manual_seed` for the draws made during training (reparameterisation noise,
+    FactorVAE permutations).
     `udr_every` > 0 (the attribute of that name, which may be changed between calls) ranks the members with the UDR
     score during training: every call writes each member's `udr-{epoch}.log` and `udr_helpers-{epoch}.pth` after
     epochs 0, e, 2e, ... and its last, what `udr` writes after that epoch (UDR over all members, seeded with
-    `evaluation_seed(loader.seed, epoch)`), independently of `metrics_every` and without known factors."""
+    `evaluation_seed(loader.seed, epoch)`), independently of `metrics_every` and without known factors.
+    `unsupervised_every` > 0 (an attribute too) writes each member's `unsupervised_scores-{epoch}.log` and
+    `unsupervised_scores_helpers-{epoch}.pth` after the same epochs of its own count, what `unsupervised_scores` writes
+    after that epoch (seeded per member, with `evaluation_seed(member's noise key, epoch)`), independently of
+    `metrics_every` and `udr_every` and without known factors."""
 
     udr_every = 0
+    unsupervised_every = 0
 
-    def __init__(self, members, seeds, udr_every=0):
+    def __init__(self, members, seeds, udr_every=0, unsupervised_every=0):
         check_udr_every(udr_every)
+        check_unsupervised_every(unsupervised_every)
         self.udr_every = udr_every
+        self.unsupervised_every = unsupervised_every
         self.members, self.seeds = list(members), list(seeds)
         if not self.members:
             raise ValueError("Sweep: no members")
@@ -110,6 +129,8 @@ class Sweep:
         self.device = devs.pop()
         if udr_every:
             self._check_udr()
+        if unsupervised_every:
+            self._check_unsupervised()
         for k, m in enumerate(self.members):
             opts = [("optimizer", m.optimizer)]
             if hasattr(m.loss_f, "call_optimize"):
@@ -159,7 +180,8 @@ class Sweep:
         `metrics_every` writes each member's `metrics-{epoch}.log` as `Trainer.__call__` does, one member after
         another on the caller's stream, over the one resident copy; `factor_score=True`, `sap_score=True` and
         `beta_vae_score=True` add each member's FactorVAE, SAP and beta-VAE scores of those epochs.  With
-        `self.udr_every` > 0 the members' UDR files of those epochs are written too (see the class)."""
+        `self.udr_every` > 0 the members' UDR files of those epochs are written too, and with
+        `self.unsupervised_every` > 0 their unsupervised scores (see the class)."""
         scores = select_scores(locals())
         first, loader_state = self._resume()
         if loader_state is not None:
@@ -169,6 +191,10 @@ class Sweep:
         check_udr_every(udr_every)
         if udr_every:
             self._check_udr()
+        unsupervised_every = self.unsupervised_every
+        check_unsupervised_every(unsupervised_every)
+        if unsupervised_every:
+            self._check_unsupervised()
         if metrics_every:
             check_resident_metrics(data_loader, metrics_batch_size, device_data=True)
         for m in self.members:
@@ -182,7 +208,7 @@ class Sweep:
         start = default_timer()
         with torch.cuda.device(self.device):
             self._run(loader, first, epochs, checkpoint_every, save_state, start, metrics_every, metrics_batch_size,
-                      scores, udr_every)
+                      scores, udr_every, unsupervised_every)
 
     def evaluate(self, is_metrics=True, is_losses=True, batch_size=1000, is_factor_score=False, is_sap_score=False,
                  is_beta_vae_score=False):
@@ -229,6 +255,30 @@ class Sweep:
                              loggers=[m.logger for m in self.members], num_points=num_points,
                              correlation=correlation, groups=groups)
 
+    def unsupervised_scores(self, num_train=10000, seed=None):
+        """Every member's unsupervised scores (`disvae.evaluate.unsupervised_scores`) over the loader of the latest
+        call -> [(scores, helpers)] in member order.  Member k's save_dir gets `unsupervised_scores.log` and
+        `unsupervised_scores_helpers.pth`.  Each member encodes only its own drawn rows, seeded with `seed`, by default
+        `evaluation_seed(its noise key, latest epoch)` -- the rule of the metrics, so a member's files do not depend on
+        the other members."""
+        if self.loader is None:
+            raise ValueError("Sweep.unsupervised_scores: the sweep has no loader yet; train it first (sweep(loader, ...))")
+        self._check_unsupervised(num_train)
+        out = []
+        with torch.cuda.device(self.device):
+            for m in self.members:
+                s = self._unsupervised_seed(m, m._next_epoch - 1) if seed is None else seed
+                out.append(write_unsupervised_scores(m.model, self.loader, m.save_dir, s, logger=m.logger,
+                                                     num_train=num_train))
+        return out
+
+    def _unsupervised_seed(self, m, epoch):
+        return evaluation_seed(m.model._noise_state(self.device)[0], epoch)
+
+    def _check_unsupervised(self, num_train=10000):
+        for m in self.members:
+            check_unsupervised_scores(m.model.latent_dim, num_train)
+
     def _check_udr(self, num_points=1000, correlation="lasso", groups=None):
         return check_udr(len(self.members), [m.model.latent_dim for m in self.members],
                          [m.model.img_size for m in self.members], num_points, correlation, groups)
@@ -259,7 +309,7 @@ class Sweep:
             yield
 
     def _run(self, loader, first, epochs, checkpoint_every, save_state, start, metrics_every, metrics_batch_size,
-             scores, udr_every=0):
+             scores, udr_every=0, unsupervised_every=0):
         members = self.members
         main = torch.cuda.current_stream(self.device)
         if self.streams is None:
@@ -321,6 +371,12 @@ class Sweep:
                         main.wait_event(ev)
                     write_udr([m.model for m in members], loader, [m.save_dir for m in members],
                               evaluation_seed(loader.seed, epoch), epoch, [m.logger for m in members])
+                if unsupervised_every and (epoch % unsupervised_every == 0 or epoch == last):
+                    for ev in done:                                # every member has ended the epoch
+                        main.wait_event(ev)
+                    for m in members:
+                        write_unsupervised_scores(m.model, loader, m.save_dir, self._unsupervised_seed(m, epoch), epoch,
+                                                  m.logger)
         finally:
             for ev in done:
                 if ev is not None:

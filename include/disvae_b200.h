@@ -579,6 +579,43 @@ int dv_udr_fit(const float* mu, const float* logvar, int K, int n, int D, int mo
                double* raw, double* pair, double* kl, int* iters, void* workspace, size_t workspace_bytes,
                void* stream);
 
+/* ---- disentanglement metrics: unsupervised scores (disentanglement_lib's unsupervised_metrics.py) ---------------
+ * dv_unsupervised_fit: the pieces of the Gaussian total correlation, the Gaussian Wasserstein correlation and the
+ * average pairwise mutual information of n drawn points, on the mean and on the sampled representation.
+ *   mu, logvar: read as dv_group_variance reads mu (element (p, d) at p*row_stride + d*ld; q_zCx in place), finite
+ *             values assumed; rows int64 [n], every entry in [0, N) (not checked); eps fp32 [n][D].
+ *   codes:    representation 0 is mu[rows[i]][d]; representation 1 is z = fmaf(expf(0.5f * lv), eps[i][d], mu) in
+ *             fp32 (lv = logvar[rows[i]][d], expf the full-precision one).
+ *   cov   fp64 [2][D][D]: np.cov of each representation's codes (ddof 1): column means in fp64 (fixed-order sums), then
+ *         sum_i (x_ia - m_a)(x_ib - m_b) / (n - 1) in fp64, a fixed-order sum over the points; exactly symmetric.
+ *   eig   fp64 [2][2][D]: per representation, the eigenvalues, ascending, of
+ *           R = the correlation matrix, R_ab = C_ab / (sqrt(C_aa) sqrt(C_bb)), R_aa = 1; a latent with C_aa = 0 has a
+ *               unit row and column;
+ *           S = diag(c)^1/2 C diag(c)^1/2 with c = diag(C), S_ab = sqrt(c_a) C_ab sqrt(c_b) (a <= b, mirrored), which
+ *               is similar to diag(c) C and symmetric positive semi-definite;
+ *         by parallel cyclic Jacobi in fp64 (round-robin order) until the off-diagonal Frobenius norm is at most 1e-15
+ *         of the Frobenius norm, at most 50 sweeps.
+ *   sweeps int32 [2][2]: the Jacobi sweeps of each matrix, -1 when the cap stopped it.
+ *   mi    fp64 [2][D][D]: mi[r][a][b] = sklearn's mutual_info_score(bins_b, bins_a) of representation r, where bins_a
+ *         is np.digitize(x_a, np.histogram(x_a, 20)[1][:-1]) of its fp32 column: dv_discrete_mutual_info with latent b's
+ *         bins as factor b (renumbered over its occupied bins; one occupied bin gives 0, sklearn's rule).  The
+ *         diagonal is written too.
+ *   edges fp32 [2][D][21] (optional, NULL for none): each column's histogram edges.
+ *   sampled fp32 [n][D] (optional, NULL for none): z.
+ * workspace: dv_unsupervised_workspace_bytes(n, D) bytes, 8-byte aligned, contents irrelevant.  Six launches (gather;
+ * columns: 2 D CTAs; covariance: D (D + 1) CTAs; eigenvalues: 4 CTAs; mutual information: two dv_discrete_mutual_info
+ * launches), no host synchronisation, graph-capturable.  Deterministic (fixed-order reductions, no floating-point
+ * atomics).
+ * DV_ERR_BAD_SHAPE: N < 1, D < 2, D > 128, n < 2, n > 32768, ld < 1 or row_stride < 1.
+ * DV_ERR_BAD_ARG: a required pointer NULL (all but edges and sampled), or a pointer misaligned (rows, cov, eig, mi and
+ * workspace 8 bytes, the others 4).
+ * DV_ERR_WORKSPACE: workspace NULL or smaller than the query. */
+size_t dv_unsupervised_workspace_bytes(int n, int D);                        /* 0: unsupported */
+int dv_unsupervised_fit(const float* mu, const float* logvar, int ld, int row_stride, int N, int D,
+                        const long long* rows, int n, const float* eps, double* cov, double* eig, int* sweeps,
+                        double* mi, float* edges, float* sampled, void* workspace, size_t workspace_bytes,
+                        void* stream);
+
 /* ---- FactorVAE pieces ---------------------------------------------------------------------
  * dv_permute_dims replaces _permute_dims (losses.py:483-508): out[b][d] = z[perm[d][b]][d].
  * perms != NULL: int64 [D][B] (the reference's CPU randperm stream, trap T7).  perms == NULL:

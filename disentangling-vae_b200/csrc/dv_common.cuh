@@ -134,6 +134,46 @@ __device__ __forceinline__ int histogram_bin(const float* edge, float v) {
   return max(b, 1) - 1;
 }
 
+// Sorting fp32 columns in shared memory (DCI's training columns, IRS's latents): order_key maps a float to an unsigned
+// key whose order is the float's (-0 just below +0), key_value maps it back, and bitonic_sort_pairs sorts P (a power of
+// two) (key, position) pairs ascending on (key, position) with kThreads threads, so equal values keep their order.
+// Padding pairs take the key 0xffffffff.  Called after a barrier; ends with one.
+inline int pow2_at_least(int n) {
+  int p = 1;
+  while (p < n) p <<= 1;
+  return p;
+}
+
+__device__ __forceinline__ unsigned order_key(float v) {
+  const unsigned u = __float_as_uint(v);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_value(unsigned k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+template <int kThreads>
+__device__ void bitonic_sort_pairs(unsigned* key, unsigned short* idx, int P) {
+  const int t = threadIdx.x;
+  for (int k = 2; k <= P; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = t; i < P; i += kThreads) {
+        const int o = i ^ j;
+        if (o > i) {
+          const unsigned ka = key[i], kb = key[o];
+          const unsigned short ia = idx[i], ib = idx[o];
+          const bool greater = ka > kb || (ka == kb && ia > ib);
+          if (greater == ((i & k) == 0)) {
+            key[i] = kb; key[o] = ka;
+            idx[i] = ib; idx[o] = ia;
+          }
+        }
+      }
+      __syncthreads();
+    }
+  }
+}
+
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));

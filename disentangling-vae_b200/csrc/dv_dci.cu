@@ -82,21 +82,7 @@ size_t dci_layout(int D, int n, int m, int K, int S, char* base, DciWs* w) {
   return total;
 }
 
-int pow2_at_least(int n) {
-  int p = 1;
-  while (p < n) p <<= 1;
-  return p;
-}
-
 __device__ __forceinline__ int dci_columns(int nc) { return nc > 2 ? nc : (nc == 2 ? 1 : 0); }
-
-__device__ __forceinline__ unsigned order_key(float v) {
-  const unsigned u = __float_as_uint(v);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key_value(unsigned k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
 
 __global__ void __launch_bounds__(kDciSortThreads, 1)
 dci_prep_kernel(const float* __restrict__ mu, int ld, int rs, const long long* __restrict__ train_rows, int n,
@@ -119,23 +105,7 @@ dci_prep_kernel(const float* __restrict__ mu, int ld, int rs, const long long* _
   }
   for (int j = t; j < m; j += kDciSortThreads) w.xe[(long long)d * m + j] = mu[test_rows[j] * (long long)rs + col];
   __syncthreads();
-  for (int k = 2; k <= P; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = t; i < P; i += kDciSortThreads) {
-        const int o = i ^ j;
-        if (o > i) {
-          const unsigned ka = key[i], kb = key[o];
-          const unsigned short ia = idx[i], ib = idx[o];
-          const bool greater = ka > kb || (ka == kb && ia > ib);
-          if (greater == ((i & k) == 0)) {
-            key[i] = kb; key[o] = ka;
-            idx[i] = ib; idx[o] = ia;
-          }
-        }
-      }
-      __syncthreads();
-    }
-  }
+  bitonic_sort_pairs<kDciSortThreads>(key, idx, P);
   for (int i = t; i < n; i += kDciSortThreads) {
     w.sval[(long long)d * n + i] = key_value(key[i]);
     w.sidx[(long long)d * n + i] = idx[i];

@@ -41,6 +41,9 @@ MODULARITY_MAX_DIM = 128                   # dv_explicitness_fit's limits: laten
 MODULARITY_MAX_TRAIN = 32768               # training rows,
 MODULARITY_MAX_CLASSES = 256               # and values of a scored factor
 MODULARITY_BINS = 20                       # disentanglement_lib's num_bins of the mutual information
+IRS_MAX_DIM = 1024                         # dv_irs_fit's limits: latents,
+IRS_MAX_TRAIN = 32768                      # and drawn rows (one latent's sort in shared memory)
+IRS_BINS = 20                              # disentanglement_lib's make_discretizer of the factors
 UDR_MAX_DIM = 128                          # dv_udr_fit's limits: latents of a model,
 UDR_MAX_COLUMNS = 4096                     # models x latents,
 UDR_MAX_POINTS = 16384                     # and points
@@ -374,14 +377,20 @@ def sap_labels(lat_sizes, train_rows, test_rows):
             torch.stack(counts).int(), present)
 
 
+def _train_rows(mu, num_train, seed):
+    """(generator, rows): a device torch.Generator seeded with `seed` and its first draw, `torch.randint(N,
+    (num_train,))`, for `mu` [N, D] (CUDA fp32).  The global generators are not touched."""
+    N.require_cuda_f32(mu)
+    gen = torch.Generator(device=mu.device)
+    gen.manual_seed(int(seed))
+    return gen, torch.randint(mu.shape[0], (int(num_train),), generator=gen, device=mu.device)
+
+
 def _sap_draws(mu, lat_sizes, num_train, num_test, seed):
     """The rows of the SAP, DCI, modularity and explicitness scores of `mu` [N, D] (CUDA fp32) -> (train_rows,
     test_rows) + `sap_labels`' tuple.  They come from a device torch.Generator seeded with `seed`: `torch.randint(N,
     (num_train,))`, then `torch.randint(N, (num_test,))`; the global generators are not touched."""
-    N.require_cuda_f32(mu)
-    gen = torch.Generator(device=mu.device)
-    gen.manual_seed(int(seed))
-    train_rows = torch.randint(mu.shape[0], (int(num_train),), generator=gen, device=mu.device)
+    gen, train_rows = _train_rows(mu, num_train, seed)
     test_rows = torch.randint(mu.shape[0], (int(num_test),), generator=gen, device=mu.device)
     return (train_rows, test_rows) + sap_labels(lat_sizes, train_rows, test_rows)
 
@@ -800,6 +809,93 @@ def modularity_explicitness(mu, lat_sizes, num_train=10000, num_test=5000, seed=
                "test_auc": auc[1].clone(), "explicitness_train": explicit[0], "explicitness_test": explicit[1],
                "solver_iterations": iters}
     return score, helpers
+
+
+# ---- IRS (Suter et al. 2019; disentanglement_lib's irs.py) -------------------------------------------------------
+def check_irs_score(dataset, latent_dim, num_train=10000, diff_quantile=0.99):
+    """ValueError unless IRS can be computed over `dataset` for a `latent_dim` model with these settings: the dataset
+    has known factors (`lat_sizes`, `lat_names`), is their full grid and has a factor of more than one value.  No GPU
+    work.  Returns lat_sizes as a list of ints."""
+    return _check_irs_grid(_dataset_lat_sizes("IRS", dataset), len(dataset), latent_dim, num_train, diff_quantile)
+
+
+def _check_irs_grid(lat_sizes, n, latent_dim, num_train, diff_quantile):
+    lat_sizes = _full_grid("IRS", lat_sizes, n)
+    if all(s == 1 for s in lat_sizes):
+        raise ValueError("IRS: every factor of %s has one value; there is no factor to intervene on" % lat_sizes)
+    if not 1 <= int(latent_dim) <= IRS_MAX_DIM:
+        raise ValueError("IRS: latent_dim must be in [1, %d], got %d" % (IRS_MAX_DIM, int(latent_dim)))
+    if not 1 <= int(num_train) <= IRS_MAX_TRAIN:
+        raise ValueError("IRS: num_train must be in [1, %d], got %d" % (IRS_MAX_TRAIN, int(num_train)))
+    if not 0.0 <= float(diff_quantile) <= 1.0:
+        raise ValueError("IRS: diff_quantile must be in [0, 1], got %r" % (diff_quantile,))
+    return lat_sizes
+
+
+def irs_fit(mu, rows, values, diff_quantile):
+    """`dv_irs_fit` on `mu` [N, D] (any strides, a view of q_zCx included), the drawn `rows` int64 [n] and the scored
+    factors' `values` int32 [K', n] -> (max_deviation fp64 [D], active int32 [D], irs_matrix fp64 [D, K'],
+    group_deviation fp64 [K', 20, D], group_count int32 [K', 20], edges fp64 [K', 21]); see include/disvae_b200.h for
+    the rules."""
+    mu_args, d = _mu_args(mu), mu.shape[1]
+    _require_operands("irs_fit", rows=(rows, torch.int64), values=(values, torch.int32))
+    n = rows.numel()
+    K = values.shape[0]
+    if values.dim() != 2 or values.shape[1] != n:
+        raise ValueError("irs_fit: values must be [K', %d], got %s" % (n, tuple(values.shape)))
+    nbytes = N.lib().dv_irs_workspace_bytes(d, n, K)
+    ws = _f64_workspace(nbytes, mu.device)
+    f64 = dict(dtype=torch.float64, device=mu.device)
+    i32 = dict(dtype=torch.int32, device=mu.device)
+    out = (torch.empty(d, **f64), torch.empty(d, **i32), torch.empty(d, K, **f64),
+           torch.empty(K, IRS_BINS, d, **f64), torch.empty(K, IRS_BINS, **i32), torch.empty(K, IRS_BINS + 1, **f64))
+    N.call("dv_irs_fit", *mu_args, N.ptr(rows), n, N.ptr(values), K, float(diff_quantile), *(N.ptr(t) for t in out),
+           N.ptr(ws), nbytes, N.stream())
+    return out
+
+
+def irs_from_matrix(irs_matrix, max_deviations, active):
+    """(IRS, per-latent scores [D], parents [D]) of `irs_fit`'s matrix [D, K'], in fp64 on the host, as irs.py's
+    scalable_disentanglement_score finishes it over the active latents: a latent's score is its row's maximum and its
+    parent that row's argmax (the lowest factor on a tie); IRS is the mean of the scores weighted by `max_deviations`,
+    added in latent order.  Inactive latents score NaN with parent -1; with no active latent IRS is 0.0."""
+    M = irs_matrix.double().cpu()
+    dev = max_deviations.double().cpu().tolist()
+    per_latent = torch.full((M.shape[0],), float("nan"), dtype=torch.float64)
+    parents = torch.full((M.shape[0],), -1, dtype=torch.int64)
+    num, den = 0.0, 0.0
+    for d in torch.nonzero(active.cpu().bool())[:, 0].tolist():
+        parents[d] = torch.argmax(M[d])                # the first of equal maxima
+        per_latent[d] = M[d, parents[d]]
+        num += dev[d] * float(per_latent[d])
+        den += dev[d]
+    return (num / den if den > 0.0 else 0.0), per_latent, parents
+
+
+def irs_score(mu, lat_sizes, num_train=10000, diff_quantile=0.99, seed=0):
+    """IRS (Suter et al. 2019) of the encoder means `mu` [N, D] (CUDA fp32, dataset index order) of the full factor
+    grid `lat_sizes` -> ({"IRS", "num_active_dims"}, helpers).  The rows are `_train_rows`' draw seeded with `seed`,
+    the training rows `_sap_draws` gives SAP, DCI and modularity; the scored factors are those of more than one value,
+    ascending, each binned by disentanglement_lib's 20-bin histogram of its drawn values.  `irs_fit` gives the
+    per-(latent, factor) matrix on the device, `irs_from_matrix` finishes it on the host.  "num_active_dims" counts the
+    latents whose drawn values are not all equal.
+    helpers: "irs_matrix" fp64 [D, K'] (NaN for an inactive latent), "disentanglement_scores" fp64 [D] (NaN when
+    inactive), "parents" int64 [D] (-1 when inactive), "max_deviations" fp64 [D], "active_dims" bool [D], "factors"
+    int64 [K'] (the scored factor indices, ascending), "bin_edges" fp64 [K', 21], "group_counts" int64 [K', 20] and
+    "group_deviations" fp64 [K', 20, D] (NaN for an empty bin)."""
+    lat_sizes = _check_irs_grid(lat_sizes, mu.shape[0], mu.shape[1], num_train, diff_quantile)
+    _, rows = _train_rows(mu, num_train, seed)
+    factors = [k for k, s in enumerate(lat_sizes) if s > 1]
+    strides = [reduce(lambda x, y: x * y, lat_sizes[k + 1:], 1) for k in range(len(lat_sizes))]
+    values = torch.stack([rows // strides[k] % lat_sizes[k] for k in factors]).int()
+    max_dev, active, matrix, group_dev, group_count, edges = (t.cpu() for t in irs_fit(mu, rows, values,
+                                                                                         diff_quantile))
+    active = active.bool()
+    irs, per_latent, parents = irs_from_matrix(matrix, max_dev, active)
+    helpers = {"irs_matrix": matrix, "disentanglement_scores": per_latent, "parents": parents,
+               "max_deviations": max_dev, "active_dims": active, "factors": torch.tensor(factors, dtype=torch.int64),
+               "bin_edges": edges, "group_counts": group_count.long(), "group_deviations": group_dev}
+    return {"IRS": irs, "num_active_dims": int(active.sum())}, helpers
 
 
 # ---- UDR (Duan et al. 2020; disentanglement_lib's udr.py, compute_udr_sklearn) ------------------------------------
@@ -1254,6 +1350,15 @@ class Evaluator:
         seed=...)`."""
         return self._score(check_modularity_explicitness, modularity_explicitness, dataloader, seed,
                            num_train=num_train, num_test=num_test)
+
+    def compute_irs_score(self, dataloader, num_train=10000, diff_quantile=0.99, seed=0):
+        """IRS (Suter et al. 2019) of the model's encoder means over `dataloader` (the dataset in index order:
+        DataLoader(shuffle=False) or DeviceLoader.in_order) -> {"IRS", "num_active_dims"}; see `irs_score` for the
+        definition and the draw.  The Evaluator's __call__, training and sweeps do not write this score; score a
+        sweep's members with `Evaluator(member.model, None, device=...).compute_irs_score(sweep.loader.in_order(1000),
+        seed=...)`."""
+        return self._score(check_irs_score, irs_score, dataloader, seed, num_train=num_train,
+                           diff_quantile=diff_quantile)
 
     def compute_unsupervised_scores(self, dataloader, num_train=10000, seed=0):
         """The unsupervised scores (Locatello et al. 2019, section 5.1) of the model's mean and sampled representations

@@ -543,6 +543,38 @@ int dv_explicitness_fit(const float* mu, int ld, int row_stride, int N, int D, c
                         double* auc, int* iters, double* mean, double* std, double* proba, void* workspace,
                         size_t workspace_bytes, void* stream);
 
+/* ---- disentanglement metrics: IRS (Suter et al. 2019; disentanglement_lib's irs.py) ------------------------------
+ * dv_irs_fit: the interventional robustness score's tables of n drawn rows over K scored factors.
+ *   mu is read as dv_group_variance reads it (element (p, d) at p*row_stride + d*ld; q_zCx in place), finite values
+ *   assumed.  rows int64 [n], every entry in [0, N) (not checked); values int32 [K][n]: factor k's value of drawn row i.
+ *   x_d = the fp32 values mu[rows[i]][d], taken in fp64.
+ *   max_deviation fp64 [D]: max_i |x_i - mean(x)|, the mean an fp64 sum in a fixed order over n.
+ *   active int32 [D]: 1 when the latent's drawn values are not all equal (-0 equal to +0), i.e. max_deviation > 0.
+ *   edges fp64 [K][21]: np.histogram(values[k], 20)'s edges of an int64 array: lo, hi = min, max (lo - 0.5, hi + 0.5
+ *         when equal), step = (hi - lo) / 20, edge_j = j * step + lo (j < 20), edge_20 = hi, each operation rounded in
+ *         fp64 without contraction.  A row's bin is the number of edge_0 .. edge_19 at or below its value, less one
+ *         (0 .. 19).
+ *   group_count int32 [K][20]: the rows of each bin.
+ *   group_deviation fp64 [K][20][D]: for a non-empty bin b of m rows with fp64 mean c of x over them,
+ *         np.percentile(|x - c|, diff_quantile * 100) by numpy's linear rule in fp64 without contraction:
+ *         q = (diff_quantile * 100) / 100, h = (m - 1) q, lo = floor(h), hi = min(lo + 1, m - 1), t = h - lo; with a, b
+ *         the ascending order statistics at lo and hi, a + (b - a) t when t < 0.5, else b - (b - a)(1 - t).  NaN for an
+ *         empty bin.
+ *   irs_matrix fp64 [D][K]: 1 - cum / max_deviation[d], cum the mean of group_deviation[k][b][d] over the non-empty bins
+ *         of factor k, added in bin order; NaN for an inactive latent.
+ * workspace: dv_irs_workspace_bytes(D, n, K) bytes, 8-byte aligned, contents irrelevant.  Three launches (columns: D
+ * CTAs; bins: K CTAs; groups: D K CTAs), no host synchronisation, graph-capturable.  Deterministic (fixed-order
+ * reductions, no floating-point atomics).
+ * DV_ERR_BAD_SHAPE: N < 1, D < 1, D > 1024, n < 1, n > 32768, K < 1, ld < 1, row_stride < 1, diff_quantile outside
+ * [0, 1] or NaN, or K*n or K*20*D above INT_MAX.
+ * DV_ERR_BAD_ARG: a NULL pointer, or one misaligned (mu, values, active and group_count 4 bytes, the others 8).
+ * DV_ERR_WORKSPACE: workspace NULL or smaller than the query. */
+size_t dv_irs_workspace_bytes(int D, int n, int K);                          /* 0: unsupported */
+int dv_irs_fit(const float* mu, int ld, int row_stride, int N, int D, const long long* rows, int n, const int* values,
+               int K, double diff_quantile, double* max_deviation, int* active, double* irs_matrix,
+               double* group_deviation, int* group_count, double* edges, void* workspace, size_t workspace_bytes,
+               void* stream);
+
 /* ---- disentanglement metrics: UDR (Duan et al. 2020; disentanglement_lib's udr.py, compute_udr_sklearn) ----------
  * dv_udr_fit: the unsupervised disentanglement ranking of K models that encoded the same n points.
  *   mu, logvar fp32 [K][n][D] contiguous (model k's encoder outputs of point p at (k n + p) D), finite values assumed.

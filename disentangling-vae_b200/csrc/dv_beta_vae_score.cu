@@ -59,7 +59,7 @@ logistic_fit_kernel(const double* __restrict__ x, int D, int num_train, int num_
   const bool multi = nc > 2;
   const int Dp = D + 1;
   const int rows = num_train + num_eval;
-  logistic_fit_cta(x, D, num_train, labels, nc, K, coef, iters, ws);
+  logistic_fit_cta(x, D, num_train, labels, nc, multi, 1.0, K, coef, iters, ws);
 
   // predictions: argmax_r W_r x + b_r (lowest r on a tie), or class 1 when w x + b > 0; 0 for nc = 1
   for (int i = t; i < rows; i += kFitThreads) {

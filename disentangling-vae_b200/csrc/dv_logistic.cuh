@@ -1,7 +1,8 @@
 // The fp64 logistic-regression solver shared by dv_logistic_fit (dv_beta_vae_score.cu) and dv_explicitness_fit
-// (dv_modularity.cu): the exact minimiser of sklearn's LogisticRegression(C=1) objective, one CTA of kFitThreads
-// threads per fit.  The objective, the method and the rules of the solve are described at the top of
-// dv_beta_vae_score.cu and in include/disvae_b200.h.
+// (dv_modularity.cu) at C = 1, and by dv_downstream_logistic_cv (dv_downstream.cu) at every C of its grid: the exact
+// minimiser of sklearn's LogisticRegression(C) objective C sum_i loss_i + 1/2 |W|^2, one CTA of kFitThreads threads per
+// fit.  The objective, the method and the rules of the solve are described at the top of dv_beta_vae_score.cu and in
+// include/disvae_b200.h.  C multiplies each row sum once, so at C = 1 every operation rounds as it did without it.
 #pragma once
 
 #include <math.h>
@@ -28,6 +29,7 @@ struct Fit {
   const int* y;         // [n] class indices
   int n, D, Dp, R, O;   // Dp = D + 1, O = R * Dp parameters, parameter (r, d) at r * Dp + d (d = D: the intercept)
   bool multi;
+  double C;             // the weight of the loss against 1/2 |W|^2
   double* mean;         // [D]
   double *theta, *grad, *scale, *dir, *res, *zv, *pv, *hp, *trial, *diag;   // [O] each
   double *P, *Q, *U;    // [n][R]
@@ -109,7 +111,7 @@ __device__ void rows_dot(const Fit& F, const double* V) {
   __syncthreads();
 }
 
-// Subtract the mean of the intercept entries (nc > 2 only).
+// Subtract the mean of the intercept entries (multinomial fits only).
 __device__ void project(const Fit& F, double* v) {
   __syncthreads();
   if (!F.multi) return;
@@ -154,17 +156,20 @@ __device__ double objective(const Fit& F, const double* V) {
   double reg = 0.0;
   for (int o = threadIdx.x; o < F.O; o += kFitThreads)
     if (o % F.Dp != F.D) reg = fma(V[o], V[o], reg);
-  return 0.5 * block_sum<kFitWarps>(reg, F.red) + block_sum<kFitWarps>(acc, F.red);
+  return 0.5 * block_sum<kFitWarps>(reg, F.red) + F.C * block_sum<kFitWarps>(acc, F.red);
 }
 
 // grad and scale at theta, from the Q of the last `objective(theta)`.
 __device__ void gradient(const Fit& F) {
   colsum(F, F.Q, false, F.grad, F.scale);
-  for (int o = threadIdx.x; o < F.O; o += kFitThreads)
+  for (int o = threadIdx.x; o < F.O; o += kFitThreads) {
+    F.grad[o] *= F.C;
+    F.scale[o] *= F.C;
     if (o % F.Dp != F.D) {
       F.grad[o] += F.theta[o];
       F.scale[o] += fabs(F.theta[o]);
     }
+  }
   project(F, F.grad);
 }
 
@@ -185,8 +190,10 @@ __device__ void hess_vec(const Fit& F, const double* v, double* hp) {
   }
   __syncthreads();
   colsum(F, F.Q, false, hp, nullptr);
-  for (int o = threadIdx.x; o < F.O; o += kFitThreads)
+  for (int o = threadIdx.x; o < F.O; o += kFitThreads) {
+    hp[o] *= F.C;
     if (o % F.Dp != F.D) hp[o] += v[o];
+  }
   project(F, hp);
 }
 
@@ -197,7 +204,7 @@ __device__ void hess_diag(const Fit& F) {
   __syncthreads();
   colsum(F, F.Q, true, F.diag, nullptr);
   for (int o = threadIdx.x; o < F.O; o += kFitThreads) {
-    const double h = F.diag[o] + (o % F.Dp != F.D ? 1.0 : 0.0);
+    const double h = F.C * F.diag[o] + (o % F.Dp != F.D ? 1.0 : 0.0);
     F.diag[o] = h > 0.0 ? h : 1.0;
   }
   __syncthreads();
@@ -210,7 +217,8 @@ __device__ double precondition(const Fit& F) {
   return dot(F, F.res, F.zv);
 }
 
-// dir ~= -H^-1 grad by preconditioned conjugate gradient.
+// dir ~= -H^-1 grad by preconditioned conjugate gradient, at most kMaxCG steps.
+template <int kMaxCG>
 __device__ void newton_direction(const Fit& F, double gnorm, double gnorm0) {
   const double eta = fmin(0.5, sqrt(gnorm / gnorm0));
   for (int o = threadIdx.x; o < F.O; o += kFitThreads) {
@@ -221,7 +229,7 @@ __device__ void newton_direction(const Fit& F, double gnorm, double gnorm0) {
   double rz = precondition(F);
   for (int o = threadIdx.x; o < F.O; o += kFitThreads) F.pv[o] = F.zv[o];
   __syncthreads();
-  for (int j = 0; j < kFitMaxCG; ++j) {
+  for (int j = 0; j < kMaxCG; ++j) {
     if (sqrt(dot(F, F.res, F.res)) <= eta * gnorm) break;
     hess_vec(F, F.pv, F.hp);
     const double php = dot(F, F.pv, F.hp);
@@ -245,17 +253,19 @@ __device__ void newton_direction(const Fit& F, double gnorm, double gnorm0) {
   }
 }
 
-// One fit by the whole CTA: the minimiser for the nc classes of `labels` [num_train] on the first num_train rows of x
-// [rows][D], into coef [K][D + 1] (row r = (W_r, b_r) for the uncentred features, NaN beyond the R = nc (nc > 2), 1
-// (nc = 2) or 0 (nc = 1) model rows) and *iters (Newton steps, -1 if not converged, 0 for nc = 1).  ws holds
-// fit_workspace_doubles(num_train, D, K) doubles.  Every thread of the CTA calls it with the same arguments; it ends
-// with the coefficients visible to the whole CTA.
+// One fit by the whole CTA: the minimiser of C sum_i loss_i + 1/2 |W|^2 for the nc classes of `labels` [num_train]
+// on the first num_train rows of x [rows][D], multinomial over R = nc model rows when `multi`, else one binary model
+// (nc = 2, R = 1), into coef [K][D + 1] (row r = (W_r, b_r) for the uncentred features, NaN beyond the R rows; R = 0
+// for nc < 2) and *iters (Newton steps, -1 if kMaxNewton did not converge, 0 for nc < 2).  The existing fits call it
+// with C = 1 and multi = nc > 2.  ws holds fit_workspace_doubles(num_train, D, K) doubles.  Every thread of the CTA
+// calls it with the same arguments; it ends with the coefficients visible to the whole CTA.
+template <int kMaxNewton = kFitMaxNewton, int kMaxCG = kFitMaxCG>
 __device__ void logistic_fit_cta(const double* __restrict__ x, int D, int num_train, const int* __restrict__ labels,
-                                 int nc, int K, double* __restrict__ coef, int* __restrict__ iters,
-                                 double* __restrict__ ws) {
+                                 int nc, bool multi, double C, int K, double* __restrict__ coef,
+                                 int* __restrict__ iters, double* __restrict__ ws) {
   __shared__ double red[kFitWarps];
   const int t = threadIdx.x;
-  const int R = nc > 2 ? nc : (nc == 2 ? 1 : 0);
+  const int R = nc < 2 ? 0 : (multi ? nc : 1);
   const int Dp = D + 1;
   for (int o = t; o < K * Dp; o += kFitThreads) coef[o] = CUDART_NAN;
   if (R == 0) {
@@ -274,7 +284,8 @@ __device__ void logistic_fit_cta(const double* __restrict__ x, int D, int num_tr
     F.Dp = Dp;
     F.R = R;
     F.O = R * Dp;
-    F.multi = nc > 2;
+    F.multi = multi;
+    F.C = C;
     const int OK = K * Dp;                        // vectors are laid out for the largest R, so the layout is fixed
     F.part_stride = max(kFitThreads, OK);
     F.mean = ws;
@@ -322,7 +333,7 @@ __device__ void logistic_fit_cta(const double* __restrict__ x, int D, int num_tr
   gradient(F);
   const double gnorm0 = sqrt(dot(F, F.grad, F.grad));
   int steps = -1;
-  for (int it = 0; it <= kFitMaxNewton; ++it) {
+  for (int it = 0; it <= kMaxNewton; ++it) {
     double gmax = 0.0, smax = 0.0;
     for (int o = t; o < F.O; o += kFitThreads) {
       gmax = fmax(gmax, fabs(F.grad[o]));
@@ -334,9 +345,9 @@ __device__ void logistic_fit_cta(const double* __restrict__ x, int D, int num_tr
       steps = it;
       break;
     }
-    if (it == kFitMaxNewton) break;
+    if (it == kMaxNewton) break;
     hess_diag(F);
-    newton_direction(F, sqrt(dot(F, F.grad, F.grad)), gnorm0);
+    newton_direction<kMaxCG>(F, sqrt(dot(F, F.grad, F.grad)), gnorm0);
     const double slope = dot(F, F.grad, F.dir);
     if (!(slope < 0.0)) break;
     // A full step that promises less than kFitFlat |f| of decrease is below what f's rounding can rank: f's noise
@@ -362,7 +373,7 @@ __device__ void logistic_fit_cta(const double* __restrict__ x, int D, int num_tr
     gradient(F);
   }
 
-  // back to uncentred features: b_r = b'_r - W_r . m, then sum_r b_r = 0 for nc > 2
+  // back to uncentred features: b_r = b'_r - W_r . m, then sum_r b_r = 0 for a multinomial fit
   for (int r = t; r < R; r += kFitThreads) {
     const double* w = F.theta + (long long)r * Dp;
     double s = 0.0;

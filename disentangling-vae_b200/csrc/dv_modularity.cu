@@ -170,7 +170,8 @@ explicitness_fit_kernel(int D, int n, int m, const int* __restrict__ train_cls, 
   const int Dp = D + 1;
   const long long rows = (long long)n + m;
   double* ck = coef + (long long)k * S * Dp;
-  logistic_fit_cta(w.feat, D, n, train_cls + (long long)k * n, nc, S, ck, iters + k, w.fit + k * w.fit_stride);
+  logistic_fit_cta(w.feat, D, n, train_cls + (long long)k * n, nc, nc > 2, 1.0, S, ck, iters + k,
+                   w.fit + k * w.fit_stride);
 
   // probabilities: softmax of the decisions (classes added in order) for nc > 2; p_1 = 1 / (1 + exp(-z)) and
   // p_0 = 1 - p_1 for nc = 2 (sklearn's predict_proba); NaN for nc < 2 and beyond the factor's columns

@@ -81,6 +81,8 @@ SIGNATURES = {
     "dv_discrete_mutual_info": (I, [P, I, I, I, I, P, I, P, P, I, I, P, P, P]),
     "dv_explicitness_workspace_bytes": (SZ, [I, I, I, I, I]),
     "dv_explicitness_fit": (I, [P, I, I, I, I, P, I, P, I, P, P, P, I, I, P, P, P, P, P, P, P, SZ, P]),
+    "dv_downstream_workspace_bytes": (SZ, [I, I, I, I, I]),
+    "dv_downstream_logistic_cv": (I, [P, I, I, I, I, P, I, P, I, P, P, I, I, P, I, P, P, P, P, P, P, P, P, SZ, P]),
     "dv_irs_workspace_bytes": (SZ, [I, I, I]),
     "dv_irs_fit": (I, [P, I, I, I, I, P, I, P, I, DBL, P, P, P, P, P, P, P, SZ, P]),
     "dv_udr_workspace_bytes": (SZ, [I, I, I]),

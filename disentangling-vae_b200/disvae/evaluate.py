@@ -16,6 +16,7 @@ from functools import reduce
 from timeit import default_timer
 from typing import Callable, NamedTuple
 
+import numpy as np
 import torch
 from tqdm import tqdm
 
@@ -41,6 +42,13 @@ MODULARITY_MAX_DIM = 128                   # dv_explicitness_fit's limits: laten
 MODULARITY_MAX_TRAIN = 32768               # training rows,
 MODULARITY_MAX_CLASSES = 256               # and values of a scored factor
 MODULARITY_BINS = 20                       # disentanglement_lib's num_bins of the mutual information
+DOWNSTREAM_PREDICTORS = ("logistic_regression", "boosted_trees")
+DOWNSTREAM_MAX_DIM = 128                   # dv_downstream_logistic_cv's limits: latents,
+DOWNSTREAM_MIN_TRAIN = 5                   # training rows of a size (every fold holds one),
+DOWNSTREAM_MAX_TRAIN = 32768
+DOWNSTREAM_MAX_CLASSES = 256               # and values of a scored factor
+DOWNSTREAM_CS = np.logspace(-4, 4, 10)     # LogisticRegressionCV(Cs=10)'s grid, numpy's bits
+DOWNSTREAM_FOLDS = 5                       # KFold(n_splits=5)
 IRS_MAX_DIM = 1024                         # dv_irs_fit's limits: latents,
 IRS_MAX_TRAIN = 32768                      # and drawn rows (one latent's sort in shared memory)
 IRS_BINS = 20                              # disentanglement_lib's make_discretizer of the factors
@@ -811,6 +819,134 @@ def modularity_explicitness(mu, lat_sizes, num_train=10000, num_test=5000, seed=
     return score, helpers
 
 
+# ---- downstream task (Locatello et al. 2019, section 6; disentanglement_lib's downstream_task.py) ------------------
+def check_downstream_task(dataset, latent_dim, predictor="logistic_regression", num_train=(10, 100, 1000, 10000),
+                          num_test=5000):
+    """ValueError unless the downstream-task score can be computed over `dataset` for a `latent_dim` model with these
+    settings: the dataset has known factors (`lat_sizes`, `lat_names`), is their full grid and has a factor of more
+    than one value.  No GPU work.  Returns lat_sizes as a list of ints."""
+    return _check_downstream_grid(_dataset_lat_sizes("downstream task", dataset), len(dataset), latent_dim, predictor,
+                                  num_train, num_test)
+
+
+def _check_downstream_grid(lat_sizes, n, latent_dim, predictor, num_train, num_test):
+    lat_sizes = _full_grid("downstream task", lat_sizes, n)
+    if all(s == 1 for s in lat_sizes):
+        raise ValueError("downstream task: every factor of %s has one value; there is nothing to predict" % lat_sizes)
+    if predictor not in DOWNSTREAM_PREDICTORS:
+        raise ValueError("downstream task: predictor must be one of %s, got %r" % (DOWNSTREAM_PREDICTORS, predictor))
+    limit = DOWNSTREAM_MAX_CLASSES if predictor == "logistic_regression" else DCI_MAX_CLASSES
+    if max(lat_sizes) > limit:
+        raise ValueError("downstream task: a factor of %s has more than the kernel's limit of %d values"
+                         % (lat_sizes, limit))
+    limit = DOWNSTREAM_MAX_DIM if predictor == "logistic_regression" else DCI_MAX_DIM
+    if not 1 <= int(latent_dim) <= limit:
+        raise ValueError("downstream task: latent_dim must be in [1, %d] for the %s predictor, got %d"
+                         % (limit, predictor, int(latent_dim)))
+    sizes = [num_train] if isinstance(num_train, int) else list(num_train)
+    if not sizes:
+        raise ValueError("downstream task: num_train must name at least one training size")
+    for size in sizes:
+        if not DOWNSTREAM_MIN_TRAIN <= int(size) <= DOWNSTREAM_MAX_TRAIN:
+            raise ValueError("downstream task: every num_train must be in [%d, %d] (5 folds of at least one row), got "
+                             "%d" % (DOWNSTREAM_MIN_TRAIN, DOWNSTREAM_MAX_TRAIN, int(size)))
+    if int(num_test) < 1:
+        raise ValueError("downstream task: num_test must be at least 1, got %d" % int(num_test))
+    return lat_sizes
+
+
+def downstream_logistic_cv(mu, train_rows, test_rows, train_cls, n_classes, class_stride, Cs=DOWNSTREAM_CS,
+                           folds=False):
+    """`dv_downstream_logistic_cv` on `mu` [N, D] (any strides, a view of q_zCx included) and `sap_labels`' training
+    classes -> (fold_acc fp64 [K', 5, nC], chosen int32 [K'], coef fp64 [K', S, D + 1], pred int32 [K', num_train +
+    num_test], iters int32 [K', 5 nC + 1], fold_coef, fold_pred): LogisticRegressionCV(Cs, cv=KFold(5)) of every factor
+    on the raw latents.  With `folds`, fold_coef fp64 [K', 5, nC, S, D + 1] and fold_pred int32 [K', nC, num_train]
+    hold every fold fit and its predictions, else they are None.  See include/disvae_b200.h for the rules."""
+    mu_args, d = _mu_args(mu), mu.shape[1]
+    _require_operands("downstream_logistic_cv", train_rows=(train_rows, torch.int64),
+                      test_rows=(test_rows, torch.int64), train_cls=(train_cls, torch.int32),
+                      n_classes=(n_classes, torch.int32))
+    K, S = n_classes.numel(), int(class_stride)
+    Cs = np.ascontiguousarray(Cs, dtype=np.float64)
+    nC = Cs.size
+    num_train, num_test = train_rows.numel(), test_rows.numel()
+    nbytes = N.lib().dv_downstream_workspace_bytes(d, num_train, K, S, nC)
+    ws = _f64_workspace(nbytes, mu.device)
+    f64 = dict(dtype=torch.float64, device=mu.device)
+    i32 = dict(dtype=torch.int32, device=mu.device)
+    out = (torch.empty(K, DOWNSTREAM_FOLDS, nC, **f64), torch.empty(K, **i32), torch.empty(K, S, d + 1, **f64),
+           torch.empty(K, num_train + num_test, **i32), torch.empty(K, DOWNSTREAM_FOLDS * nC + 1, **i32))
+    fold = ((torch.empty(K, DOWNSTREAM_FOLDS, nC, S, d + 1, **f64), torch.empty(K, nC, num_train, **i32)) if folds
+            else (None, None))
+    N.call("dv_downstream_logistic_cv", *mu_args, N.ptr(train_rows), num_train, N.ptr(test_rows), num_test,
+           N.ptr(train_cls), N.ptr(n_classes), K, S, Cs.ctypes.data, nC, *(N.ptr(t) for t in out + fold), N.ptr(ws),
+           nbytes, N.stream())
+    return out + fold
+
+
+def downstream_task(mu, lat_sizes, predictor="logistic_regression", num_train=(10, 100, 1000, 10000), num_test=5000,
+                    seed=0):
+    """The downstream-task accuracies (Locatello et al. 2019, section 6) of the encoder means `mu` [N, D] (CUDA fp32,
+    dataset index order) of the full factor grid `lat_sizes`, as disentanglement_lib's downstream_task.py computes
+    them -> (score, helpers).  The draws come from a device torch.Generator seeded with `seed`: for each training size
+    in order, `torch.randint(N, (size,))` training rows, then `torch.randint(N, (num_test,))` test rows; the global
+    generators are not touched.  The classes are `sap_labels`' of each size's rows (a test value unseen in training is
+    never predicted right).  For every scored factor (those of more than one value, ascending; factor i of the keys is
+    the i-th of them) the predictor is fitted on the training rows and scored on both sets:
+    - "logistic_regression": LogisticRegressionCV(Cs=10, cv=KFold(5)) on the raw means by `downstream_logistic_cv`;
+      a factor seen with one value in training predicts it;
+    - "boosted_trees": GradientBoostingClassifier() by `dci_fit`.
+    score: for every size s, "{s}:mean_train_accuracy", "{s}:mean_test_accuracy", "{s}:min_train_accuracy",
+    "{s}:min_test_accuracy" and "{s}:train_accuracy_factor_{i}", "{s}:test_accuracy_factor_{i}".
+    helpers: "factors" int64 [K'] (the scored factor indices, ascending), "predictor", and per size s, helpers[s]:
+    "classes" int64 [K', S] (each factor's training values, ascending, -1 beyond), "train_accuracy" and
+    "test_accuracy" fp64 [K']; for the logistic predictor also "Cs" fp64 [10], "fold_accuracy" fp64 [K', 5, 10],
+    "chosen_C" fp64 [K'], "coef" fp64 [K', S, D] and "intercept" fp64 [K', S] (the refit's model rows, NaN beyond),
+    "solver_iterations" int32 [K', 51] (the fold fits' Newton steps, fold-major, then the refit's; -1 for a fit that
+    did not converge, which also raises a RuntimeWarning)."""
+    lat_sizes = _check_downstream_grid(lat_sizes, mu.shape[0], mu.shape[1], predictor, num_train, num_test)
+    N.require_cuda_f32(mu)
+    sizes = [int(num_train)] if isinstance(num_train, int) else [int(s) for s in num_train]
+    gen = torch.Generator(device=mu.device)
+    gen.manual_seed(int(seed))
+    score, helpers = {}, {"predictor": predictor}
+    failed = 0
+    for size in sizes:
+        train_rows = torch.randint(mu.shape[0], (size,), generator=gen, device=mu.device)
+        test_rows = torch.randint(mu.shape[0], (int(num_test),), generator=gen, device=mu.device)
+        factors, train_cls, test_cls, n_classes, counts, present = sap_labels(lat_sizes, train_rows, test_rows)
+        S = counts.shape[1]
+        h = {}
+        if predictor == "boosted_trees":
+            _, pred, _ = dci_fit(mu, train_rows, test_rows, train_cls, n_classes, counts)
+        else:
+            fold_acc, chosen, coef, pred, iters, _, _ = downstream_logistic_cv(mu, train_rows, test_rows, train_cls,
+                                                                               n_classes, S)
+            coef, iters, chosen = coef.cpu(), iters.cpu(), chosen.cpu().long()
+            failed += int((iters < 0).sum())
+            h.update({"Cs": torch.from_numpy(DOWNSTREAM_CS.copy()), "fold_accuracy": fold_acc.cpu(),
+                      "chosen_C": torch.from_numpy(DOWNSTREAM_CS.copy())[chosen], "coef": coef[..., :-1].clone(),
+                      "intercept": coef[..., -1].clone(), "solver_iterations": iters})
+        right = pred == torch.cat([train_cls, test_cls], 1)
+        train_acc = right[:, :size].double().mean(1).cpu()
+        test_acc = right[:, size:].double().mean(1).cpu()
+        h.update({"classes": _classes_table(present.cpu()), "train_accuracy": train_acc, "test_accuracy": test_acc})
+        helpers[size] = h
+        helpers["factors"] = torch.tensor(factors, dtype=torch.int64)
+        s = str(size)
+        score[s + ":mean_train_accuracy"] = float(train_acc.mean())
+        score[s + ":mean_test_accuracy"] = float(test_acc.mean())
+        score[s + ":min_train_accuracy"] = float(train_acc.min())
+        score[s + ":min_test_accuracy"] = float(test_acc.min())
+        for i in range(len(factors)):
+            score[s + ":train_accuracy_factor_%d" % i] = float(train_acc[i])
+            score[s + ":test_accuracy_factor_%d" % i] = float(test_acc[i])
+    if failed:
+        warnings.warn("downstream task: %d of the logistic-regression fits did not converge in the solver's step "
+                      "limit; see helpers[size]['solver_iterations'] (-1)" % failed, RuntimeWarning)
+    return score, helpers
+
+
 # ---- IRS (Suter et al. 2019; disentanglement_lib's irs.py) -------------------------------------------------------
 def check_irs_score(dataset, latent_dim, num_train=10000, diff_quantile=0.99):
     """ValueError unless IRS can be computed over `dataset` for a `latent_dim` model with these settings: the dataset
@@ -1349,6 +1485,17 @@ class Evaluator:
         members with `Evaluator(member.model, ...).compute_modularity_explicitness(sweep.loader.in_order(1000),
         seed=...)`."""
         return self._score(check_modularity_explicitness, modularity_explicitness, dataloader, seed,
+                           num_train=num_train, num_test=num_test)
+
+    def compute_downstream_task(self, dataloader, predictor="logistic_regression", num_train=(10, 100, 1000, 10000),
+                                num_test=5000, seed=0):
+        """The downstream-task accuracies (Locatello et al. 2019, section 6) of the model's encoder means over
+        `dataloader` (the dataset in index order: DataLoader(shuffle=False) or DeviceLoader.in_order) with the
+        "logistic_regression" or "boosted_trees" predictor -> {"{size}:mean_train_accuracy", ...}; see
+        `downstream_task` for the definition and the order of the draws.  The Evaluator's __call__, training and sweeps
+        do not write this score; score a sweep's members with `Evaluator(member.model, None,
+        device=...).compute_downstream_task(sweep.loader.in_order(1000), seed=...)`."""
+        return self._score(check_downstream_task, downstream_task, dataloader, seed, predictor=predictor,
                            num_train=num_train, num_test=num_test)
 
     def compute_irs_score(self, dataloader, num_train=10000, diff_quantile=0.99, seed=0):

@@ -543,6 +543,57 @@ int dv_explicitness_fit(const float* mu, int ld, int row_stride, int N, int D, c
                         double* auc, int* iters, double* mean, double* std, double* proba, void* workspace,
                         size_t workspace_bytes, void* stream);
 
+/* ---- disentanglement metrics: downstream task (Locatello et al. 2019, section 6; downstream_task.py) --------------
+ * dv_downstream_logistic_cv: for every scored factor k < K, sklearn's LogisticRegressionCV(Cs, cv=KFold(5)) on the raw
+ * latents: a fit per fold and C, the C of the best summed fold accuracy, the refit at that C on every training row,
+ * and the predicted class of every training and test row.
+ * Inputs: mu is read as dv_group_variance reads it (element (n, d) at n*row_stride + d*ld; q_zCx in place), finite
+ * values assumed; x_i = the fp32 means of row i in fp64.  train_rows int64 [num_train] and test_rows int64 [num_test],
+ * every entry in [0, N) (not checked).  train_cls int32 [K][num_train] (classes 0 .. nc-1, every class present) and
+ * n_classes int32 [K] (nc, clamped to [0, class_stride]), as dv_sap_score_matrix takes them.  Cs fp64 [nC] in host
+ * memory, each finite and positive; the values travel in the launches' parameters, so a captured graph keeps them.
+ *   fit at C over a set of rows: the exact minimiser of C sum_i loss_i + 1/2 |W|_F^2, the intercepts unpenalised, by
+ *         dv_logistic_fit's solver, rules and convergence test (at most 300 Newton steps of at most 500 conjugate-
+ *         gradient steps): multinomial over the p classes the rows have when nc > 2 (even for p = 2, which is not the
+ *         binary model: it equals a binary fit at 2C), one binary model when nc = 2 and both classes are present, no
+ *         fit when p < 2.  Classes the rows lack are the limit of sklearn's objective, whose intercepts go to -inf:
+ *         they are never predicted.
+ *   folds: KFold without shuffling: fold f is the contiguous training rows [s_f, s_f + n/5 + [f < n % 5]) in draw
+ *         order.  Fit (k, f, c) is the fit at Cs[c] over the other training rows; it predicts the fold's rows (the
+ *         argmax over its present classes, the lowest on a tie; class 1 iff w.x + b > 0 when binary; the one present
+ *         class when p = 1), and fold_acc = right / fold rows in fp64.
+ *   choice: for each c, fold_acc[k][0][c] + ... + fold_acc[k][4][c] added in fold order; the first maximum.
+ *   refit: the fit at the chosen C over every training row (nc classes), and the prediction of every row by the same
+ *         rule (0 for nc < 2).
+ * Outputs:
+ *   fold_acc  fp64 [K][5][nC]
+ *   chosen    int32 [K]: the index of the chosen C
+ *   coef      fp64 [K][class_stride][D + 1]: the refit's rows (W_r, b_r) (as dv_logistic_fit's coef, one row when
+ *             binary, sum_r b_r = 0 when multinomial), NaN beyond its model rows
+ *   pred      int32 [K][num_train + num_test]: the refit's class of every training row, then of every test row
+ *   iters     int32 [K][5 nC + 1]: the Newton steps of fit (f, c) at f nC + c, the refit's last; -1 for a fit that did
+ *             not converge, 0 where there is no fit
+ *   fold_coef fp64 [K][5][nC][class_stride][D + 1] (optional, NULL for none): each fold fit's rows, row v for class v
+ *             (NaN for a class the fold lacks and beyond the model rows; one row, class 0's, when binary)
+ *   fold_pred int32 [K][nC][num_train] (optional, NULL for none): each training row's class predicted by the fit of
+ *             its fold at each C
+ * workspace: dv_downstream_workspace_bytes(D, num_train, K, class_stride, nC) bytes, 8-byte aligned, contents
+ * irrelevant: a slot per resident CTA (at most 132, at most 5 K nC, within 8 GiB, at least one), each holding one fit
+ * of num_train rows.  Two launches (the fold fits, then one CTA per factor that chooses C, refits and predicts), each
+ * a grid of slots walking its fits in a fixed order; no host synchronisation, graph-capturable.  Deterministic
+ * (fixed-order reductions, no floating-point atomics), and independent of the slot count.
+ * DV_ERR_BAD_SHAPE: N < 1, D < 1, D > 128, num_train < 5, num_train > 32768, num_test < 1, K < 1, class_stride < 1,
+ * class_stride > 256, nC < 1, nC > 32, ld < 1, row_stride < 1, or num_train + num_test or 5 K nC above INT_MAX.
+ * DV_ERR_BAD_ARG: a required pointer NULL (all but fold_coef and fold_pred), a C not finite and positive, or a pointer
+ * misaligned (rows, fold_acc, coef, fold_coef and workspace 8 bytes, the others 4).
+ * DV_ERR_WORKSPACE: workspace NULL or smaller than the query. */
+size_t dv_downstream_workspace_bytes(int D, int num_train, int K, int class_stride, int nC);  /* 0: unsupported */
+int dv_downstream_logistic_cv(const float* mu, int ld, int row_stride, int N, int D, const long long* train_rows,
+                              int num_train, const long long* test_rows, int num_test, const int* train_cls,
+                              const int* n_classes, int K, int class_stride, const double* Cs, int nC,
+                              double* fold_acc, int* chosen, double* coef, int* pred, int* iters, double* fold_coef,
+                              int* fold_pred, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- disentanglement metrics: IRS (Suter et al. 2019; disentanglement_lib's irs.py) ------------------------------
  * dv_irs_fit: the interventional robustness score's tables of n drawn rows over K scored factors.
  *   mu is read as dv_group_variance reads it (element (p, d) at p*row_stride + d*ld; q_zCx in place), finite values
